@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""bench.py — measurement-update throughput of the B200 engine (and, with --impl reference, of the
+"""bench.py — measurement-update throughput of the CUDA engine on an H100 (and, with --impl reference, of the
 reference's own CPU path) on BASELINE.json's configs.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload c2] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload c2] [--impl b200|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 One "step" = one measurement update (the hot path) over one batch: every particle x every sampled
-scan point.  Prints ONE JSON line on rank 0 (see the contract in the task statement):
+scan point.  Every timed loop runs exactly K steps.  Prints ONE JSON line on rank 0:
   value     whole-job particle x point evals/s with all inputs resident in HBM (CUDA events, max over ranks).
             N > 1: one process per GPU, particles sharded, map replicated; the ONE exchange of the path (the gather
             of the 24-byte records) is folded into the measurement kernels, which store every record into every
@@ -20,12 +20,16 @@ scan point.  Prints ONE JSON line on rank 0 (see the contract in the task statem
             arrays page-locked via mcl3dl_host_alloc, scans in ordinary memory; L2 flushed before every call).
             N > 1: ONE host process (rank 0) drives all N GPUs through the in-process multi-device engine
             (mcl3dl_create with N device ids) and receives every record in one host array — what a ROS node would do.
-  roofline  dominant kernel: algorithmic bytes / CUDA-event duration vs MEASURED_PEAKS.json hbm_gbs
+  roofline  dominant kernel: algorithmic bytes / CUDA-event duration vs MEASURED_PEAKS.json hbm_gbs (else the H100 SXM
+            data-sheet HBM3 bandwidth, 3.35 TB/s)
   cpu_baseline  the reference CPU path (oracle/_ref if present, else the port) on a bounded sample, 1 thread
-  workloads driver-run secondaries: c3 (beam DDA), c3_kd (the node's default raycaster), c5 (65 536 spread particles,
+  workloads secondaries of the c2 run: c3 (beam DDA), c3_kd (the node's default raycaster), c5 (65 536 spread particles,
             strong scaling at N > 1), each with value / kernel times / counted roofline
 Workloads (BASELINE.json configs): c1 64x(96+3)/50k map, c2 1024x512 likelihood/1M map (default, the
 metric's config), c3 4096x256 beam DDA/1M map, c4 16384x1024 lik+beam/10M map, c5 65536 spread lik+beam.
+--dump-outputs DIR: the records of the last timed step of the primary workload (what mcl3dl_measure_device hands its
+caller; all ranks' records at N > 1), one DIR/<field>.npy per record field (float32 scores, float64 counts).  The inputs
+are seeded: the same arguments give the same inputs on every run.
 """
 import argparse
 import functools
@@ -84,11 +88,11 @@ def peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured"
     except Exception:
-        return 6650.0, "fallback"
+        return 3350.0, "H100 SXM data sheet"
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons during the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -313,6 +317,20 @@ class Ctx:
     pass
 
 
+class _DevView:
+    """Raw device memory as a torch tensor (CUDA array interface)."""
+    def __init__(self, ptr, nbytes):
+        self.__cuda_array_interface__ = {"shape": (nbytes,), "typestr": "|u1", "data": (ptr, False), "version": 3}
+
+
+def dump_outputs(path, records):
+    """One <field>.npy per record field: float32 scores, float64 counts (exact)."""
+    os.makedirs(path, exist_ok=True)
+    for f in records.dtype.names:
+        dt = np.float32 if records.dtype[f].kind == "f" else np.float64
+        np.save(os.path.join(path, f + ".npy"), records[f].astype(dt))
+
+
 def device_leg(cx, workload, raycaster, steps, warmup, exchange="peer", graph=True, keep_spinning=False, field=False):
     """Device-resident leg of one workload on every rank: value (CUDA events, max over ranks), per-model kernel
     times, counted roofline.  Returns (result dict, live objects for the e2e leg)."""
@@ -435,10 +453,21 @@ def device_leg(cx, workload, raycaster, steps, warmup, exchange="peer", graph=Tr
             dist.all_reduce(t, op=dist.ReduceOp.MAX)
         return float(t.item()), per
 
+    def last_records():
+        """The records the last step handed its caller (untimed; all ranks' records with the folded exchange)."""
+        torch.cuda.synchronize()
+        if peer:
+            ptr, _ = eng.exchange_current(torch.cuda.current_stream().cuda_stream)
+            out = torch.as_tensor(_DevView(ptr, world * P_rank * 24), device=dev)
+        else:
+            out = d_all if world > 1 else d_out
+        return np.frombuffer(out.cpu().numpy().tobytes(), dtype=synth.RESULT).copy()
+
     for _ in range(warmup):
         step()
     barrier()
     total_ms, per_step = timed(step, steps)
+    records = {"flush": last_records()}
     if keep_spinning:
         # the timed region lasts a few milliseconds, shorter than one nvidia-smi period: keep the same step running
         # (untimed, same count on every rank) for ~0.5 s so that the clock record holds samples taken under this load
@@ -448,8 +477,8 @@ def device_leg(cx, workload, raycaster, steps, warmup, exchange="peer", graph=Tr
 
     # ---- the back-to-back protocol: ALL `steps` steps in one CUDA graph, one event pair around the replay, consecutive
     # steps on different input sets ("inputs larger than L2" instead of a flush before every step).  A pair of events
-    # around one launch costs ~5 us on this system and a graph launch ~3 us (profiles/r02z_cold.txt): per-step event
-    # pairs add that to every step, which is most of a 20 us step and none of the kernel's work.
+    # around one launch and a graph launch each cost microseconds: per-step event pairs add that to every step, which is
+    # a large share of a step of a few tens of microseconds and none of the kernel's work.
     b2b = None
     if graph and graphed:
         n_st = 4 if spread else 32
@@ -502,6 +531,7 @@ def device_leg(cx, workload, raycaster, steps, warmup, exchange="peer", graph=Tr
                 g_rot.replay()
             barrier()
             official = replay_ms(g_rot)                       # the timed region: exactly `steps` steps
+            records["rotate"] = last_records()
             repeats = [replay_ms(g_rot) for _ in range(4)]
             g_same = capture(lambda i: 0)                     # comparison: every step on the same inputs (L2-warm)
             g_same.replay()
@@ -526,9 +556,6 @@ def device_leg(cx, workload, raycaster, steps, warmup, exchange="peer", graph=Tr
                          "graph": graphed, "bytes_per_rank_per_step": P_rank * 24 * (world if peer else 1)}
         if peer:
             # the folded exchange against NCCL on the same inputs (outside every timed region), byte for byte
-            class _DevView:  # raw device memory as a torch tensor (CUDA array interface)
-                def __init__(self, ptr, nbytes):
-                    self.__cuda_array_interface__ = {"shape": (nbytes,), "typestr": "|u1", "data": (ptr, False), "version": 3}
             st = torch.cuda.current_stream().cuda_stream
             plain_measure(st)
             sharding.gather_records_device(d_out, d_all)
@@ -550,7 +577,7 @@ def device_leg(cx, workload, raycaster, steps, warmup, exchange="peer", graph=Tr
     res = {"value": evals_step / (ms_per_step * 1e-3), "ms_per_step": ms_per_step, "scaling": scaling,
            "graph": graphed, "launches_per_step": int(launches_per_step), "l2": l2_used,
            "flushed_step_ms_min_med_max": [float(np.min(per_step)), float(np.median(per_step)), float(np.max(per_step))],
-           "back_to_back": b2b, "exchange": exchange_info}
+           "back_to_back": b2b, "exchange": exchange_info, "records": records[l2_used]}
     if field_info:
         res["field_mode"] = field_info
 
@@ -604,23 +631,8 @@ def device_leg(cx, workload, raycaster, steps, warmup, exchange="peer", graph=Tr
                         + io_bytes + n_beam * 16)
         survey_note = "SURVEY 8d beam: 1 B per cell stepped + 8 B CSR + 16 B per point tested"
     achieved = alg_bytes / (kern[dom] * 1e-3) / 1e9
-    traffic, traffic_src, binding = None, None, None
-    try:
-        with open(os.path.join(ROOT, "profiles", "ncu_summary.json")) as f:
-            ncu = json.load(f)
-        key = (workload + ("" if raycaster == "dda" or not n_beam else "_kd") + ("_spread" if FORCE_SPREAD else "")
-               + ("_field" if field else ""))
-        ent = ncu.get(key, {})
-        traffic = ent.get(dom + "_dram_bytes_per_launch")
-        traffic_src = ent.get(dom + "_source")
-        binding = ent.get(dom + "_binding_resource")
-    except Exception:
-        pass
     res["roofline"] = {"bound": "hbm", "kernel": dom + "_kernel", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                       "frac": achieved / peak, "peak_source": peak_src, "traffic": traffic, "traffic_source": traffic_src,
-                       "binding_resource_ncu": binding,
-                       "dram_frac": (traffic / (kern[dom] * 1e-3) / 1e9 / peak) if traffic else None,
-                       "kernel_ms": kern[dom], "kernel_ms_source": kern_src, "algorithmic_bytes_per_launch": alg_bytes,
+                       "frac": achieved / peak, "peak_source": peak_src, "kernel_ms": kern[dom], "kernel_ms_source": kern_src, "algorithmic_bytes_per_launch": alg_bytes,
                        "model": note,
                        "kernel_ms_all": kern, "work_counters_per_step": ws,
                        "survey_8d_model": {"bytes_per_launch": survey_bytes,
@@ -831,6 +843,7 @@ def main():
     ap.add_argument("--raycaster", default="dda", choices=["dda", "kd"],
                     help="beam raycaster: RaycastUsingDDA (north_star) or RaycastUsingKDTree (the node's default)")
     ap.add_argument("--spread", action="store_true", help="spread (global-localisation style) particles: the HBM-bound variant")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the records of the last timed step as DIR/<field>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     global FORCE_SPREAD, USE_DDA, L2_MODE
@@ -851,7 +864,7 @@ def main():
     cx.notes = []
     if cx.world > 1:
         os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
-        # NCCL_DEBUG is left as the launcher set it (the driver reads the communicator's rank count from NCCL's own log)
+        # NCCL_DEBUG is left as the launcher set it
         dist.init_process_group("nccl", device_id=torch.device("cuda", cx.local))
         # host-side waits (a rank that idles while rank 0 drives every GPU must not park an NCCL kernel on its device)
         cx.cpu_group = dist.new_group(backend="gloo")
@@ -867,6 +880,9 @@ def main():
         clocks.start()
     graph = not args.no_graph
     res, live = device_leg(cx, args.workload, args.raycaster, args.steps, args.warmup, args.exchange, graph, keep_spinning=True)
+    records = res.pop("records")
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, records)
     e2e = e2e_leg(cx, args.workload, args.raycaster, args.steps, live)
     clk = clocks.stop() if rank == 0 else None
     n_lik, n_beam, P_rank, s = live["n_lik"], live["n_beam"], live["P_rank"], live["scene"]
@@ -899,15 +915,16 @@ def main():
     out_host = live.get("out_host")
     del live
 
-    # ---- driver-run secondaries (fewer steps; no CPU leg): what north_star names besides the primary metric
+    # ---- secondaries (no CPU leg): what north_star names besides the primary metric
     secondaries = {}
     if not args.no_secondaries and args.workload == "c2" and not args.spread:
         sec = ([("c5", "c5", "dda")] if world > 1 else
                [("c3", "c3", "dda"), ("c3_kd", "c3", "kd"), ("c5", "c5", "dda"), ("c5_field", "c5", "dda")])
-        k = max(10, min(args.steps, 30))
+        k = args.steps
         for name, wl, caster in sec:
             try:
                 r2, live2 = device_leg(cx, wl, caster, k, 3, args.exchange, graph, field=name.endswith("_field"))
+                del r2["records"]
                 r2["metric"] = metric_name(live2["n_lik"])
                 r2["unit"] = "evals/s"
                 r2["steps"] = k
@@ -923,7 +940,7 @@ def main():
                 secondaries[name] = {"error": "%s: %s" % (type(exc).__name__, exc)}
         if world == 1:
             try:
-                secondaries["c5_resident"] = resident_leg(cx, "c5", max(10, min(args.steps, 30)))
+                secondaries["c5_resident"] = resident_leg(cx, "c5", args.steps)
             except Exception as exc:
                 secondaries["c5_resident"] = {"error": "%s: %s" % (type(exc).__name__, exc)}
         USE_DDA = args.raycaster == "dda"

@@ -1,5 +1,5 @@
 /*
- * mcl3dl_b200.h — C ABI of the B200-native measurement-update engine for mcl_3dl.
+ * mcl3dl_b200.h — C ABI of the CUDA measurement-update engine for mcl_3dl (sm_90a, H100).
  *
  * This is the drop-in boundary: plain C, plain pointers and sizes, no STL, no torch
  * types, no exceptions.  Every entry point names the reference interface it replaces
@@ -31,7 +31,7 @@ enum
   MCL3DL_ERR_INVALID_ARG = -1,  /* null pointer / bad size / label out of origins range */
   MCL3DL_ERR_NO_MAP = -2,       /* measure() before set_map() */
   MCL3DL_ERR_CUDA = -3,         /* a CUDA runtime call failed; see mcl3dl_last_error_detail */
-  MCL3DL_ERR_NO_DEVICE = -4,    /* no usable sm_100 device */
+  MCL3DL_ERR_NO_DEVICE = -4,    /* no usable sm_90 (H100) device */
   MCL3DL_ERR_TOO_LARGE = -5,    /* grid would exceed 2^31-1 cells (int point_total, raycast_using_dda.h:176) */
   MCL3DL_ERR_RADIUS = -6        /* match_dist_min > chunk length semantics (chunked_kdtree.h:224-225) */
 };
@@ -230,7 +230,7 @@ void mcl3dl_beam_params_from_reference(mcl3dl_beam_params* out,
 int mcl3dl_get_map_info(const mcl3dl_engine*, mcl3dl_map_info* out);
 
 /* ---- Resident particle set (SURVEY.md §8 row f3; the per-particle arithmetic is verified on the host bit for bit
- * against the oracle, the kernels by tests/test_gpu_resident.py on a B200).
+ * against the oracle, the kernels by tests/test_gpu_resident.py on an H100).
  * The particles of pf::ParticleFilter<State6DOF> stay in device memory between updates, so an update moves only the
  * scans and the odometry in and a summary out.  Engines with exactly one device.
  *
@@ -381,8 +381,8 @@ int mcl3dl_collect_stats(mcl3dl_engine*, int enable);
 int mcl3dl_read_stats(mcl3dl_engine*, mcl3dl_work_stats* out);
 
 /* Device times of the last mcl3dl_measure call (CUDA events on the engine's stream, max over
- * devices): host->device copies, the two kernels, device->host copy.  The events cost ~28 us per update
- * (measured, profiles/r01y_ab_variants.txt), so they are only recorded after mcl3dl_collect_timing(eng, 1)
+ * devices): host->device copies, the two kernels, device->host copy.  The events cost tens of
+ * microseconds per update, so they are only recorded after mcl3dl_collect_timing(eng, 1)
  * (or with MCL3DL_TIMING=1 in the environment); otherwise the four values read 0. */
 int mcl3dl_collect_timing(mcl3dl_engine*, int enable);
 int mcl3dl_last_timing(const mcl3dl_engine*, double* h2d_ms, double* lik_kernel_ms, double* beam_kernel_ms,

@@ -12,8 +12,7 @@
 #include "device_math.cuh"
 
 // MCL3DL_NEAR_BITS=1 (default) compiles the near-field screens below into the searches; -DMCL3DL_NEAR_BITS=0 builds
-// the kernels without them (A/B: profiles/r01y_ab_variants.txt — results byte-identical, likelihood kernel -6 %,
-// KD-tree raycaster -16 %).
+// the kernels without them.
 #ifndef MCL3DL_NEAR_BITS
 #define MCL3DL_NEAR_BITS 1
 #endif
@@ -297,8 +296,8 @@ __device__ __forceinline__ int dda_to_index(float v, float mn, double grid)
 
 // One ray: RaycastUsingDDA::setRay + getNextCastResult loop + getBeamStatus's decision.
 //
-// Measured choices (profiles/r01g_variants.txt, r01h_variants.txt; all variants bit-exact):
-//   * the axis choice is evaluated branch-free (selects): 200 -> 177 us on c3, the 3-way branch
+// Measured choices:
+//   * the axis choice is evaluated branch-free (selects): the 3-way branch
 //     diverges whenever the lanes of a warp cross different faces;
 //   * t_max needs float(|index - begin|): kept as a float counter (+1.0f per step) instead of an
 //     int->float conversion per step;
@@ -306,13 +305,13 @@ __device__ __forceinline__ int dda_to_index(float v, float mn, double grid)
 //   * replacing the twelve fp64 divisions of the set-up by guarded reciprocal multiplications, caching
 //     the per-sensor ray origin, or screening the cone test in float changed nothing measurable
 //     (the kernel is latency/occupancy bound, not fp64 bound) and were dropped again;
-//   * occupancy matters most: __launch_bounds__(256, 4) (<= 64 registers) 200 -> 165 us.
+//   * occupancy matters most: __launch_bounds__(256, 4) (<= 64 registers).
 //
 // The ray is cut into three pieces: dda_setup (setRay), dda_advance (getNextCastResult up to the next occupied cell: a
 // tight stepping loop with nothing else in it) and dda_test_cell (hasIntersection + getBeamStatus, fp64).  With the cone
-// test inside the stepping loop it executed with 2-3 live lanes and took a quarter of the samples
-// (profiles/r02a_ncu_beam_c3.txt); as a loop of "advance, then test" the lanes of a warp reconverge after the walk and
-// test together: c3 155 -> 117 us (profiles/r02i_*), same operations per lane, same bits.
+// test inside the stepping loop it executed with 2-3 live lanes and took a large share of the samples;
+// as a loop of "advance, then test" the lanes of a warp reconverge after the walk and test together: same operations
+// per lane, same bits.
 struct DdaRay
 {
   F3 b, e, dir;
@@ -580,10 +579,8 @@ __device__ __forceinline__ int nnf_lookup(const NnFieldDev& f, float qx, float q
 
 // A voxel's candidate list is walked 16 bytes at a time, one 32-byte sector per two records and every new sector a fresh
 // L2 / DRAM latency when the list is cold.  Ask for the sectors behind the first one as soon as the directory entry is
-// decoded (no registers held; lists of up to 7-8 records are covered).  c2 15.0 -> 13.3 us, c5 likelihood kernel
-// 137 -> 108 us (profiles/r02ac_summary.txt).  MCL3DL_NF_PREFETCH: 0 off, 1 prefetch.global.L1, 2 prefetch.global.L2.
-// (The KD caster's marching search gains nothing from it: c3_kd 234 -> 239 us, profiles/r02ad_summary.txt; neither do a
-// deeper list prefetch or a prefetch of the next trip's poses: profiles/r02af_summary.txt.)
+// decoded (no registers held; lists of up to 7-8 records are covered).
+// MCL3DL_NF_PREFETCH: 0 off, 1 prefetch.global.L1, 2 prefetch.global.L2.
 #ifndef MCL3DL_NF_PREFETCH
 #define MCL3DL_NF_PREFETCH 2
 #endif

@@ -344,7 +344,7 @@ struct DeviceCtx
 {
   int dev = 0;
   cudaStream_t stream = nullptr;
-  int sm_count = 148;
+  int sm_count = 132;
   // map
   DevBuf nn_cell_start, nn_pts, nn_row3, dda_occ, dda_cell_start, dda_pts;
   NnGridDev nn{};
@@ -419,8 +419,8 @@ struct mcl3dl_engine
   size_t near_max_bytes = size_t(256) << 20;  // MCL3DL_NEAR_MAX_MB
   int near_info_k[2] = {0, 0};
   uint64_t near_info_bytes[2] = {0, 0};
-  // Host-path choices measured in profiles/r01y_ab_variants.txt (c2 e2e 102 -> 71 us per update with both):
-  int timing = 0;               // the per-call timing events of mcl3dl_last_timing cost ~28 us per update: off unless
+  // Host-path choices:
+  int timing = 0;               // the per-call timing events of mcl3dl_last_timing cost tens of us per update: off unless
                                 // mcl3dl_collect_timing(eng, 1) or MCL3DL_TIMING=1
   size_t zero_copy_max = 8192;  // the kernels of updates with <= this many particles per device store their records
                                 // straight into the pinned result block (no D2H copy launch); MCL3DL_ZEROCOPY_OUT
@@ -429,8 +429,7 @@ struct mcl3dl_engine
                             // round 1: off until the f2 parity tests have run with it)
   int field_mode = 0;  // 1: the likelihood model reads the trilinear distance volume (opt-in, inexact; MCL3DL_LIK_MODE=field)
   size_t field_max_bytes = size_t(24) << 30;  // MCL3DL_FIELD_MAX_MB
-  int beam_dq = 2;  // beam kernel: 2 = by job size (dynamic queue from 262 144 rays up: c3 118 -> 107 us, c3_kd 266 -> 232 us,
-                    // profiles/r02r_ab.jsonl; the static kernel is faster on small jobs, profiles/r02s_c5e.txt), 1 = MCL3DL_BEAM=dq, 0 = MCL3DL_BEAM=pl
+  int beam_dq = 2;  // beam kernel: 2 = by job size, 1 = MCL3DL_BEAM=dq, 0 = MCL3DL_BEAM=pl
   int beam_dq_ppl = 0;  // MCL3DL_BEAM_DQ_PPL: rays per item (0 = chosen from the job size)
   int lik_share = 4;  // CTA slots per SM the likelihood kernel takes while the beam kernel runs next to it (MCL3DL_LIK_SHARE)
   int nnf_kd_r2 = 1;  // MCL3DL_NNF_KD_R2=0: the NN field also covers the KD-tree raycaster's second search radius
@@ -442,8 +441,7 @@ struct mcl3dl_engine
   // DMA-ed (or, small updates, written by the kernels) in place instead of going through the engine's staging block
   std::vector<std::pair<char*, size_t>> host_blocks;
   size_t direct_min_bytes = size_t(64) << 10;  // smaller pose arrays ride in the staging block's single copy: a second DMA
-                                               // operation costs more than their memcpy (c2, 32 KB: 36.6 vs 40.7 us;
-                                               // c3, 128 KB: 130 -> 126 us; profiles/r02ae_summary.txt); MCL3DL_DIRECT_MIN_KB
+                                               // operation costs more than their memcpy; MCL3DL_DIRECT_MIN_KB
 };
 
 static bool in_host_block(const mcl3dl_engine* eng, const void* p, size_t bytes)
@@ -776,8 +774,7 @@ int launch_lik_field(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_pose* poses,
 PlShape pick_pl_shape(size_t P, size_t N, int sm_count)
 {
   // Every warp walks `ppl` consecutive scan points for 32 particles.  The kernels hold 4 CTAs = 32 warps per SM
-  // (64 registers), and a grid slightly larger than the resident slots runs a mostly empty second wave (c3 and c5 both
-  // sat at 1.73 waves, profiles/r02a_ncu_beam_c*.txt): size the chunks so that the whole grid is resident at once when
+  // (64 registers), and a grid slightly larger than the resident slots runs a mostly empty second wave: size the chunks so that the whole grid is resident at once when
   // the job allows it, and otherwise make it many waves deep.
   const size_t groups = (P + 31) / 32;
   const size_t slots = static_cast<size_t>(sm_count) * 4;  // resident CTAs
@@ -1518,9 +1515,9 @@ int mcl3dl_create(mcl3dl_engine** out, const int* device_ids, int n_devices)
     }
     cudaDeviceProp prop;
     if (cudaSetDevice(c.dev) != cudaSuccess || cudaGetDeviceProperties(&prop, c.dev) != cudaSuccess ||
-        prop.major < 10)
+        prop.major != 9 || prop.minor != 0)
     {
-      mcl3dl_destroy(eng);  // built for sm_100a only; anything else cannot run these kernels
+      mcl3dl_destroy(eng);  // built for sm_90a only; anything else cannot run these kernels
       return MCL3DL_ERR_NO_DEVICE;
     }
     c.sm_count = prop.multiProcessorCount;
@@ -2518,7 +2515,6 @@ static int measure_host(mcl3dl_engine* eng, const mcl3dl_pose* poses, size_t P, 
     // into the unified address space), which saves the D2H copy launch; large ones keep the bulk copy
     const bool zc = !status && Pd <= eng->zero_copy_max;  // (per-ray status bytes would be scattered 1-byte PCIe writes)
     if (timed) CK(cudaEventRecord(c.ev[0], st));
-    // (an SM copy kernel reading the mapped block instead of the copy engine measured the same: profiles/r02p_e2e.txt)
     if (poses_direct)
     {
       CK(cudaMemcpyAsync(c.d_poses.p, poses + p0[d], b_poses, cudaMemcpyHostToDevice, st));

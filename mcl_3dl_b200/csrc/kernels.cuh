@@ -1,4 +1,4 @@
-// kernels.cuh — the two hot kernels of the measurement update, hand-written for sm_100a.
+// kernels.cuh — the two hot kernels of the measurement update, hand-written for sm_90a (H100).
 //
 //   lik_kernel   LidarMeasurementModelLikelihood::measure  (src/lidar_measurement_model_likelihood.cpp:105-139)
 //                + ChunkedKdtree::radiusSearch semantics   (include/mcl_3dl/chunked_kdtree.h:217-237)
@@ -259,12 +259,10 @@ __global__ void __launch_bounds__(kBlockThreads)
 // --------------------------------------------------------------------------------------------
 // Warp-item likelihood kernel.
 //
-// ncu on the straightforward kernel above (profiles/r01a_ncu_lik_c2.txt): 9.7 of 32 lanes active and
+// Profiled, the straightforward kernel above runs with few of its 32 lanes active and
 // ~70 % of the stall samples sit on the map-point loads of the inner loop, which runs with ~5 live
 // lanes — an eval next to a surface scans ~30 map points, one that misses scans ~2, and every lane
-// waits for the slowest one, one dependent load at a time.  (A CTA-wide sort by candidate count was
-// tried, profiles/r01d_*: it halves the issued instructions but trades them for barrier stalls,
-// because the heavy evals all land in one warp.)  Here each warp works on 32 evals at a time in two
+// waits for the slowest one, one dependent load at a time.  Here each warp works on 32 evals at a time in two
 // warp-synchronous phases, no CTA barrier:
 //   phase 1 (lane = eval, uniform): transform, window, ALL row bounds of the <=3x3 window issued back
 //            to back (18 independent loads in flight per lane); the non-empty [s0,s1) runs go to
@@ -277,8 +275,8 @@ __global__ void __launch_bounds__(kBlockThreads)
 // The eval's owner lane then adds its contribution to its running sum exactly as before, so results
 // are bit-identical to the plain kernel.  Requires cell edge > window half-width (<= 3 cells/axis).
 constexpr int kMaxWinRows = 9;
-// map points fetched per batch of an item; measured 1/2/4/8 -> 90/56/52/59 us on c2 (profiles/r01i_variants.txt);
-// (before the window table) capping registers below 64 for more resident CTAs only spilled and lost (66-149 us)
+// map points fetched per batch of an item (4 was the fastest of 1/2/4/8 on c2);
+// (before the window table) capping registers below 64 for more resident CTAs only spilled and lost
 constexpr int kWiUnroll = 4;
 
 struct LikWarpSmem
@@ -290,7 +288,7 @@ struct LikWarpSmem
 };
 
 // __launch_bounds__(256, 4): with the window table the kernel wants 72 registers (3 CTAs/SM); capping at 64
-// costs 24 bytes of spill and wins (c2 55 -> 48 us, c5 373 -> 320 us; profiles/r01n_*).
+// costs 24 bytes of spill and wins.
 template <int TPP, bool STAGED>
 __global__ void __launch_bounds__(kBlockThreads, 4)
     lik_kernel_wi(const mcl3dl_pose* __restrict__ poses, int P, const float4* __restrict__ scan, int N, NnGridDev g,
@@ -455,7 +453,7 @@ __global__ void __launch_bounds__(kBlockThreads, 4)
       for (int k = 0; k < nr; ++k) sm.items[first + k] = static_cast<uint16_t>(lane | (k << 5));
       __syncwarp();
       // ---------------- phase 2: lane = item (one contiguous run of map points); a 4-lanes-per-item variant that
-      // coalesces the point loads was measured and lost (c2 48 -> 57 us, profiles/r01o_*)
+      // coalesces the point loads was measured and lost
       for (int it = lane; it < n_items; it += 32)
       {
         const uint32_t iv = sm.items[it];
@@ -520,12 +518,11 @@ __global__ void __launch_bounds__(kBlockThreads, 4)
 // --------------------------------------------------------------------------------------------
 // NN-field likelihood kernel (the default when set_map staged the field, device_funcs.cuh: NnFieldDev).
 //
-// ncu on lik_kernel_wi (profiles/r02a_ncu_lik_c2.txt / _c5.txt): 36-41 warp instructions per eval at 17-19 live lanes,
-// L1/TEX the busiest unit (48 % on c2, 85 % on c5), DRAM < 1 %: bound by the instructions and gather wavefronts of
-// walking a 3 x 3 window of CSR rows per eval.  With the field an eval is: transform, one 8-byte directory entry, then
+// Profiled, lik_kernel_wi issues tens of warp instructions per eval at about half its lanes live, with L1/TEX the
+// busiest unit and DRAM nearly idle: bound by the instructions and gather wavefronts of walking a 3 x 3 window of CSR
+// rows per eval.  With the field an eval is: transform, one 8-byte directory entry, then
 // the 1-6 contiguous candidates of its voxel — two dependent loads and ~1/4 of the instructions.  What is left is
-// latency (profiles/r02b_ncu_lik_c2.txt: issue 32 %, long scoreboard 10 per issue, SMs active 60 % of the launch), so
-// the kernel is built around loads in flight:
+// latency, so the kernel is built around loads in flight:
 //   * lane = eval, kNfU = 4 evals per lane in flight (their directory loads, then their candidate loads, overlap);
 //   * TPP in {8 .. 256} lanes per particle, chosen on the host so that a particle's scan gives every lane ~4 evals and
 //     the whole grid is resident in ONE wave where the job is small (c2: 128 lanes x 2 particles x 512 CTAs);
@@ -539,7 +536,6 @@ __global__ void __launch_bounds__(kBlockThreads, 4)
 #endif
 constexpr int kNfU = MCL3DL_NF_U;
 // resident CTAs per SM the compiler must allow (register cap): 3 -> 80 registers, 4 -> 64, 5 -> 48, 6 -> 40
-// (measured, profiles/r02c_ab.jsonl: 4 beats 3 and 5 on every workload)
 #ifndef MCL3DL_NF_MINB
 #define MCL3DL_NF_MINB 4
 #endif
@@ -936,9 +932,8 @@ __global__ void __launch_bounds__(kBlockThreads)
 // A warp takes 32 consecutive particles (one per lane) and a chunk of consecutive rays; every lane
 // casts the SAME scan ray at the same time.  In tracking mode the 32 poses are within a few
 // decimetres of each other, so the lanes walk nearly the same voxels for nearly the same number of
-// steps: the occupancy words coalesce and the trip counts agree (measured: c3 204 -> 162 us).  With
-// spread particles nothing is lost relative to the group mapping.  (The same mapping was measured
-// for the likelihood model and lost to the warp-item kernel: profiles/r01c_*.)  A CTA = one particle group x 8 chunks (8 warps); when a scan needs more than
+// steps: the occupancy words coalesce and the trip counts agree.  With
+// spread particles nothing is lost relative to the group mapping.  A CTA = one particle group x 8 chunks (8 warps); when a scan needs more than
 // 8 chunks to fill the chip, several CTAs share a particle group and the last one to finish (ticket
 // counter) folds the per-CTA partials in chunk order, so the result is still deterministic.
 constexpr int kPlWarps = kBlockThreads / 32;
@@ -1010,8 +1005,7 @@ __global__ void __launch_bounds__(kBlockThreads, 4)
       const F3 begin = ray_origin(pos, q, origins, __float_as_uint(sp.w));
       // cast_ray / cast_ray_kd are loops of "walk to the next candidate cell / marching position" followed by the
       // expensive test (fp64 cone test / nearest-neighbour searches): the lanes of the warp reconverge after the walk, so
-      // the tests of the lanes that found a candidate run together.  (An explicit warp-wide phase loop around the
-      // split functions measured the same, profiles/r02j_ab.jsonl, and was dropped.)
+      // the tests of the lanes that found a candidate run together.
       int st = ST_LONG;
       if (live)
         st = KD ? cast_ray_kd(kd, nn, g, begin, end, st_steps, st_occ, st_tested) : cast_ray(g, begin, end, st_steps, st_occ, st_tested);
@@ -1100,10 +1094,10 @@ __global__ void __launch_bounds__(kBlockThreads, 4)
 
 
 // ============================================================================================
-// Dynamic-queue variant of the lane-per-particle beam kernel (MCL3DL_BEAM=dq; A/B in profiles/).
+// Dynamic-queue variant of the lane-per-particle beam kernel.
 //
 // beam_kernel_pl gives every CTA a fixed set of (particle group, ray chunk) pairs and folds the tallies at a CTA barrier:
-// ncu shows 15.6 % of the samples of c3 waiting there (rays differ in length, the CTA waits for its slowest warp), and
+// profiles show a large share of the samples of c3 waiting there (rays differ in length, the CTA waits for its slowest warp), and
 // whole-wave grids leave nothing to fill the tail with.  Here the grid is the resident warps; every warp pulls
 // (group, chunk) items from one global counter until the queue is empty, adds its integer tallies to the particles'
 // global counters (integers: the order of the additions cannot change a bit) and the warp that completes a group's
@@ -1440,7 +1434,7 @@ __global__ void __launch_bounds__(32)
     st_release_sys(t.flags[threadIdx.x] + t.rank, step);
     const uint32_t* mine = t.flags[t.rank] + threadIdx.x;
     // steps increase monotonically; the difference is taken modulo 2^32.  Bounded: a peer that died must not hang
-    // this GPU (~2^22 polls of ~1 us, then the error word is set and the step completes with stale data)
+    // this GPU
     long polls = 0;
     while (static_cast<int32_t>(ld_acquire_sys(mine) - step) < 0)
       if (++polls > (1L << 22))

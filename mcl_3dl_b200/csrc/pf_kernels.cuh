@@ -1,5 +1,5 @@
 // pf_kernels.cuh — kernels of the resident particle set (scope row f3, SURVEY.md §8f): one thread per particle around the
-// host-verified per-particle functions of pf_funcs.cuh (first run on a B200: driver record GPUTEST_r01).
+// host-verified per-particle functions of pf_funcs.cuh.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,5 +1,5 @@
 // lidar_measurement_model_b200.h — host C++ adapter: the reference's own plugin classes with
-// measure() re-routed to the B200 engine through the C ABI (include/mcl3dl_b200.h).
+// measure() re-routed to the CUDA engine (H100) through the C ABI (include/mcl3dl_b200.h).
 //
 // Drop-in rule: the ROS node keeps calling exactly what it calls today
 //   setGlobalLocalizationStatus / filter      once per model per update  (src/mcl_3dl.cpp:378-383)

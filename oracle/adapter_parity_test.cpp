@@ -3,9 +3,8 @@
 // Drives the host C++ adapter (mcl_3dl_b200/host/lidar_measurement_model_b200.h) exactly the way
 // MCL3dlNode::measure does (src/mcl_3dl.cpp:376-426) and compares it, particle by particle, with the
 // reference's own LidarMeasurementModelLikelihood / LidarMeasurementModelBeam running on the CPU in
-// the same process.  Built only where /root/reference exists (make -C oracle adapter), against
-// oracle/shim/; the binary lands in oracle/_ref/ and travels to the GPU box, where
-// tests/test_gpu_adapter.py runs it.
+// the same process.  Built only where a checkout of the reference exists (make -C oracle adapter
+// REFERENCE=<path>), against oracle/shim/; the binary lands in oracle/_ref/, where tests/test_gpu_adapter.py runs it.
 #include <cmath>
 #include <cstdio>
 #include <map>

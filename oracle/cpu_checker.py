@@ -2,7 +2,8 @@
 
 Loads either CPU checker:
   kind="port"       oracle/libmcl3dl_oracle.so   (repo-owned restatement, always available)
-  kind="reference"  oracle/_ref/libmcl3dl_ref.so (reference's own sources; prebuilt in the dev container)
+  kind="reference"  oracle/_ref/libmcl3dl_ref.so (reference's own sources, built where a checkout of at-wat/mcl_3dl
+                    exists: oracle/Makefile's REFERENCE, or $MCL3DL_REFERENCE)
 
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs may import
 this module.  The product package (mcl_3dl_b200/) never does.
@@ -14,6 +15,7 @@ import subprocess
 import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
+REFERENCE = os.environ.get("MCL3DL_REFERENCE")  # overrides the Makefile's default location of the reference checkout
 
 POINT = np.dtype([("x", "<f4"), ("y", "<f4"), ("z", "<f4"), ("label", "<u4")])
 POSE = np.dtype([("px", "<f4"), ("py", "<f4"), ("pz", "<f4"), ("_pad", "<f4"),
@@ -107,16 +109,24 @@ def lib_path(kind):
         return os.path.join(HERE, "libmcl3dl_oracle.so")
     if kind == "reference":
         return os.path.join(HERE, "_ref", "libmcl3dl_ref.so")
+    if kind == "adapter":
+        return os.path.join(HERE, "_ref", "adapter_parity_test")
     raise ValueError(kind)
 
 
+def _make(args, quiet=True):
+    ref = ["REFERENCE=" + REFERENCE] if REFERENCE else []
+    return subprocess.run(["make", "-C", HERE] + args + ref, capture_output=quiet, text=True)
+
+
 def build(kind="port", quiet=True):
-    """Compile the checker if its .so is missing (make in oracle/)."""
+    """Compile a checker if it is missing or stale (make in oracle/).  "reference" and "adapter" compile the reference's
+    own sources from its checkout; where there is none they only report whether an earlier build exists."""
     path = lib_path(kind)
-    target = [] if kind == "port" else ["ref"]
-    if kind == "reference" and not os.path.isdir("/root/reference/include/mcl_3dl"):
+    target = {"port": [], "reference": ["ref"], "adapter": ["adapter"]}[kind]
+    if kind != "port" and _make(["-s", "has-ref"]).returncode != 0:
         return os.path.exists(path)
-    r = subprocess.run(["make", "-C", HERE] + target, capture_output=quiet, text=True)
+    r = _make(target, quiet)
     if r.returncode != 0:
         raise RuntimeError("oracle build failed:\n" + (r.stdout or "") + (r.stderr or ""))
     return os.path.exists(path)

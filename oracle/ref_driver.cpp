@@ -2,8 +2,8 @@
 //
 // Thin C-ABI driver around the REFERENCE's own, unmodified hot-path sources.  It is compiled
 // (oracle/Makefile, target _ref) together with
-//     /root/reference/src/lidar_measurement_model_likelihood.cpp
-//     /root/reference/src/lidar_measurement_model_beam.cpp
+//     $(REFERENCE)/src/lidar_measurement_model_likelihood.cpp
+//     $(REFERENCE)/src/lidar_measurement_model_beam.cpp
 // and the reference headers they include, where they lie, against the stand-in headers in
 // oracle/shim/ (PCL, Eigen, ROS are not installed here).  Output: oracle/_ref/libmcl3dl_ref.so,
 // git-ignored.  No reference source is copied into this repository.

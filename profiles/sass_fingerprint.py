@@ -1,8 +1,8 @@
 #!/usr/bin/env python
 """Per-kernel SASS fingerprints of a built library (addresses stripped), to tell whether an edit touched a kernel's code.
 
-    python profiles/sass_fingerprint.py [lib.so] > profiles/<tag>_sass_fingerprint.txt
-    python profiles/sass_fingerprint.py --diff profiles/r02_sass_fingerprint.txt [lib.so]
+    python profiles/sass_fingerprint.py [lib.so] > profiles/sass_fingerprint.txt
+    python profiles/sass_fingerprint.py --diff profiles/sass_fingerprint.txt [lib.so]
 """
 import hashlib
 import os
@@ -12,6 +12,13 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 DEFAULT = os.path.join(ROOT, "mcl_3dl_b200", "libmcl3dl_b200.so")
+# nvcc names a translation unit's anonymous namespace after hashes of its source path: strip them, so that the same
+# code built in another directory has the same names
+ANON_NS = re.compile(r"_GLOBAL__N__[0-9a-f]{8}_(\d+_\w*?)_[0-9a-f]{8}")
+
+
+def _stable(text):
+    return ANON_NS.sub(r"_GLOBAL__N__\1", text)
 
 
 def fingerprints(lib):
@@ -20,11 +27,11 @@ def fingerprints(lib):
     for line in out.splitlines():
         m = re.match(r"\s*Function : (\S+)", line)
         if m:
-            cur = m.group(1)
+            cur = _stable(m.group(1))
             funcs[cur] = hashlib.sha256()
             continue
         if cur:
-            funcs[cur].update(re.sub(r"/\*[0-9a-f]{4,}\*/", "", line).encode())
+            funcs[cur].update(_stable(re.sub(r"/\*[0-9a-f]{4,}\*/", "", line)).encode())
     return {k: v.hexdigest()[:16] for k, v in funcs.items()}
 
 

@@ -10,7 +10,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; run with -m gpu)")
 
 
 def _cuda_usable():
@@ -26,7 +26,7 @@ def _cuda_usable():
 
 def pytest_collection_modifyitems(config, items):
     if any(it.get_closest_marker("gpu") for it in items) and not _cuda_usable():
-        skip = pytest.mark.skip(reason="needs a CUDA device (run on the B200 box with -m gpu)")
+        skip = pytest.mark.skip(reason="needs a CUDA device (an H100; run with -m gpu)")
         for it in items:
             if it.get_closest_marker("gpu"):
                 it.add_marker(skip)
@@ -38,19 +38,6 @@ def port():
     from oracle import cpu_checker as cc
     cc.build("port")
     return cc.CpuChecker("port")
-
-
-@pytest.fixture(scope="session")
-def reference():
-    """The reference's own sources compiled against shims (oracle/_ref); skip where unavailable."""
-    from oracle import cpu_checker as cc
-    try:
-        ok = cc.build("reference")
-    except RuntimeError:
-        ok = cc.available("reference")
-    if not ok:
-        pytest.skip("oracle/_ref not built and /root/reference absent")
-    return cc.CpuChecker("reference")
 
 
 def golden(name):

@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE: a stand-in for mcl_3dl_b200.engine whose Engine runs on the HOST through tests/hostsim (the
 product's per-thread device functions compiled for the host).  It lets the CPU suite execute the bodies of GPU tests
-whose kernels are thin wrappers around those functions (tests/test_gpu_resident.py), so that a failure on the B200 can
+whose kernels are thin wrappers around those functions (tests/test_gpu_resident.py), so that a failure on the H100 can
 only come from the kernels / plumbing, not from the tests' own expectations.  Never imported by the product."""
 import ctypes as C
 import os

@@ -1,9 +1,9 @@
 """Regenerate tests/golden/*.npz by running the REFERENCE's own sources (oracle/_ref).
 
-Only runnable in the development container (needs /root/reference to build oracle/_ref).
+Needs a checkout of the reference to build oracle/_ref (oracle/Makefile's REFERENCE, or $MCL3DL_REFERENCE):
     python tests/golden/make_golden.py
-The committed .npz files hold inputs AND the reference outputs, so the GPU box (which has no
-/root/reference) can check both the port oracle and the CUDA engine against them.
+The committed .npz files hold the reference outputs (and the inputs, where they are not regenerated from a seed by the
+tests), so a checkout without the reference can check both the port oracle and the CUDA engine against them.
 
 Fixtures
   beam_likelihood_world.npz  the world and parameter sweep of test/src/test_beam_likelihood.cpp:81-138
@@ -14,6 +14,9 @@ Fixtures
                              synthetic room scenes (mcl_3dl_b200.synth) -> per-particle records + per-ray status.
   chunked_radius_search.npz  random ChunkedKdtree::radiusSearch queries (ids + d2), incl. chunk borders.
   transform.npz              State6DOF::transform of random points by random (non-unit) quaternions.
+  reference_checks.npz       the reference build's outputs for the seeded cases of tests/test_oracle_golden.py
+                             (resampling, motion prediction, scan clipping, pose estimate, scene records).
+  reference_properties.npz   the reference build's outputs for the fixed examples of tests/test_oracle_properties.py.
 """
 import os
 import sys
@@ -22,6 +25,7 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))  # the seeded inputs of the reference cross-checks live with their tests
 from mcl_3dl_b200 import synth  # noqa: E402
 from oracle import cpu_checker as cc  # noqa: E402
 
@@ -146,8 +150,52 @@ def gen_transform(ref):
     print("transform ok")
 
 
+def gen_reference_checks(ref):
+    import test_oracle_golden as T
+    out = {}
+    for key, (probs, states, seed, sigma) in T.pf_resample_cases():
+        out[key + "_s"], out[key + "_p"] = ref.pf_resample_1d(probs, states, seed=seed, sigma=sigma)
+    for key, args in T.motion_prediction_cases():
+        out[key] = T.digest(ref.motion_predict(*args))
+    for key, (probs, st, seed, sp, sr) in T.state6dof_resample_cases():
+        a, out[key + "_p"] = ref.pf_resample_6dof(probs, st, seed, sp, sr)
+        out[key] = a.view(np.uint8)
+    pts = T.filter_clip_points()
+    for i, args in enumerate(T.CLIP_ARGS):
+        out["clip_%d" % i] = np.packbits(ref.filter_clip(pts, *args))
+    out["point_budget"] = np.array([ref.global_localization_points(*args) for args in T.BUDGET_ARGS], dtype=np.int64)
+    for row in T.REFERENCE_SCENES:
+        s, lik, braw, msr = T.reference_scene(*row)
+        m = ref.create(s["map"], lik, braw, 20.0, msr)
+        key = "scene_%d" % row[0]
+        out[key + "_beam_params"] = np.frombuffer(bytes(m.beam_params()), dtype=np.uint8)
+        out[key + "_records"] = m.measure(s["particles"], s["lik"], s["beam"], s["origins"]).view(np.uint8)
+        out[key + "_status"] = m.beam_status(s["particles"], s["beam"], s["origins"])
+        m.close()
+    for key, args in T.pose_estimate_cases():
+        mean, best, cov = ref.pf_estimate(*args)
+        out[key + "_mean"], out[key + "_max_index"], out[key + "_cov"] = mean.view(np.uint8), np.int64(best), cov
+    np.savez_compressed(os.path.join(OUT, "reference_checks.npz"), **out)
+    print("reference_checks", len(out), "arrays")
+
+
+def gen_reference_properties(ref):
+    import test_oracle_properties as T
+    from test_oracle_golden import digest
+    out = {}
+    for i, ex in enumerate(T.DDA_EXAMPLES):
+        out["dda_%d" % i] = T.dda_walks(ref, *ex)
+    for i, ex in enumerate(T.KD_EXAMPLES):
+        out["kd_%d" % i] = digest(T.kd_walks(ref, *ex))
+    for i, ex in enumerate(T.RECORD_EXAMPLES):
+        rec, out["status_%d" % i], out["radius_%d" % i] = T.records(ref, *ex)
+        out["rec_%d" % i] = rec.view(np.uint8)
+    np.savez_compressed(os.path.join(OUT, "reference_properties.npz"), **out)
+    print("reference_properties", len(out), "arrays")
+
+
 if __name__ == "__main__":
-    assert cc.build("reference"), "oracle/_ref cannot be built here (no /root/reference)"
+    assert cc.build("reference"), "oracle/_ref cannot be built here (no reference tree)"
     ref = cc.CpuChecker("reference")
     gen_beam_likelihood(ref)
     gen_room(ref, "room_iso", (1, 1, 1), False, seed=100)
@@ -157,3 +205,5 @@ if __name__ == "__main__":
     gen_room(ref, "room_kd_aniso", (1, 1, 5), False, seed=500, use_dda=False, filter_label_max=1, short_only=False)
     gen_radius_search(ref)
     gen_transform(ref)
+    gen_reference_checks(ref)
+    gen_reference_properties(ref)

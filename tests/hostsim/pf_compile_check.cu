@@ -1,6 +1,6 @@
 // pf_compile_check.cu — TEST INFRASTRUCTURE ONLY: instantiates every function of mcl_3dl_b200/csrc/pf_funcs.cuh in device
-// code, so that `nvcc -gencode arch=compute_100a,code=sm_100a -c` proves the f3 groundwork compiles for the B200
-// (tests/test_hostsim.py::test_pf_funcs_compile_for_sm_100a).  The thin kernels below are also the shape the round-2
+// code, so that `nvcc -gencode arch=compute_90a,code=sm_90a -c` proves the f3 groundwork compiles for the H100
+// (tests/test_hostsim.py::test_pf_funcs_compile_for_sm_90a).  The thin kernels below are also the shape the round-2
 // kernels will take: one thread per particle around the host-verified per-thread functions.
 #include <cuda_runtime.h>
 

@@ -122,9 +122,10 @@ def test_bound_measure_call_resolves_buffers_once():
 
 
 def test_kernels_match_the_last_gpu_validated_fingerprint():
-    """Informational guard: profiles/r02_sass_fingerprint.txt holds per-kernel SASS hashes of the build that last ran on
-    a B200.  A kernel that differs has not been validated on hardware yet: re-run the GPU suite, then regenerate the file
-    (python profiles/sass_fingerprint.py).  Reported as xfail, never as a failure."""
+    """Informational guard: profiles/sass_fingerprint.txt holds per-kernel SASS hashes of the build that last passed the
+    GPU suite on an H100.  A kernel that differs has not been validated on hardware yet: re-run the GPU suite, then
+    regenerate the file (python profiles/sass_fingerprint.py > profiles/sass_fingerprint.txt).  Reported as xfail, never
+    as a failure."""
     import shutil
     import sys
     if not shutil.which("cuobjdump"):
@@ -133,7 +134,7 @@ def test_kernels_match_the_last_gpu_validated_fingerprint():
     import sass_fingerprint as sf
     from mcl_3dl_b200 import engine
     engine.load_library()   # builds if stale
-    want = dict(line.split() for line in open(os.path.join(ROOT, "profiles", "r02_sass_fingerprint.txt"))
+    want = dict(line.split() for line in open(os.path.join(ROOT, "profiles", "sass_fingerprint.txt"))
                 if line.strip() and not line.startswith("#"))
     got = sf.fingerprints(sf.DEFAULT)
     changed = sorted(k for k in got if k in want and want[k] != got[k])

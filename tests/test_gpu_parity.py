@@ -1,5 +1,5 @@
 """GPU parity: the CUDA engine, called through the C ABI, against the CPU oracle and the committed
-golden outputs of the reference's own sources.  Everything here needs a B200 (`-m gpu`).
+golden outputs of the reference's own sources.  Everything here needs an H100 (`-m gpu`).
 
 Bars (BASELINE.json north_star): beam HIT/SHORT/LONG tallies and per-ray BeamStatus bit-exact;
 match counts bit-exact; likelihood scores within 1e-4 relative (the per-particle float sum is
@@ -482,7 +482,7 @@ def test_page_locked_caller_arrays_are_transferred_in_place(eng_mod, eng_mod_eng
     assert eng.measure(keep, s["lik"], s["beam"], s["origins"]).tobytes() == want.tobytes()
 
 
-# ------------------------------------------------------------------ engine options (profiles/r01y_ab_variants.txt)
+# ------------------------------------------------------------------ engine options
 @pytest.mark.parametrize("use_dda", [True, False])
 def test_options_change_no_record(eng_mod, monkeypatch, use_dda):
     """The near-field screens, the zero-copy record stores and the timing events are pure performance options:

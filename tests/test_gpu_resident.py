@@ -1,6 +1,5 @@
 """Resident particle set (scope row f3, mcl3dl_particles_*): predict, measure + weight update, resample on the device.
 
-First run on a B200: driver record GPUTEST_r01 (10 passed as XPASS); the first-run marker is gone since round 2.
 """
 import numpy as np
 import pytest

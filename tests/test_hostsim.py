@@ -466,12 +466,12 @@ def test_pf_resample_device_semantics(hostsim, port):
     assert np.all(out_p == np.float32(1.0 / n))
 
 
-def test_pf_funcs_compile_for_sm_100a(tmp_path):
-    """The f3 groundwork is device code: nvcc must accept it for sm_100a with the product's flags (no GPU needed)."""
+def test_pf_funcs_compile_for_sm_90a(tmp_path):
+    """The f3 groundwork is device code: nvcc must accept it for sm_90a with the product's flags (no GPU needed)."""
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
     if not os.path.exists(nvcc):
         pytest.skip("nvcc not available")
-    r = subprocess.run([nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-fmad=false", "-std=c++17", "-c",
+    r = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-fmad=false", "-std=c++17", "-c",
                         "-o", str(tmp_path / "pf.o"), os.path.join(HS, "pf_compile_check.cu")], capture_output=True, text=True)
     assert r.returncode == 0, r.stderr
 

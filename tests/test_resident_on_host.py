@@ -1,6 +1,6 @@
 """The bodies of tests/test_gpu_resident.py executed on the HOST: tests/fake_engine.py implements the resident particle
 set with the product's per-thread device functions compiled for the host (tests/hostsim).  If these pass here, a failure
-of the same test on the B200 can only come from the kernels or the engine's plumbing around those functions."""
+of the same test on the H100 can only come from the kernels or the engine's plumbing around those functions."""
 import pytest
 
 import fake_engine
