@@ -577,36 +577,22 @@ __device__ __forceinline__ int nnf_lookup(const NnFieldDev& f, float qx, float q
   return nnf_slot(f, d, (vx & 1) | ((vy & 1) << 1) | ((vz & 1) << 2), start);
 }
 
-// A voxel's candidate list is walked 16 bytes at a time, one 32-byte sector per two records and every new sector a fresh
-// L2 / DRAM latency when the list is cold.  Ask for the sectors behind the first one as soon as the directory entry is
-// decoded (no registers held; lists of up to 7-8 records are covered).
-// MCL3DL_NF_PREFETCH: 0 off, 1 prefetch.global.L1, 2 prefetch.global.L2.
-#ifndef MCL3DL_NF_PREFETCH
-#define MCL3DL_NF_PREFETCH 2
-#endif
-__device__ __forceinline__ void nnf_prefetch_list(const NnFieldDev& f, uint32_t start, int count)
+// Warp-cooperative candidate scan (kernels.cuh: lik_kernel_nf, phase B).  The candidate lists of a warp's evals are laid
+// end to end in one list of (eval, candidate) slots; the list of eval `e` occupies slots [base, base + count).  A pass
+// covers slots [lo, hi): name `e` as the owner of its slots in that range (own[slot - lo]).
+__device__ __forceinline__ void nnf_fill_owner(uint8_t* own, int lo, int hi, int base, int count, int e)
 {
-#if defined(__CUDA_ARCH__) && MCL3DL_NF_PREFETCH
-  const float4* cp = f.cand + start;
-  const int i0 = 2 - static_cast<int>(start & 1u);  // first record of the next sector
-#ifndef MCL3DL_NF_PREFETCH_DEPTH
-#define MCL3DL_NF_PREFETCH_DEPTH 3
-#endif
-#pragma unroll
-  for (int k = 0; k < MCL3DL_NF_PREFETCH_DEPTH; ++k)
-    if (i0 + 2 * k < count)
-    {
-#if MCL3DL_NF_PREFETCH == 1
-      asm volatile("prefetch.global.L1 [%0];" ::"l"(cp + i0 + 2 * k));
-#else
-      asm volatile("prefetch.global.L2 [%0];" ::"l"(cp + i0 + 2 * k));
-#endif
-    }
-#else
-  (void)f;
-  (void)start;
-  (void)count;
-#endif
+  const int a = max(base, lo), b = min(base + count, hi);
+  for (int i = a; i < b; ++i) own[i - lo] = static_cast<uint8_t>(e);
+}
+
+// flann::L2_Simple of one candidate: sequential float accumulate of squared differences
+__device__ __forceinline__ float nnf_cand_d2(float qx, float qy, float qz, const float4& m)
+{
+  const float dx = fsub(qx, m.x);
+  const float dy = fsub(qy, m.y);
+  const float dz = fsub(qz, m.z);
+  return fadd(fadd(fmul(dx, dx), fmul(dy, dy)), fmul(dz, dz));
 }
 
 // nn_dist2 through the field (likelihood model): min over the voxel's candidates, r2 if none is closer.
