@@ -7,6 +7,8 @@
 #include <cuda_runtime.h>
 #endif
 #include <math.h>
+#include <algorithm>
+#include <cmath>
 #include <stdint.h>
 
 #include "device_math.cuh"
@@ -593,6 +595,66 @@ __device__ __forceinline__ float nnf_cand_d2(float qx, float qy, float qz, const
   const float dy = fsub(qy, m.y);
   const float dz = fsub(qz, m.z);
   return fadd(fadd(fmul(dx, dx), fmul(dy, dy)), fmul(dz, dz));
+}
+
+// Point-major likelihood kernel (kernels.cuh: lik_kernel_nf_pm).  The scan is cut into n_slices slices of `slice`
+// points (a multiple of `unit`, the points of one warp trip): as many as put one CTA of every (particle block, slice)
+// pair in the `slots` resident CTA slots, `blocks` particle blocks given.  Each slice adds one 64-bit word per particle
+// into the particle's accumulator: [arr_bits: 1, the slice's arrival | cnt_bits: its matches | the rest, signed: the sum
+// of its contributions in 2^-fx_shift fixed point].  The fields below the sum never carry (arrivals <= n_slices <
+// 2^arr_bits, matches <= N < 2^cnt_bits), and fx_shift keeps N contributions of at most match_dist_min * |match_weight|
+// each below a quarter of the sum field's range.  ok: the rounding of N terms stays below 2^-30 of that bound (scans of
+// up to a few thousand points); otherwise the particle-major kernel runs.
+struct NfPmShape
+{
+  int slice, n_slices, fx_shift, arr_bits, cnt_bits;
+  bool ok;
+};
+inline int nf_bit_width(int v)
+{
+  int b = 0;
+  while (b < 31 && (v >> b) != 0) ++b;
+  return b;
+}
+inline NfPmShape nf_pm_shape(int N, int blocks, int slots, int unit, float match_dist_min, float match_weight)
+{
+  NfPmShape s;
+  const int n = std::max(1, std::min(slots / std::max(blocks, 1), (N + unit - 1) / unit));
+  s.slice = std::max(unit, ((N + n - 1) / n + unit - 1) / unit * unit);
+  s.n_slices = std::max(1, (N + s.slice - 1) / s.slice);
+  s.arr_bits = nf_bit_width(s.n_slices);
+  s.cnt_bits = nf_bit_width(N);
+  const int sum_bits = 64 - s.arr_bits - s.cnt_bits;
+  const double bound = static_cast<double>(std::max(N, 1)) * std::fabs(static_cast<double>(match_dist_min)) *
+                       std::fabs(static_cast<double>(match_weight));
+  int e = 0;
+  if (bound > 0.0)
+    std::frexp(bound, &e);  // bound < 2^e
+  s.fx_shift = std::max(-120, std::min(120, sum_bits - 3 - e));
+  s.ok = sum_bits - 3 - nf_bit_width(N) >= 30;
+  return s;
+}
+// one eval's contribution in fixed point (exact but for the bits below 2^-fx_shift: the scale is a power of two)
+__device__ __forceinline__ long long nf_fx_term(float contribution, int fx_shift)
+{
+  return static_cast<long long>(rintf(fmul(contribution, ldexpf(1.0f, fx_shift))));
+}
+// the word one slice adds to a particle's accumulator
+__device__ __forceinline__ unsigned long long nf_pm_word(long long sum, uint32_t cnt, const NfPmShape& s)
+{
+  return (static_cast<unsigned long long>(sum) << (s.arr_bits + s.cnt_bits)) +
+         (static_cast<unsigned long long>(cnt) << s.arr_bits) + 1ull;
+}
+// the accumulator after a slice's addition: true when it was the particle's last slice, with the match count and the
+// score (the fixed-point sum back in float, rounded once)
+__device__ __forceinline__ bool nf_pm_done(unsigned long long v, const NfPmShape& s, uint32_t& cnt, float& score)
+{
+  if ((v & ((1ull << s.arr_bits) - 1ull)) != static_cast<unsigned long long>(s.n_slices))
+    return false;
+  cnt = static_cast<uint32_t>((v >> s.arr_bits) & ((1ull << s.cnt_bits) - 1ull));
+  const long long sum = static_cast<long long>(v) >> (s.arr_bits + s.cnt_bits);  // arithmetic: the sum is signed
+  score = fmul(static_cast<float>(sum), ldexpf(1.0f, -s.fx_shift));               // int64 -> float rounds to nearest
+  return true;
 }
 
 // nn_dist2 through the field (likelihood model): min over the voxel's candidates, r2 if none is closer.

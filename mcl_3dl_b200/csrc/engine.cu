@@ -370,6 +370,7 @@ struct DeviceCtx
   DevBuf d_w, d_post, d_wpart, d_wticket;   // fused weight update: w_i, posterior, per-CTA partials, last-CTA tickets (2)
   DevBuf d_partial, d_tickets;  // lane-per-particle kernels: per-CTA partials + per-group ticket counters
   DevBuf d_tally, d_queue;      // dynamic-queue beam kernel: per-particle integer tallies, item counter (left at zero)
+  DevBuf d_lacc;                // point-major likelihood kernel: per-particle accumulators (left at zero)
   size_t tally_zeroed = 0;
   size_t tickets_zeroed = 0;
   std::vector<const void*> smem_opted;  // kernels already opted in to large dynamic shared memory on this device
@@ -655,11 +656,47 @@ int launch_lik_nf_t(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_pose* poses, 
   return MCL3DL_OK;
 }
 
+// point-major mapping (kernels.cuh: lik_kernel_nf_pm): 256 particles per CTA, the scan cut into slices (nf_pm_shape)
+int launch_lik_nf_pm(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_pose* poses, int P, const float4* scan, int N,
+                     mcl3dl_result* out, int beam_defaults, cudaStream_t st, const RecordSink& sink, int blocks,
+                     const NfPmShape& sh)
+{
+  // one accumulator per particle; zeroed once, the kernel leaves it at zero
+  const size_t bytes = static_cast<size_t>(P) * 8;
+  if (bytes > c.d_lacc.cap || !c.d_lacc.p)
+  {
+    if (int rc = reserve(eng, c.d_lacc, bytes))
+      return rc;
+    CK(cudaMemsetAsync(c.d_lacc.p, 0, c.d_lacc.cap, st));
+  }
+  auto* acc = static_cast<unsigned long long*>(c.d_lacc.p);
+#define PM_LAUNCH(O)                                                                                                       \
+  lik_kernel_nf_pm<O><<<blocks * sh.n_slices, kBlockThreads, 0, st>>>(poses, P, scan, N, c.nn, eng->likdev, out,           \
+                                                                      beam_defaults, c.stats_ptr(), sink, sh, acc)
+  if (eng->nnf_overflow_cells != 0)
+    PM_LAUNCH(true);
+  else
+    PM_LAUNCH(false);
+#undef PM_LAUNCH
+  CK(cudaGetLastError());
+  eng->launches++;
+  return MCL3DL_OK;
+}
+
 int launch_lik_nf(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_pose* poses, size_t P, const mcl3dl_point* scan, size_t N,
                   mcl3dl_result* out, int beam_defaults, cudaStream_t st, const RecordSink& sink)
 {
   const float4* s4 = reinterpret_cast<const float4*>(scan);
   const int p = static_cast<int>(P), n = static_cast<int>(N);
+  if (P >= static_cast<size_t>(kBlockThreads))  // a full CTA of particles per scan point
+  {
+    const int blocks = (p + kBlockThreads - 1) / kBlockThreads;
+    const int per_sm = beam_defaults ? kNfCtasPerSm : std::max(1, std::min(kNfCtasPerSm, eng->lik_share));
+    const NfPmShape sh = nf_pm_shape(n, blocks, c.sm_count * per_sm, kNfU, eng->likdev.match_dist_min,
+                                     eng->likdev.match_weight);
+    if (sh.ok)
+      return launch_lik_nf_pm(eng, c, poses, p, s4, n, out, beam_defaults, st, sink, blocks, sh);
+  }
   switch (pick_tpp_nf(P, N, c.sm_count))
   {
     case 8: return launch_lik_nf_t<8>(eng, c, poses, p, s4, n, out, beam_defaults, st, sink);
@@ -1598,7 +1635,7 @@ void mcl3dl_destroy(mcl3dl_engine* eng)
                       &c.s_clip[0], &c.s_clip[1], &c.s_out[0], &c.s_out[1], &c.s_tmp, &c.s_counts})
       free_buf(*b);
     for (DevBuf* b : {&c.nn_cell_start, &c.nn_pts, &c.nn_row3, &c.dda_occ, &c.dda_cell_start, &c.dda_pts, &c.raw_pts, &c.near_lik, &c.near_kd, &c.nnf_dir, &c.nnf_cand, &c.nnf_wide, &c.fld_cells, &c.d_poses,
-                      &c.d_out, &c.d_status, &c.d_stats, &c.d_partial, &c.d_tickets, &c.d_tally, &c.d_queue, &c.d_w, &c.d_post, &c.d_wpart, &c.d_wticket})
+                      &c.d_out, &c.d_status, &c.d_stats, &c.d_partial, &c.d_tickets, &c.d_tally, &c.d_queue, &c.d_lacc, &c.d_w, &c.d_post, &c.d_wpart, &c.d_wticket})
       free_buf(*b);
     if (c.fld_nodes.ptr)
       cudaFree(c.fld_nodes.ptr);

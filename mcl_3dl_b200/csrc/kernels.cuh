@@ -818,6 +818,192 @@ __global__ void __launch_bounds__(kBlockThreads, MCL3DL_NF_MINB)
 }
 
 // --------------------------------------------------------------------------------------------
+// Point-major mapping of the NN-field likelihood kernel (many particles per scan point).
+//
+// A lane owns one particle; the warp's 32 lanes are 32 consecutive particles on the SAME scan point, and the CTA's 8
+// warps are 256 consecutive particles on the same slice of `slice` scan points.  In tracking mode the particles of a
+// cloud see one scan point in nearly the same place, so their directory and candidate sectors coalesce within the
+// load instruction and the CTA's other warps find them in L1, where lik_kernel_nf (a warp = one particle's points)
+// sends every eval's sectors to L2 on its own.  The transform, the directory lookup (phase A) and the warp-flattened
+// candidate scan (phase B) are lik_kernel_nf's; only eval e = u * 32 + lane now means (particle lane, point j0 + u).
+//
+// A particle's points are spread over the grid's slices, so its score is folded across CTAs.  Each lane sums its
+// slice's contributions in 2^-fx_shift fixed point and adds one word (device_funcs.cuh: nf_pm_word: the sum, the match
+// count and an arrival) to the particle's 64-bit accumulator with one atomic.  Integer additions give the same total
+// in any order, so the records are deterministic; the returned value tells the lane that brings the arrivals to
+// n_slices, which stores the record and leaves the accumulator at zero.  No fence, ticket or read-back: the fold is one
+// round trip to L2 after the candidate scan.  The score is the exact sum of the float contributions rounded once to
+// float (to the fixed-point step, below 2^-30 / N of the largest possible score: nf_pm_shape).  A fold of the float contributions in scan
+// order would be a chain of N dependent adds over N loads at the end of the kernel, after every other warp has finished.
+template <bool OVF>
+__global__ void __launch_bounds__(kBlockThreads, MCL3DL_NF_MINB)
+    lik_kernel_nf_pm(const mcl3dl_pose* __restrict__ poses, int P, const float4* __restrict__ scan, int N, NnGridDev g,
+                     LikDev lp, mcl3dl_result* __restrict__ out, int write_beam_defaults,
+                     unsigned long long* __restrict__ stats, RecordSink sink, NfPmShape sh,
+                     unsigned long long* __restrict__ acc)
+{
+  __shared__ NfWarpSmem nfw[kBlockThreads / 32];
+  const int lane = threadIdx.x & 31;
+  const int group = (blockIdx.x / sh.n_slices) * (kBlockThreads / 32) + (threadIdx.x >> 5);
+  if (group * 32 >= P)
+    return;  // warp-uniform: no CTA barrier below
+  NfWarpSmem& ws = nfw[threadIdx.x >> 5];
+  const int s0 = (blockIdx.x % sh.n_slices) * sh.slice, s1 = min(N, s0 + sh.slice);
+  const int p = group * 32 + lane;
+  const bool live = p < P;
+  const NnFieldDev& f = g.field;
+  uint32_t st_rows = 0, st_pts = 0;
+  long long sum = 0;
+  uint32_t cnt = 0;
+  F3 pos;
+  Q4 rn;
+  pos.x = pos.y = pos.z = 0.0f;
+  rn.x = rn.y = rn.z = 0.0f;
+  rn.w = 1.0f;
+  if (live)
+  {
+    const float4 a = __ldg(reinterpret_cast<const float4*>(poses + p));
+    const float4 b = __ldg(reinterpret_cast<const float4*>(poses + p) + 1);
+    pos.x = a.x;
+    pos.y = a.y;
+    pos.z = a.z;
+    Q4 q;
+    q.x = b.x;
+    q.y = b.y;
+    q.z = b.z;
+    q.w = b.w;
+    rn = qnormalized(q);  // state_6dof.h:217
+  }
+  // every lane of the warp runs every trip (dead particles: no candidates), as in lik_kernel_nf
+  for (int j0 = s0; j0 < s1; j0 += kNfU)
+  {
+    // ---- phase A: one scan point per u, the same for every lane (one broadcast load)
+    int c[kNfU], b[kNfU];
+    uint32_t s[kNfU];
+    int tot = 0;
+#pragma unroll
+    for (int u = 0; u < kNfU; ++u)
+    {
+      c[u] = 0;
+      s[u] = 0;
+      float4 q = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+      if (j0 + u < s1)
+      {
+        const float4 sp = __ldg(scan + j0 + u);
+        if (live)
+        {
+          F3 v;
+          v.x = sp.x;
+          v.y = sp.y;
+          v.z = sp.z;
+          const F3 t = transform_point(rn, pos, v);
+          // PointRepresentation::vectorize with rescale values (mcl_3dl.cpp:1270)
+          q.x = fmul(t.x, g.wx);
+          q.y = fmul(t.y, g.wy);
+          q.z = fmul(t.z, g.wz);
+          c[u] = nnf_lookup(f, q.x, q.y, q.z, s[u]);
+          tot += max(c[u], 0);
+          st_rows++;
+        }
+      }
+      ws.q[u * 32 + lane] = q;
+    }
+    // ---- flatten and phase B: lik_kernel_nf's
+    int incl = tot;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1)
+    {
+      const int v = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= o)
+        incl += v;
+    }
+    const int W = __shfl_sync(0xffffffffu, incl, 31);
+    int base = incl - tot;
+#pragma unroll
+    for (int u = 0; u < kNfU; ++u)
+    {
+      b[u] = base;
+      base += max(c[u], 0);
+      ws.q[u * 32 + lane].w = __uint_as_float(s[u] - static_cast<uint32_t>(b[u]));
+      ws.best[u * 32 + lane] = __float_as_uint(lp.r2);
+    }
+    for (int lo = 0; lo < W; lo += kNfSlots)
+    {
+      const int hi = min(W, lo + kNfSlots);
+#pragma unroll
+      for (int u = 0; u < kNfU; ++u) nnf_fill_owner(ws.own, lo, hi, b[u], max(c[u], 0), u * 32 + lane);
+      __syncwarp();
+      for (int k = lo + lane; k < hi; k += 32 * kNfB)
+      {
+        int e[kNfB];
+        float4 m[kNfB];
+#pragma unroll
+        for (int v = 0; v < kNfB; ++v)
+          if (k + 32 * v < hi)
+          {
+            e[v] = ws.own[k + 32 * v - lo];
+            m[v] = __ldg(f.cand + (__float_as_uint(ws.q[e[v]].w) + static_cast<uint32_t>(k + 32 * v)));
+          }
+#pragma unroll
+        for (int v = 0; v < kNfB; ++v)
+          if (k + 32 * v < hi)
+          {
+            const float4 qe = ws.q[e[v]];
+            atomicMin(&ws.best[e[v]], __float_as_uint(nnf_cand_d2(qe.x, qe.y, qe.z, m[v])));
+          }
+      }
+      __syncwarp();
+    }
+    // ---- back to the owners: this lane's particle at points j0 .. j0 + kNfU - 1
+#pragma unroll
+    for (int u = 0; u < kNfU; ++u)
+    {
+      float best = __uint_as_float(ws.best[u * 32 + lane]);
+      if (OVF && c[u] < 0)
+      {
+        const float4 qu = ws.q[u * 32 + lane];
+        best = nn_dist2(g, lp, qu.x, qu.y, qu.z, st_rows, st_pts);
+      }
+      else
+        st_pts += static_cast<uint32_t>(max(c[u], 0));
+      if (best < lp.r2)  // (dead lanes and points beyond the slice keep best = r2)
+      {
+        // likelihood.cpp:128-133
+        const float dist = fsub(lp.match_dist_min, fmaxf(__fsqrt_rn(best), lp.match_dist_flat));
+        if (!(dist < 0.0f))
+        {
+          sum += nf_fx_term(fmul(dist, lp.match_weight), sh.fx_shift);
+          cnt++;
+        }
+      }
+    }
+    __syncwarp();  // the next trip overwrites q / best
+  }
+  // ---- fold across the slices: one atomic per particle and slice, whose result tells the last slice
+  if (live)
+  {
+    const unsigned long long w = nf_pm_word(sum, cnt, sh);
+    uint32_t n;
+    float score;
+    if (nf_pm_done(atomicAdd(acc + p, w) + w, sh, n, score))
+    {
+      acc[p] = 0ull;  // every slice has added: nothing else touches it in this launch
+      // empty scan -> LidarMeasurementResult(1, 0), likelihood.cpp:111-114
+      sink_store_lik(sink, out, p, (N == 0) ? 1.0f : score, n, write_beam_defaults);
+    }
+  }
+  if (stats)
+  {
+    const uint32_t r = warp_sum_u32(st_rows), q = warp_sum_u32(st_pts);
+    if (lane == 0)
+    {
+      atomicAdd(stats + 0, static_cast<unsigned long long>(r));
+      atomicAdd(stats + 1, static_cast<unsigned long long>(q));
+    }
+  }
+}
+
+// --------------------------------------------------------------------------------------------
 // Field-mode likelihood kernel (opt-in, mcl3dl_field_mode; device_funcs.cuh: FieldDev): same mapping and reductions as
 // lik_kernel_nf, but an eval is the transform plus ONE 32-byte gather (the 8 corner distances of its lattice cell) and a
 // trilinear blend — BASELINE.json north_star's literal kernel.  Its scores deviate from the reference's exact
