@@ -11,6 +11,7 @@
 #include <cmath>
 #include <stdint.h>
 
+#include "../../include/mcl3dl_b200.h"
 #include "device_math.cuh"
 
 // MCL3DL_NEAR_BITS=1 (default) compiles the near-field screens below into the searches; -DMCL3DL_NEAR_BITS=0 builds
@@ -289,6 +290,17 @@ __device__ __forceinline__ float nn_dist2(const NnGridDev& g, const LikDev& lp, 
   return best;
 }
 
+// likelihood.cpp:128-133: the contribution of a neighbour at distance d (below match_dist_min); false when it does not
+// count (d beyond match_dist_min after the flat zone)
+__device__ __forceinline__ bool lik_term(float d, const LikDev& lp, float& contribution)
+{
+  const float dist = fsub(lp.match_dist_min, fmaxf(d, lp.match_dist_flat));
+  if (dist < 0.0f)
+    return false;
+  contribution = fmul(dist, lp.match_weight);
+  return true;
+}
+
 // --------------------------------------------------------------------------------------------
 __device__ __forceinline__ int dda_to_index(float v, float mn, double grid)
 {
@@ -492,6 +504,20 @@ __device__ __forceinline__ int cast_ray(const DdaGridDev& g, const F3& b, const 
       st = dda_test_cell(g, r, n_occ, n_tested);
   }
   return st;
+}
+
+// beam.cpp:146-152: the same factor multiplied in sequentially, then the floor; 1 for an empty scan (beam.cpp:130-133)
+__device__ __forceinline__ float beam_score(uint32_t n_short, uint32_t n_long, int N, const DdaGridDev& g)
+{
+  float score = 1.0f;
+  if (N > 0)
+  {
+    const uint32_t k = n_short + (g.short_only ? 0u : n_long);
+    for (uint32_t i = 0; i < k; ++i) score = fmul(score, g.beam_likelihood);
+    if (score < g.beam_likelihood_min)
+      score = g.beam_likelihood_min;
+  }
+  return score;
 }
 
 // 1-NN within a radius with the index of the winner (ChunkedKdtree::radiusSearch(p, r, id, d2, 1)); ties go to
@@ -987,6 +1013,20 @@ __device__ __forceinline__ F3 ray_origin(const F3& pos, const Q4& q_raw, const f
   begin.y = fadd(pos.y, ro.y);
   begin.z = fadd(pos.z, ro.z);
   return begin;
+}
+
+// a particle's position and raw (not normalised) rotation: the two 16-byte halves of mcl3dl_pose
+__device__ __forceinline__ void load_pose(const mcl3dl_pose* pose, F3& pos, Q4& q)
+{
+  const float4 a = __ldg(reinterpret_cast<const float4*>(pose));
+  const float4 b = __ldg(reinterpret_cast<const float4*>(pose) + 1);
+  pos.x = a.x;
+  pos.y = a.y;
+  pos.z = a.z;
+  q.x = b.x;
+  q.y = b.y;
+  q.z = b.z;
+  q.w = b.w;
 }
 
 }  // namespace mcl3dl

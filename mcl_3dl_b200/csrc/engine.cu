@@ -10,6 +10,7 @@
 #include <cstring>
 #include <limits>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include <cub/device/device_radix_sort.cuh>
@@ -434,10 +435,9 @@ struct mcl3dl_engine
   int beam_dq_ppl = 0;  // MCL3DL_BEAM_DQ_PPL: rays per item (0 = chosen from the job size)
   int lik_share = 4;  // CTA slots per SM the likelihood kernel takes while the beam kernel runs next to it (MCL3DL_LIK_SHARE)
   int nnf_kd_r2 = 1;  // MCL3DL_NNF_KD_R2=0: the NN field also covers the KD-tree raycaster's second search radius
-  int nnf = 1;  // stage the NN field (exact per-voxel candidate lists) and use lik_kernel_nf; MCL3DL_NNF=0: the CSR window kernels
+  int nnf = 1;  // stage the NN field (exact per-voxel candidate lists) and use lik_kernel_nf*; MCL3DL_NNF=0: lik_kernel_wi
   size_t nnf_max_bytes = size_t(32) << 30;  // MCL3DL_NNF_MAX_MB: directory + candidates above this -> no field
   uint64_t nnf_bytes = 0, nnf_cands = 0, nnf_overflow_cells = 0, nnf_wide_cells = 0;
-  int mapping = 1;  // 1 = tuned kernels (lik_kernel_wi + beam_kernel_pl); 0 = the plain group kernels (MCL3DL_MAPPING=group)
   // page-locked blocks handed to the caller by mcl3dl_host_alloc: pose / record arrays that live in one of them are
   // DMA-ed (or, small updates, written by the kernels) in place instead of going through the engine's staging block
   std::vector<std::pair<char*, size_t>> host_blocks;
@@ -526,6 +526,17 @@ int pick_tpp(size_t P, size_t N, int sm_count)
   return tpp;
 }
 
+// launch(std::integral_constant<int, TPP>()) for the lanes per particle `tpp` chosen at run time: a power of two from
+// LO to kBlockThreads, the kernels' template instances
+template <int LO, typename F>
+int with_tpp(int tpp, F&& launch)
+{
+  if constexpr (LO < kBlockThreads)
+    if (tpp > LO)
+      return with_tpp<2 * LO>(tpp, launch);
+  return launch(std::integral_constant<int, LO>());
+}
+
 // cudaFuncSetAttribute is a driver call: opt each kernel instantiation in to the large dynamic shared memory
 // size once per device instead of on every launch.
 template <typename K>
@@ -541,62 +552,24 @@ int opt_in_smem(mcl3dl_engine* eng, DeviceCtx& c, K kernel, int bytes)
   return MCL3DL_OK;
 }
 
+// CSR-window likelihood kernel (no NN field staged)
 template <int TPP>
-int launch_lik_t(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_pose* poses, int P, const float4* scan, int N,
-                 mcl3dl_result* out, int beam_defaults, cudaStream_t st, const RecordSink& sink)
+int launch_lik_wi_t(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_pose* poses, int P, const float4* scan, int N,
+                    mcl3dl_result* out, int beam_defaults, cudaStream_t st, const RecordSink& sink)
 {
   constexpr int PPB = kBlockThreads / TPP;
   const int groups = (P + PPB - 1) / PPB;
   const int grid = std::max(1, std::min(groups, c.sm_count * 8));
   const size_t bytes = static_cast<size_t>(N) * 16;
-  if (eng->mapping != 0)
-  {
-    if (bytes <= static_cast<size_t>(kMaxStagedSorted))
-    {
-      if (int rc = opt_in_smem(eng, c, lik_kernel_wi<TPP, true>, kMaxStagedSorted)) return rc;
-      lik_kernel_wi<TPP, true><<<grid, kBlockThreads, bytes, st>>>(poses, P, scan, N, c.nn, eng->likdev, out, beam_defaults, c.stats_ptr(), sink);
-    }
-    else
-    {
-      lik_kernel_wi<TPP, false><<<grid, kBlockThreads, 0, st>>>(poses, P, scan, N, c.nn, eng->likdev, out, beam_defaults, c.stats_ptr(), sink);
-    }
-  }
-  else if (bytes <= static_cast<size_t>(kMaxStagedBytes))
-  {
-    if (int rc = opt_in_smem(eng, c, lik_kernel<TPP, true>, kMaxStagedBytes)) return rc;
-    lik_kernel<TPP, true><<<grid, kBlockThreads, bytes, st>>>(poses, P, scan, N, c.nn, eng->likdev, out, beam_defaults, c.stats_ptr(), sink);
-  }
-  else
-  {
-    lik_kernel<TPP, false><<<grid, kBlockThreads, 0, st>>>(poses, P, scan, N, c.nn, eng->likdev, out, beam_defaults, c.stats_ptr(), sink);
-  }
+  const bool staged = bytes <= static_cast<size_t>(kMaxStagedSorted);
+  const auto kernel = staged ? lik_kernel_wi<TPP, true> : lik_kernel_wi<TPP, false>;
+  if (staged)
+    if (int rc = opt_in_smem(eng, c, kernel, kMaxStagedSorted)) return rc;
+  kernel<<<grid, kBlockThreads, staged ? bytes : 0, st>>>(poses, P, scan, N, c.nn, eng->likdev, out, beam_defaults, c.stats_ptr(), sink);
   CK(cudaGetLastError());
   eng->launches++;
   return MCL3DL_OK;
 }
-
-template <int TPP>
-int launch_beam_t(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_pose* poses, int P, const float4* scan, int N,
-                  const float* origins, mcl3dl_result* out, uint8_t* status, int lik_defaults, cudaStream_t st, const RecordSink& sink)
-{
-  constexpr int PPB = kBlockThreads / TPP;
-  const int groups = (P + PPB - 1) / PPB;
-  const int grid = std::max(1, std::min(groups, c.sm_count * 8));
-  const size_t bytes = static_cast<size_t>(N) * 16;
-  if (bytes <= static_cast<size_t>(kMaxStagedBytes))
-  {
-    if (int rc = opt_in_smem(eng, c, beam_kernel<TPP, true>, kMaxStagedBytes)) return rc;
-    beam_kernel<TPP, true><<<grid, kBlockThreads, bytes, st>>>(poses, P, scan, N, origins, c.dda, out, status, lik_defaults, c.stats_ptr(), sink);
-  }
-  else
-  {
-    beam_kernel<TPP, false><<<grid, kBlockThreads, 0, st>>>(poses, P, scan, N, origins, c.dda, out, status, lik_defaults, c.stats_ptr(), sink);
-  }
-  CK(cudaGetLastError());
-  eng->launches++;
-  return MCL3DL_OK;
-}
-
 
 // ---- NN-field likelihood kernel: lanes per particle, staging and grid (kernels.cuh: lik_kernel_nf)
 constexpr int kNfCtasPerSm = MCL3DL_NF_MINB;
@@ -612,12 +585,6 @@ int pick_tpp_nf(size_t P, size_t N, int sm_count)
   while (tpp < kBlockThreads && static_cast<size_t>(tpp) < N && ctas(tpp) * 2 <= static_cast<size_t>(sm_count)) tpp *= 2;
   // a grid a little larger than the resident slots would run a mostly empty second wave: fewer, longer CTAs instead
   while (tpp > 8 && ctas(tpp) > slots && ctas(tpp) < 2 * slots) tpp /= 2;
-  if (const char* v = std::getenv("MCL3DL_NF_TPP"))  // experiments
-  {
-    const int t = std::atoi(v);
-    if (t == 8 || t == 16 || t == 32 || t == 64 || t == 128 || t == 256)
-      tpp = t;
-  }
   return tpp;
 }
 
@@ -635,22 +602,12 @@ int launch_lik_nf_t(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_pose* poses, 
   const size_t bytes = static_cast<size_t>(N) * 16;
   const bool ovf = eng->nnf_overflow_cells != 0;
   // the tile pays when several particles of the CTA (or several loop trips) read it; otherwise the scan comes from L2
-  bool staged = bytes <= static_cast<size_t>(kMaxStagedBytes) / 2 && (PPB >= 4 || groups > grid);
-  if (const char* v = std::getenv("MCL3DL_NF_STAGE"))  // experiments
-    staged = bytes <= static_cast<size_t>(kMaxStagedBytes) / 2 && std::atoi(v) != 0;
-#define NF_LAUNCH(S, O)                                                                                                    \
-  do                                                                                                                       \
-  {                                                                                                                        \
-    if (S)                                                                                                                 \
-      if (int rc = opt_in_smem(eng, c, lik_kernel_nf<TPP, S, O>, kMaxStagedBytes / 2)) return rc;                          \
-    lik_kernel_nf<TPP, S, O><<<grid, kBlockThreads, (S) ? bytes : 0, st>>>(poses, P, scan, N, c.nn, eng->likdev, out,       \
-                                                                           beam_defaults, c.stats_ptr(), sink);            \
-  } while (0)
-  if (staged && ovf) NF_LAUNCH(true, true);
-  else if (staged) NF_LAUNCH(true, false);
-  else if (ovf) NF_LAUNCH(false, true);
-  else NF_LAUNCH(false, false);
-#undef NF_LAUNCH
+  const bool staged = bytes <= static_cast<size_t>(kMaxStagedBytes) / 2 && (PPB >= 4 || groups > grid);
+  const auto kernel = staged ? (ovf ? lik_kernel_nf<TPP, true, true> : lik_kernel_nf<TPP, true, false>)
+                             : (ovf ? lik_kernel_nf<TPP, false, true> : lik_kernel_nf<TPP, false, false>);
+  if (staged)
+    if (int rc = opt_in_smem(eng, c, kernel, kMaxStagedBytes / 2)) return rc;
+  kernel<<<grid, kBlockThreads, staged ? bytes : 0, st>>>(poses, P, scan, N, c.nn, eng->likdev, out, beam_defaults, c.stats_ptr(), sink);
   CK(cudaGetLastError());
   eng->launches++;
   return MCL3DL_OK;
@@ -670,14 +627,9 @@ int launch_lik_nf_pm(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_pose* poses,
     CK(cudaMemsetAsync(c.d_lacc.p, 0, c.d_lacc.cap, st));
   }
   auto* acc = static_cast<unsigned long long*>(c.d_lacc.p);
-#define PM_LAUNCH(O)                                                                                                       \
-  lik_kernel_nf_pm<O><<<blocks * sh.n_slices, kBlockThreads, 0, st>>>(poses, P, scan, N, c.nn, eng->likdev, out,           \
-                                                                      beam_defaults, c.stats_ptr(), sink, sh, acc)
-  if (eng->nnf_overflow_cells != 0)
-    PM_LAUNCH(true);
-  else
-    PM_LAUNCH(false);
-#undef PM_LAUNCH
+  const auto kernel = eng->nnf_overflow_cells != 0 ? lik_kernel_nf_pm<true> : lik_kernel_nf_pm<false>;
+  kernel<<<blocks * sh.n_slices, kBlockThreads, 0, st>>>(poses, P, scan, N, c.nn, eng->likdev, out, beam_defaults,
+                                                         c.stats_ptr(), sink, sh, acc);
   CK(cudaGetLastError());
   eng->launches++;
   return MCL3DL_OK;
@@ -697,15 +649,9 @@ int launch_lik_nf(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_pose* poses, si
     if (sh.ok)
       return launch_lik_nf_pm(eng, c, poses, p, s4, n, out, beam_defaults, st, sink, blocks, sh);
   }
-  switch (pick_tpp_nf(P, N, c.sm_count))
-  {
-    case 8: return launch_lik_nf_t<8>(eng, c, poses, p, s4, n, out, beam_defaults, st, sink);
-    case 16: return launch_lik_nf_t<16>(eng, c, poses, p, s4, n, out, beam_defaults, st, sink);
-    case 32: return launch_lik_nf_t<32>(eng, c, poses, p, s4, n, out, beam_defaults, st, sink);
-    case 64: return launch_lik_nf_t<64>(eng, c, poses, p, s4, n, out, beam_defaults, st, sink);
-    case 128: return launch_lik_nf_t<128>(eng, c, poses, p, s4, n, out, beam_defaults, st, sink);
-    default: return launch_lik_nf_t<256>(eng, c, poses, p, s4, n, out, beam_defaults, st, sink);
-  }
+  return with_tpp<8>(pick_tpp_nf(P, N, c.sm_count), [&](auto tpp) {
+    return launch_lik_nf_t<decltype(tpp)::value>(eng, c, poses, p, s4, n, out, beam_defaults, st, sink);
+  });
 }
 
 // ---- field mode: staging and launch
@@ -797,15 +743,9 @@ int launch_lik_field(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_pose* poses,
 {
   const float4* s4 = reinterpret_cast<const float4*>(scan);
   const int p = static_cast<int>(P), n = static_cast<int>(N);
-  switch (pick_tpp_nf(P, N, c.sm_count))
-  {
-    case 8: return launch_lik_field_t<8>(eng, c, poses, p, s4, n, out, beam_defaults, st, sink);
-    case 16: return launch_lik_field_t<16>(eng, c, poses, p, s4, n, out, beam_defaults, st, sink);
-    case 32: return launch_lik_field_t<32>(eng, c, poses, p, s4, n, out, beam_defaults, st, sink);
-    case 64: return launch_lik_field_t<64>(eng, c, poses, p, s4, n, out, beam_defaults, st, sink);
-    case 128: return launch_lik_field_t<128>(eng, c, poses, p, s4, n, out, beam_defaults, st, sink);
-    default: return launch_lik_field_t<256>(eng, c, poses, p, s4, n, out, beam_defaults, st, sink);
-  }
+  return with_tpp<8>(pick_tpp_nf(P, N, c.sm_count), [&](auto tpp) {
+    return launch_lik_field_t<decltype(tpp)::value>(eng, c, poses, p, s4, n, out, beam_defaults, st, sink);
+  });
 }
 
 PlShape pick_pl_shape(size_t P, size_t N, int sm_count)
@@ -860,15 +800,10 @@ int launch_beam_pl(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_pose* poses, s
   const int gpc = kPlWarps / sh.cpg;
   const int groups = static_cast<int>(((P + 31) / 32 + gpc - 1) / gpc);
   const size_t smem = static_cast<size_t>(kPlWarps) * sh.ppl * 16;
-#define PL_LAUNCH(KD)                                                                                                             \
-  beam_kernel_pl<KD><<<groups * sh.cb, kBlockThreads, smem, st>>>(                                                                \
-      poses, static_cast<int>(P), reinterpret_cast<const float4*>(scan), static_cast<int>(N), origins, c.dda, c.kd, c.nn, out, status, \
-      lik_defaults, c.stats_ptr(), sh, static_cast<uint32_t*>(c.d_partial.p), static_cast<unsigned int*>(c.d_tickets.p), sink)
-  if (eng->beam.use_raycast_using_dda)
-    PL_LAUNCH(false);
-  else
-    PL_LAUNCH(true);
-#undef PL_LAUNCH
+  const auto kernel = eng->beam.use_raycast_using_dda ? beam_kernel_pl<false> : beam_kernel_pl<true>;
+  kernel<<<groups * sh.cb, kBlockThreads, smem, st>>>(
+      poses, static_cast<int>(P), reinterpret_cast<const float4*>(scan), static_cast<int>(N), origins, c.dda, c.kd, c.nn, out, status,
+      lik_defaults, c.stats_ptr(), sh, static_cast<uint32_t*>(c.d_partial.p), static_cast<unsigned int*>(c.d_tickets.p), sink);
   CK(cudaGetLastError());
   eng->launches++;
   return MCL3DL_OK;
@@ -904,17 +839,11 @@ int launch_beam_dq(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_pose* poses, s
       return rc;
     CK(cudaMemsetAsync(c.d_queue.p, 0, 256, st));
   }
-#define DQ_LAUNCH(KD)                                                                                                              \
-  beam_kernel_dq<KD><<<grid, kBlockThreads, 0, st>>>(poses, static_cast<int>(P), reinterpret_cast<const float4*>(scan),             \
-                                                     static_cast<int>(N), origins, c.dda, c.kd, c.nn, out, status, lik_defaults,   \
-                                                     c.stats_ptr(), static_cast<int>(ppl), n_chunks,                               \
-                                                     static_cast<uint32_t*>(c.d_tally.p), static_cast<unsigned int*>(c.d_tickets.p), \
-                                                     static_cast<unsigned int*>(c.d_queue.p), sink)
-  if (eng->beam.use_raycast_using_dda)
-    DQ_LAUNCH(false);
-  else
-    DQ_LAUNCH(true);
-#undef DQ_LAUNCH
+  const auto kernel = eng->beam.use_raycast_using_dda ? beam_kernel_dq<false> : beam_kernel_dq<true>;
+  kernel<<<grid, kBlockThreads, 0, st>>>(poses, static_cast<int>(P), reinterpret_cast<const float4*>(scan), static_cast<int>(N),
+                                         origins, c.dda, c.kd, c.nn, out, status, lik_defaults, c.stats_ptr(),
+                                         static_cast<int>(ppl), n_chunks, static_cast<uint32_t*>(c.d_tally.p),
+                                         static_cast<unsigned int*>(c.d_tickets.p), static_cast<unsigned int*>(c.d_queue.p), sink);
   CK(cudaGetLastError());
   eng->launches++;
   return MCL3DL_OK;
@@ -925,34 +854,22 @@ int launch_lik(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_pose* poses, size_
 {
   if (eng->field_mode && c.nn.fld.cells)
     return launch_lik_field(eng, c, poses, P, scan, N, out, beam_defaults, st, sink);
-  if (eng->mapping != 0 && c.nn.field.dir)
+  if (c.nn.field.dir)
     return launch_lik_nf(eng, c, poses, P, scan, N, out, beam_defaults, st, sink);
   const float4* s4 = reinterpret_cast<const float4*>(scan);
-  switch (pick_tpp(P, N, c.sm_count))
-  {
-    case 32: return launch_lik_t<32>(eng, c, poses, static_cast<int>(P), s4, static_cast<int>(N), out, beam_defaults, st, sink);
-    case 64: return launch_lik_t<64>(eng, c, poses, static_cast<int>(P), s4, static_cast<int>(N), out, beam_defaults, st, sink);
-    case 128: return launch_lik_t<128>(eng, c, poses, static_cast<int>(P), s4, static_cast<int>(N), out, beam_defaults, st, sink);
-    default: return launch_lik_t<256>(eng, c, poses, static_cast<int>(P), s4, static_cast<int>(N), out, beam_defaults, st, sink);
-  }
+  const int p = static_cast<int>(P), n = static_cast<int>(N);
+  return with_tpp<32>(pick_tpp(P, N, c.sm_count), [&](auto tpp) {
+    return launch_lik_wi_t<decltype(tpp)::value>(eng, c, poses, p, s4, n, out, beam_defaults, st, sink);
+  });
 }
 
 int launch_beam(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_pose* poses, size_t P, const mcl3dl_point* scan, size_t N,
                 const float* origins, int n_origins, mcl3dl_result* out, uint8_t* status, int lik_defaults, cudaStream_t st,
                 const RecordSink& sink)
 {
-  if (eng->mapping != 0 && (eng->beam_dq == 1 || (eng->beam_dq == 2 && P * N >= 262144)))
+  if (eng->beam_dq == 1 || (eng->beam_dq == 2 && P * N >= 262144))
     return launch_beam_dq(eng, c, poses, P, scan, N, origins, out, status, lik_defaults, st, sink);
-  if (eng->mapping != 0 || !eng->beam.use_raycast_using_dda)  // the KD-tree caster exists in the pl kernel only
-    return launch_beam_pl(eng, c, poses, P, scan, N, origins, n_origins, out, status, lik_defaults, st, sink);
-  const float4* s4 = reinterpret_cast<const float4*>(scan);
-  switch (pick_tpp(P, N, c.sm_count))
-  {
-    case 32: return launch_beam_t<32>(eng, c, poses, static_cast<int>(P), s4, static_cast<int>(N), origins, out, status, lik_defaults, st, sink);
-    case 64: return launch_beam_t<64>(eng, c, poses, static_cast<int>(P), s4, static_cast<int>(N), origins, out, status, lik_defaults, st, sink);
-    case 128: return launch_beam_t<128>(eng, c, poses, static_cast<int>(P), s4, static_cast<int>(N), origins, out, status, lik_defaults, st, sink);
-    default: return launch_beam_t<256>(eng, c, poses, static_cast<int>(P), s4, static_cast<int>(N), origins, out, status, lik_defaults, st, sink);
-  }
+  return launch_beam_pl(eng, c, poses, P, scan, N, origins, n_origins, out, status, lik_defaults, st, sink);
 }
 
 void derive_lik(mcl3dl_engine* eng)
@@ -1321,7 +1238,7 @@ int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_point* h_
         radius = std::max(radius, eng->nnf_kd_r2 ? tmp.r2_pad : tmp.r1_pad);
       }
       g.field = NnFieldDev{};
-      if (eng->nnf && eng->mapping != 0)
+      if (eng->nnf)
         CKB(build_nn_field(eng, c, st, pts, n32, g, radius, sc_min, sc_max));
     }
     // window table of the CSR-window kernel (lik_kernel_wi): only when the field is not staged
@@ -1538,8 +1455,6 @@ int mcl3dl_create(mcl3dl_engine** out, const int* device_ids, int n_devices)
     eng->nnf_max_bytes = static_cast<size_t>(std::max(std::atol(v), 1L)) << 20;
   if (const char* o = std::getenv("MCL3DL_OVERLAP"))
     eng->overlap = std::atoi(o) != 0;
-  if (const char* m = std::getenv("MCL3DL_MAPPING"))
-    eng->mapping = (std::strcmp(m, "group") == 0) ? 0 : 1;
   eng->devs.resize(n_devices);
   for (int i = 0; i < n_devices; ++i)
   {

@@ -1,15 +1,20 @@
-// kernels.cuh — the two hot kernels of the measurement update, hand-written for sm_90a (H100).
+// kernels.cuh — the kernels of the measurement update, hand-written for sm_90a (H100).
 //
-//   lik_kernel   LidarMeasurementModelLikelihood::measure  (src/lidar_measurement_model_likelihood.cpp:105-139)
-//                + ChunkedKdtree::radiusSearch semantics   (include/mcl_3dl/chunked_kdtree.h:217-237)
-//   beam_kernel  LidarMeasurementModelBeam::measure / getBeamStatus (src/lidar_measurement_model_beam.cpp:124-192)
-//                + RaycastUsingDDA                          (include/mcl_3dl/raycasts/raycast_using_dda.h:66-270)
+//   likelihood model  LidarMeasurementModelLikelihood::measure (src/lidar_measurement_model_likelihood.cpp:105-139)
+//                     + ChunkedKdtree::radiusSearch semantics (include/mcl_3dl/chunked_kdtree.h:217-237):
+//       lik_kernel_nf_pm  NN field, point-major: a lane owns a particle, a warp 32 particles on one scan point
+//       lik_kernel_nf     NN field, particle-major: TPP lanes (8 .. 256) own a particle and stride its scan points
+//       lik_kernel_wi     no NN field staged: the CSR window search, particle-major (TPP >= 32)
+//       lik_kernel_field  the opt-in, inexact field mode
+//   beam model        LidarMeasurementModelBeam::measure / getBeamStatus (src/lidar_measurement_model_beam.cpp:124-192)
+//                     + RaycastUsingDDA / RaycastUsingKDTree:
+//       beam_kernel_pl    a lane owns a particle, a warp casts one chunk of rays; fixed CTA mapping
+//       beam_kernel_dq    the same lanes, (particle group, ray chunk) items pulled from a global queue
+//   weight_kernel / normalize_kernel*: the fused weight update; exchange_signal_kernel: the multi-GPU record exchange.
 //
-// Layout: particle-major.  A group of TPP threads (1..8 warps) owns one particle; its lanes stride
-// the sampled scan points, which the CTA stages once into shared memory with a TMA bulk copy
-// (cp.async.bulk + mbarrier).  Per-particle partials are reduced with warp shuffles and a fixed-order
-// shared-memory pass, so results are deterministic run to run.  No tensor cores: there is no dense
-// contraction anywhere on this path (HBM/L2 gather bound).
+// The per-thread arithmetic (transform, searches, ray casts, likelihood term, beam score) lives in device_funcs.cuh,
+// which tests/hostsim also compiles for the host.  Every reduction has a fixed order or sums integers, so results are
+// deterministic run to run.  No tensor cores: there is no dense contraction anywhere on this path (HBM/L2 gather bound).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -101,8 +106,9 @@ __device__ __forceinline__ void sink_store_beam(const RecordSink& s, mcl3dl_resu
 }
 
 // --------------------------------------------------------------------------------------------
-// Stage `bytes` (multiple of 16) from global to shared with one TMA bulk copy; all threads wait.
-__device__ __forceinline__ void stage_tile(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar)
+// Stage `bytes` (multiple of 16) from global to shared with one TMA bulk copy (cp.async.bulk + mbarrier): thread 0
+// issues it, every thread waits for it.  stage_issue early and stage_wait late overlap the copy with other work.
+__device__ __forceinline__ void stage_issue(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar)
 {
   const uint32_t bar_a = static_cast<uint32_t>(__cvta_generic_to_shared(bar));
   const uint32_t dst_a = static_cast<uint32_t>(__cvta_generic_to_shared(smem_dst));
@@ -110,16 +116,17 @@ __device__ __forceinline__ void stage_tile(void* smem_dst, const void* gsrc, uin
   {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar_a));
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  if (threadIdx.x == 0)
-  {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_a), "r"(bytes) : "memory");
     asm volatile(
         "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst_a),
         "l"(gsrc), "r"(bytes), "r"(bar_a)
         : "memory");
   }
+}
+__device__ __forceinline__ void stage_wait(uint64_t* bar)
+{
+  const uint32_t bar_a = static_cast<uint32_t>(__cvta_generic_to_shared(bar));
+  __syncthreads();  // the barrier's initialisation (thread 0) is visible to every waiter
   uint32_t done = 0;
   while (!done)
   {
@@ -135,135 +142,72 @@ __device__ __forceinline__ void stage_tile(void* smem_dst, const void* gsrc, uin
   }
 }
 
-// Fixed-order reduction of one value per thread over the TPP threads that own a particle.
-// red must hold kBlockThreads/32 entries per quantity.
-template <int TPP>
-__device__ __forceinline__ void group_reduce(float& f, uint32_t& a, uint32_t& b, uint32_t& c, float* red_f,
-                                             uint32_t* red_u)
+__device__ __forceinline__ void stage_tile(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar)
 {
-  f = warp_sum(f);
-  a = warp_sum_u32(a);
-  b = warp_sum_u32(b);
-  c = warp_sum_u32(c);
-  if (TPP > 32)
+  stage_issue(smem_dst, gsrc, bytes, bar);
+  stage_wait(bar);
+}
+
+// Fold one value per lane over the TPP lanes that own a particle, in a fixed order.  TPP < 32: the particle's lanes
+// are an aligned sub-group of the warp (xor-shuffle tree).  TPP >= 32: the warp's xor-shuffle tree, then the particle's
+// warps in order through shared memory (red_f / red_u: one entry per warp).
+template <int TPP>
+__device__ __forceinline__ void particle_reduce(float& f, uint32_t& a, float* red_f, uint32_t* red_u)
+{
+  if (TPP >= 32)
   {
-    constexpr int WPP = TPP / 32;
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
-    __syncthreads();
-    if (lane == 0)
+    f = warp_sum(f);
+    a = warp_sum_u32(a);
+    if (TPP > 32)
     {
-      red_f[warp] = f;
-      red_u[warp * 3 + 0] = a;
-      red_u[warp * 3 + 1] = b;
-      red_u[warp * 3 + 2] = c;
-    }
-    __syncthreads();
-    const int w0 = (warp / WPP) * WPP;
-    float sf = red_f[w0];
-    uint32_t sa = red_u[w0 * 3], sb = red_u[w0 * 3 + 1], sc = red_u[w0 * 3 + 2];
+      constexpr int WPP = TPP / 32;
+      const int warp = threadIdx.x >> 5;
+      __syncthreads();
+      if ((threadIdx.x & 31) == 0)
+      {
+        red_f[warp] = f;
+        red_u[warp] = a;
+      }
+      __syncthreads();
+      const int w0 = (warp / WPP) * WPP;
+      float sf = red_f[w0];
+      uint32_t sa = red_u[w0];
 #pragma unroll
-    for (int k = 1; k < WPP; ++k)
-    {
-      sf = fadd(sf, red_f[w0 + k]);
-      sa += red_u[(w0 + k) * 3];
-      sb += red_u[(w0 + k) * 3 + 1];
-      sc += red_u[(w0 + k) * 3 + 2];
+      for (int k = 1; k < WPP; ++k)
+      {
+        sf = fadd(sf, red_f[w0 + k]);
+        sa += red_u[w0 + k];
+      }
+      f = sf;
+      a = sa;
     }
-    f = sf;
-    a = sa;
-    b = sb;
-    c = sc;
+  }
+  else
+  {
+#pragma unroll
+    for (int o = TPP / 2; o > 0; o >>= 1)
+    {
+      f = fadd(f, __shfl_xor_sync(0xffffffffu, f, o));
+      a += __shfl_xor_sync(0xffffffffu, a, o);
+    }
   }
 }
 
-template <int TPP, bool STAGED>
-__global__ void __launch_bounds__(kBlockThreads)
-    lik_kernel(const mcl3dl_pose* __restrict__ poses, int P, const float4* __restrict__ scan, int N, NnGridDev g,
-               LikDev lp, mcl3dl_result* __restrict__ out, int write_beam_defaults,
-               unsigned long long* __restrict__ stats, RecordSink sink)
+// add one per-thread work counter to stats[i] (SURVEY 5: the node's status path wants evals/steps): a warp sum and
+// one atomic per warp
+__device__ __forceinline__ void stats_add(unsigned long long* stats, int i, uint32_t v)
 {
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  __shared__ uint64_t bar;
-  __shared__ float red_f[kBlockThreads / 32];
-  __shared__ uint32_t red_u[3 * kBlockThreads / 32];
-  const float4* pts = scan;
-  if (STAGED && N > 0)
-  {
-    stage_tile(smem_raw, scan, static_cast<uint32_t>(N) * 16u, &bar);
-    pts = reinterpret_cast<const float4*>(smem_raw);
-  }
-  constexpr int PPB = kBlockThreads / TPP;
-  const int sub = threadIdx.x / TPP;
-  const int l = threadIdx.x % TPP;
-  const int n_groups = (P + PPB - 1) / PPB;
-  uint32_t st_rows = 0, st_pts = 0;
-  for (int grp = blockIdx.x; grp < n_groups; grp += gridDim.x)
-  {
-    const int p = grp * PPB + sub;
-    const bool live = p < P;
-    float score = 0.0f;
-    uint32_t cnt = 0, z0 = 0, z1 = 0;
-    if (live)
-    {
-      const float4 a = __ldg(reinterpret_cast<const float4*>(poses + p));
-      const float4 b = __ldg(reinterpret_cast<const float4*>(poses + p) + 1);
-      F3 pos;
-      pos.x = a.x;
-      pos.y = a.y;
-      pos.z = a.z;
-      Q4 q;
-      q.x = b.x;
-      q.y = b.y;
-      q.z = b.z;
-      q.w = b.w;
-      const Q4 rn = qnormalized(q);  // state_6dof.h:217
-      for (int j = l; j < N; j += TPP)
-      {
-        const float4 sp = pts[j];
-        F3 v;
-        v.x = sp.x;
-        v.y = sp.y;
-        v.z = sp.z;
-        const F3 t = transform_point(rn, pos, v);
-        // PointRepresentation::vectorize with rescale values (mcl_3dl.cpp:1270)
-        const float d2 = nn_dist2(g, lp, fmul(t.x, g.wx), fmul(t.y, g.wy), fmul(t.z, g.wz), st_rows, st_pts);
-        if (d2 < lp.r2)
-        {
-          // likelihood.cpp:128-133
-          const float dist = fsub(lp.match_dist_min, fmaxf(__fsqrt_rn(d2), lp.match_dist_flat));
-          if (!(dist < 0.0f))
-          {
-            score = fadd(score, fmul(dist, lp.match_weight));
-            cnt++;
-          }
-        }
-      }
-    }
-    group_reduce<TPP>(score, cnt, z0, z1, red_f, red_u);
-    if (live && l == 0)  // empty scan -> LidarMeasurementResult(1, 0), likelihood.cpp:111-114
-      sink_store_lik(sink, out, p, (N == 0) ? 1.0f : score, cnt, write_beam_defaults);
-  }
-  if (stats)
-  {
-    // per-call counters (SURVEY 5: the node's status path wants evals/steps): index rows read, map points scanned
-    const uint32_t r = warp_sum_u32(st_rows), q = warp_sum_u32(st_pts);
-    if ((threadIdx.x & 31) == 0)
-    {
-      atomicAdd(stats + 0, static_cast<unsigned long long>(r));
-      atomicAdd(stats + 1, static_cast<unsigned long long>(q));
-    }
-  }
+  v = warp_sum_u32(v);
+  if ((threadIdx.x & 31) == 0)
+    atomicAdd(stats + i, static_cast<unsigned long long>(v));
 }
 
 // --------------------------------------------------------------------------------------------
-// Warp-item likelihood kernel.
+// Warp-item likelihood kernel (no NN field staged: MCL3DL_NNF=0, or a field above MCL3DL_NNF_MAX_MB).
 //
-// Profiled, the straightforward kernel above runs with few of its 32 lanes active and
-// ~70 % of the stall samples sit on the map-point loads of the inner loop, which runs with ~5 live
-// lanes — an eval next to a surface scans ~30 map points, one that misses scans ~2, and every lane
-// waits for the slowest one, one dependent load at a time.  Here each warp works on 32 evals at a time in two
-// warp-synchronous phases, no CTA barrier:
+// A kernel whose lanes each walk their own eval's window runs with few of its 32 lanes active: an eval next to a
+// surface scans ~30 map points, one that misses scans ~2, and every lane waits for the slowest one, one dependent load
+// at a time.  Here each warp works on 32 evals at a time in two warp-synchronous phases, no CTA barrier:
 //   phase 1 (lane = eval, uniform): transform, window, ALL row bounds of the <=3x3 window issued back
 //            to back (18 independent loads in flight per lane); the non-empty [s0,s1) runs go to
 //            this warp's shared-memory slab;
@@ -272,8 +216,8 @@ __global__ void __launch_bounds__(kBlockThreads)
 //            lanes whose evals had nothing to scan; each item is one contiguous run of map points,
 //            read 4 at a time; minima are merged with shared-memory atomicMin on the float bits
 //            (order independent -> deterministic).
-// The eval's owner lane then adds its contribution to its running sum exactly as before, so results
-// are bit-identical to the plain kernel.  Requires cell edge > window half-width (<= 3 cells/axis).
+// The eval's owner lane then adds its contribution to its running sum in scan order.  Requires cell edge > window
+// half-width (<= 3 cells/axis).
 constexpr int kMaxWinRows = 9;
 // map points fetched per batch of an item (4 was the fastest of 1/2/4/8 on c2);
 // (before the window table) capping registers below 64 for more resident CTAs only spilled and lost
@@ -320,7 +264,7 @@ __global__ void __launch_bounds__(kBlockThreads, 4)
     const int p = grp * PPB + sub;
     const bool live = p < P;
     float score = 0.0f;
-    uint32_t cnt = 0, z0 = 0, z1 = 0;
+    uint32_t cnt = 0;
     F3 pos;
     Q4 rn;
     pos.x = pos.y = pos.z = 0.0f;
@@ -328,16 +272,8 @@ __global__ void __launch_bounds__(kBlockThreads, 4)
     rn.w = 1.0f;
     if (live)
     {
-      const float4 a = __ldg(reinterpret_cast<const float4*>(poses + p));
-      const float4 b = __ldg(reinterpret_cast<const float4*>(poses + p) + 1);
-      pos.x = a.x;
-      pos.y = a.y;
-      pos.z = a.z;
       Q4 q;
-      q.x = b.x;
-      q.y = b.y;
-      q.z = b.z;
-      q.w = b.w;
+      load_pose(poses + p, pos, q);
       rn = qnormalized(q);  // state_6dof.h:217
     }
     // a warp's 32 lanes always belong to one particle (TPP >= 32), so the trip count is warp-uniform
@@ -483,34 +419,27 @@ __global__ void __launch_bounds__(kBlockThreads, 4)
           atomicMin(&sm.best[e], __float_as_uint(best));
       }
       __syncwarp();
-      // ---------------- owner lane: likelihood.cpp:128-133
+      // ---------------- owner lane
       if (valid)
       {
         const float d2 = __uint_as_float(sm.best[lane]);
-        if (d2 < lp.r2)
+        float t;
+        if (d2 < lp.r2 && lik_term(__fsqrt_rn(d2), lp, t))
         {
-          const float dist = fsub(lp.match_dist_min, fmaxf(__fsqrt_rn(d2), lp.match_dist_flat));
-          if (!(dist < 0.0f))
-          {
-            score = fadd(score, fmul(dist, lp.match_weight));
-            cnt++;
-          }
+          score = fadd(score, t);
+          cnt++;
         }
       }
       __syncwarp();
     }
-    group_reduce<TPP>(score, cnt, z0, z1, red_f, red_u);
+    particle_reduce<TPP>(score, cnt, red_f, red_u);
     if (live && l == 0)  // empty scan -> LidarMeasurementResult(1, 0), likelihood.cpp:111-114
       sink_store_lik(sink, out, p, (N == 0) ? 1.0f : score, cnt, write_beam_defaults);
   }
   if (stats)
   {
-    const uint32_t r = warp_sum_u32(st_rows), q = warp_sum_u32(st_pts);
-    if ((threadIdx.x & 31) == 0)
-    {
-      atomicAdd(stats + 0, static_cast<unsigned long long>(r));
-      atomicAdd(stats + 1, static_cast<unsigned long long>(q));
-    }
+    stats_add(stats, 0, st_rows);
+    stats_add(stats, 1, st_pts);
   }
 }
 
@@ -537,7 +466,7 @@ __global__ void __launch_bounds__(kBlockThreads, 4)
 // Distances are sums of squares (non-negative, finite) and the best starts at r2 > 0, so the unsigned min over their
 // bit patterns is fminf over the same set in any order: the best of an eval does not depend on which lane folded what.
 // Per-lane accumulation runs in scan order (j = l, l + TPP, ...), lanes are folded by the xor-shuffle tree and warps in
-// order: deterministic, and bit-identical to lik_kernel / lik_kernel_wi whenever those run with the same TPP.
+// order: deterministic, and bit-identical to lik_kernel_wi whenever it runs with the same TPP.
 #ifndef MCL3DL_NF_U
 #define MCL3DL_NF_U 4
 #endif
@@ -555,7 +484,7 @@ constexpr int kNfSlots = 1024;
 #define MCL3DL_NF_MINB 4
 #endif
 
-// per-warp shared memory of lik_kernel_nf's phase B
+// per-warp shared memory of the NN-field kernels' candidate scan
 struct NfWarpSmem
 {
   float4 q[kNfEvals];       // query of eval e; .w = bits of (first candidate - first slot) of its list
@@ -563,82 +492,78 @@ struct NfWarpSmem
   uint8_t own[kNfSlots];    // slot -> eval, for the pass's slots
 };
 
-__device__ __forceinline__ void stage_issue(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar)
+// The candidate scan of one warp trip of the NN-field kernels (lik_kernel_nf, lik_kernel_nf_pm).  Phase A has left the
+// query of this lane's eval u (eval e = u * 32 + lane) in ws.q[e].xyz, and its candidate count c[u] (-1: overflow cell)
+// and first candidate s[u] from nnf_lookup; an eval without a query has c[u] = 0.  tot: the lane's candidates in all
+// (the sum of max(c[u], 0), counted in phase A: summed here, it costs a spill).  Returns each eval's best d^2 in d2[u]
+// (r2 when no map point is closer).  Every lane of the warp calls it: it shuffles and synchronises the whole warp.
+template <bool OVF>
+__device__ __forceinline__ void nf_warp_scan(NfWarpSmem& ws, const NnGridDev& g, const LikDev& lp, const int (&c)[kNfU],
+                                             const uint32_t (&s)[kNfU], int tot, float (&d2)[kNfU], uint32_t& st_rows,
+                                             uint32_t& st_pts)
 {
-  const uint32_t bar_a = static_cast<uint32_t>(__cvta_generic_to_shared(bar));
-  const uint32_t dst_a = static_cast<uint32_t>(__cvta_generic_to_shared(smem_dst));
-  if (threadIdx.x == 0)
-  {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar_a));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_a), "r"(bytes) : "memory");
-    asm volatile(
-        "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst_a),
-        "l"(gsrc), "r"(bytes), "r"(bar_a)
-        : "memory");
-  }
-}
-__device__ __forceinline__ void stage_wait(uint64_t* bar)
-{
-  const uint32_t bar_a = static_cast<uint32_t>(__cvta_generic_to_shared(bar));
-  __syncthreads();  // the barrier's initialisation (thread 0) is visible to every waiter
-  uint32_t done = 0;
-  while (!done)
-  {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0;\n"
-        "selp.u32 %0, 1, 0, p;\n"
-        "}\n"
-        : "=r"(done)
-        : "r"(bar_a)
-        : "memory");
-  }
-}
-
-// fold one value per lane over the TPP lanes that own a particle (TPP < 32: the particle's lanes are an aligned
-// sub-group of the warp; TPP >= 32: group_reduce's warp tree + fixed-order shared-memory pass)
-template <int TPP>
-__device__ __forceinline__ void nf_reduce(float& f, uint32_t& a, float* red_f, uint32_t* red_u)
-{
-  if (TPP >= 32)
-  {
-    // group_reduce's order for one float and one count
-    f = warp_sum(f);
-    a = warp_sum_u32(a);
-    if (TPP > 32)
-    {
-      constexpr int WPP = TPP / 32;
-      const int warp = threadIdx.x >> 5;
-      __syncthreads();
-      if ((threadIdx.x & 31) == 0)
-      {
-        red_f[warp] = f;
-        red_u[warp] = a;
-      }
-      __syncthreads();
-      const int w0 = (warp / WPP) * WPP;
-      float sf = red_f[w0];
-      uint32_t sa = red_u[w0];
+  const int lane = threadIdx.x & 31;
+  const NnFieldDev& f = g.field;
+  // ---- flatten: the lanes' lists end to end (inclusive shuffle scan of the lane totals), W slots in all
+  int incl = tot;
 #pragma unroll
-      for (int k = 1; k < WPP; ++k)
-      {
-        sf = fadd(sf, red_f[w0 + k]);
-        sa += red_u[w0 + k];
-      }
-      f = sf;
-      a = sa;
-    }
-  }
-  else
+  for (int o = 1; o < 32; o <<= 1)
   {
+    const int v = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o)
+      incl += v;
+  }
+  const int W = __shfl_sync(0xffffffffu, incl, 31);
+  int b[kNfU];
+  int base = incl - tot;
 #pragma unroll
-    for (int o = TPP / 2; o > 0; o >>= 1)
+  for (int u = 0; u < kNfU; ++u)
+  {
+    b[u] = base;
+    base += max(c[u], 0);
+    ws.q[u * 32 + lane].w = __uint_as_float(s[u] - static_cast<uint32_t>(b[u]));  // slot + .w = candidate index
+    ws.best[u * 32 + lane] = __float_as_uint(lp.r2);
+  }
+  // ---- phase B: kNfB candidates per lane in flight, folded into their evals' bests
+  for (int lo = 0; lo < W; lo += kNfSlots)
+  {
+    const int hi = min(W, lo + kNfSlots);
+#pragma unroll
+    for (int u = 0; u < kNfU; ++u) nnf_fill_owner(ws.own, lo, hi, b[u], max(c[u], 0), u * 32 + lane);
+    __syncwarp();
+    for (int k = lo + lane; k < hi; k += 32 * kNfB)
     {
-      f = fadd(f, __shfl_xor_sync(0xffffffffu, f, o));
-      a += __shfl_xor_sync(0xffffffffu, a, o);
+      int e[kNfB];
+      float4 m[kNfB];
+#pragma unroll
+      for (int v = 0; v < kNfB; ++v)
+        if (k + 32 * v < hi)
+        {
+          e[v] = ws.own[k + 32 * v - lo];
+          m[v] = __ldg(f.cand + (__float_as_uint(ws.q[e[v]].w) + static_cast<uint32_t>(k + 32 * v)));
+        }
+#pragma unroll
+      for (int v = 0; v < kNfB; ++v)
+        if (k + 32 * v < hi)
+        {
+          const float4 qe = ws.q[e[v]];
+          atomicMin(&ws.best[e[v]], __float_as_uint(nnf_cand_d2(qe.x, qe.y, qe.z, m[v])));
+        }
     }
+    __syncwarp();  // the bests are final, and the next pass may overwrite `own`
+  }
+  // ---- back to the owners
+#pragma unroll
+  for (int u = 0; u < kNfU; ++u)
+  {
+    d2[u] = __uint_as_float(ws.best[u * 32 + lane]);
+    if (OVF && c[u] < 0)  // overflow cell (raw clouds): the CSR window search
+    {
+      const float4 qu = ws.q[u * 32 + lane];
+      d2[u] = nn_dist2(g, lp, qu.x, qu.y, qu.z, st_rows, st_pts);
+    }
+    else
+      st_pts += static_cast<uint32_t>(max(c[u], 0));
   }
 }
 
@@ -677,16 +602,8 @@ __global__ void __launch_bounds__(kBlockThreads, MCL3DL_NF_MINB)
     rn.w = 1.0f;
     if (live)
     {
-      const float4 a = __ldg(reinterpret_cast<const float4*>(poses + p));
-      const float4 b = __ldg(reinterpret_cast<const float4*>(poses + p) + 1);
-      pos.x = a.x;
-      pos.y = a.y;
-      pos.z = a.z;
       Q4 q;
-      q.x = b.x;
-      q.y = b.y;
-      q.z = b.z;
-      q.w = b.w;
+      load_pose(poses + p, pos, q);
       rn = qnormalized(q);  // state_6dof.h:217
     }
     if (!staged_ready)
@@ -701,7 +618,7 @@ __global__ void __launch_bounds__(kBlockThreads, MCL3DL_NF_MINB)
     {
       const int j = j0 + l;
       // ---- phase A: the queries and directory entries of up to kNfU evals (independent loads in flight)
-      int c[kNfU], b[kNfU];
+      int c[kNfU];
       uint32_t s[kNfU];
       int tot = 0;
 #pragma unroll
@@ -725,82 +642,25 @@ __global__ void __launch_bounds__(kBlockThreads, MCL3DL_NF_MINB)
           c[u] = nnf_lookup(f, q.x, q.y, q.z, s[u]);
           tot += max(c[u], 0);
         }
-        ws.q[u * 32 + lane] = q;  // .w: below, once the eval's first slot is known
+        ws.q[u * 32 + lane] = q;  // .w: nf_warp_scan's, once the eval's first slot is known
       }
-      // ---- flatten: the lanes' lists end to end (inclusive shuffle scan of the lane totals), W slots in all
-      int incl = tot;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1)
-      {
-        const int v = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= o)
-          incl += v;
-      }
-      const int W = __shfl_sync(0xffffffffu, incl, 31);
-      int base = incl - tot;
+      float d2[kNfU];
+      nf_warp_scan<OVF>(ws, g, lp, c, s, tot, d2, st_rows, st_pts);
+      // ---- the owners score their evals in scan order
 #pragma unroll
       for (int u = 0; u < kNfU; ++u)
       {
-        b[u] = base;
-        base += max(c[u], 0);
-        ws.q[u * 32 + lane].w = __uint_as_float(s[u] - static_cast<uint32_t>(b[u]));  // slot + .w = candidate index
-        ws.best[u * 32 + lane] = __float_as_uint(lp.r2);
-      }
-      // ---- phase B: kNfB candidates per lane in flight, folded into their evals' bests
-      for (int lo = 0; lo < W; lo += kNfSlots)
-      {
-        const int hi = min(W, lo + kNfSlots);
-#pragma unroll
-        for (int u = 0; u < kNfU; ++u) nnf_fill_owner(ws.own, lo, hi, b[u], max(c[u], 0), u * 32 + lane);
-        __syncwarp();
-        for (int k = lo + lane; k < hi; k += 32 * kNfB)
+        float t;
+        if (d2[u] < lp.r2 && lik_term(__fsqrt_rn(d2[u]), lp, t))  // (evals beyond N keep d2 = r2)
         {
-          int e[kNfB];
-          float4 m[kNfB];
-#pragma unroll
-          for (int v = 0; v < kNfB; ++v)
-            if (k + 32 * v < hi)
-            {
-              e[v] = ws.own[k + 32 * v - lo];
-              m[v] = __ldg(f.cand + (__float_as_uint(ws.q[e[v]].w) + static_cast<uint32_t>(k + 32 * v)));
-            }
-#pragma unroll
-          for (int v = 0; v < kNfB; ++v)
-            if (k + 32 * v < hi)
-            {
-              const float4 qe = ws.q[e[v]];
-              atomicMin(&ws.best[e[v]], __float_as_uint(nnf_cand_d2(qe.x, qe.y, qe.z, m[v])));
-            }
-        }
-        __syncwarp();  // the bests are final, and the next pass may overwrite `own`
-      }
-      // ---- back to the owners, scored in scan order
-#pragma unroll
-      for (int u = 0; u < kNfU; ++u)
-      {
-        float best = __uint_as_float(ws.best[u * 32 + lane]);
-        if (OVF && c[u] < 0)  // overflow cell (raw clouds): the CSR window search
-        {
-          const float4 qu = ws.q[u * 32 + lane];
-          best = nn_dist2(g, lp, qu.x, qu.y, qu.z, st_rows, st_pts);
-        }
-        else
-          st_pts += static_cast<uint32_t>(max(c[u], 0));
-        if (best < lp.r2)  // (evals beyond N keep best = r2)
-        {
-          // likelihood.cpp:128-133
-          const float dist = fsub(lp.match_dist_min, fmaxf(__fsqrt_rn(best), lp.match_dist_flat));
-          if (!(dist < 0.0f))
-          {
-            score = fadd(score, fmul(dist, lp.match_weight));
-            cnt++;
-          }
+          score = fadd(score, t);
+          cnt++;
         }
       }
     }
     if (live && l < N)
       st_rows += static_cast<uint32_t>((N - l + TPP - 1) / TPP);  // one directory entry per eval of this lane
-    nf_reduce<TPP>(score, cnt, red_f, red_u);
+    particle_reduce<TPP>(score, cnt, red_f, red_u);
     if (live && l == 0)  // empty scan -> LidarMeasurementResult(1, 0), likelihood.cpp:111-114
       sink_store_lik(sink, out, p, (N == 0) ? 1.0f : score, cnt, write_beam_defaults);
   }
@@ -808,12 +668,8 @@ __global__ void __launch_bounds__(kBlockThreads, MCL3DL_NF_MINB)
     stage_wait(&bar);  // never leave with the bulk copy in flight
   if (stats)
   {
-    const uint32_t r = warp_sum_u32(st_rows), q = warp_sum_u32(st_pts);
-    if ((threadIdx.x & 31) == 0)
-    {
-      atomicAdd(stats + 0, static_cast<unsigned long long>(r));
-      atomicAdd(stats + 1, static_cast<unsigned long long>(q));
-    }
+    stats_add(stats, 0, st_rows);
+    stats_add(stats, 1, st_pts);
   }
 }
 
@@ -824,8 +680,8 @@ __global__ void __launch_bounds__(kBlockThreads, MCL3DL_NF_MINB)
 // warps are 256 consecutive particles on the same slice of `slice` scan points.  In tracking mode the particles of a
 // cloud see one scan point in nearly the same place, so their directory and candidate sectors coalesce within the
 // load instruction and the CTA's other warps find them in L1, where lik_kernel_nf (a warp = one particle's points)
-// sends every eval's sectors to L2 on its own.  The transform, the directory lookup (phase A) and the warp-flattened
-// candidate scan (phase B) are lik_kernel_nf's; only eval e = u * 32 + lane now means (particle lane, point j0 + u).
+// sends every eval's sectors to L2 on its own.  The transform, the directory lookup (phase A) and the candidate scan
+// (nf_warp_scan) are lik_kernel_nf's; only eval e = u * 32 + lane now means (particle lane, point j0 + u).
 //
 // A particle's points are spread over the grid's slices, so its score is folded across CTAs.  Each lane sums its
 // slice's contributions in 2^-fx_shift fixed point and adds one word (device_funcs.cuh: nf_pm_word: the sum, the match
@@ -862,23 +718,15 @@ __global__ void __launch_bounds__(kBlockThreads, MCL3DL_NF_MINB)
   rn.w = 1.0f;
   if (live)
   {
-    const float4 a = __ldg(reinterpret_cast<const float4*>(poses + p));
-    const float4 b = __ldg(reinterpret_cast<const float4*>(poses + p) + 1);
-    pos.x = a.x;
-    pos.y = a.y;
-    pos.z = a.z;
     Q4 q;
-    q.x = b.x;
-    q.y = b.y;
-    q.z = b.z;
-    q.w = b.w;
+    load_pose(poses + p, pos, q);
     rn = qnormalized(q);  // state_6dof.h:217
   }
   // every lane of the warp runs every trip (dead particles: no candidates), as in lik_kernel_nf
   for (int j0 = s0; j0 < s1; j0 += kNfU)
   {
     // ---- phase A: one scan point per u, the same for every lane (one broadcast load)
-    int c[kNfU], b[kNfU];
+    int c[kNfU];
     uint32_t s[kNfU];
     int tot = 0;
 #pragma unroll
@@ -908,73 +756,17 @@ __global__ void __launch_bounds__(kBlockThreads, MCL3DL_NF_MINB)
       }
       ws.q[u * 32 + lane] = q;
     }
-    // ---- flatten and phase B: lik_kernel_nf's
-    int incl = tot;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1)
-    {
-      const int v = __shfl_up_sync(0xffffffffu, incl, o);
-      if (lane >= o)
-        incl += v;
-    }
-    const int W = __shfl_sync(0xffffffffu, incl, 31);
-    int base = incl - tot;
+    float d2[kNfU];
+    nf_warp_scan<OVF>(ws, g, lp, c, s, tot, d2, st_rows, st_pts);
+    // ---- the owners: this lane's particle at points j0 .. j0 + kNfU - 1
 #pragma unroll
     for (int u = 0; u < kNfU; ++u)
     {
-      b[u] = base;
-      base += max(c[u], 0);
-      ws.q[u * 32 + lane].w = __uint_as_float(s[u] - static_cast<uint32_t>(b[u]));
-      ws.best[u * 32 + lane] = __float_as_uint(lp.r2);
-    }
-    for (int lo = 0; lo < W; lo += kNfSlots)
-    {
-      const int hi = min(W, lo + kNfSlots);
-#pragma unroll
-      for (int u = 0; u < kNfU; ++u) nnf_fill_owner(ws.own, lo, hi, b[u], max(c[u], 0), u * 32 + lane);
-      __syncwarp();
-      for (int k = lo + lane; k < hi; k += 32 * kNfB)
+      float t;
+      if (d2[u] < lp.r2 && lik_term(__fsqrt_rn(d2[u]), lp, t))  // (dead lanes and points beyond the slice keep d2 = r2)
       {
-        int e[kNfB];
-        float4 m[kNfB];
-#pragma unroll
-        for (int v = 0; v < kNfB; ++v)
-          if (k + 32 * v < hi)
-          {
-            e[v] = ws.own[k + 32 * v - lo];
-            m[v] = __ldg(f.cand + (__float_as_uint(ws.q[e[v]].w) + static_cast<uint32_t>(k + 32 * v)));
-          }
-#pragma unroll
-        for (int v = 0; v < kNfB; ++v)
-          if (k + 32 * v < hi)
-          {
-            const float4 qe = ws.q[e[v]];
-            atomicMin(&ws.best[e[v]], __float_as_uint(nnf_cand_d2(qe.x, qe.y, qe.z, m[v])));
-          }
-      }
-      __syncwarp();
-    }
-    // ---- back to the owners: this lane's particle at points j0 .. j0 + kNfU - 1
-#pragma unroll
-    for (int u = 0; u < kNfU; ++u)
-    {
-      float best = __uint_as_float(ws.best[u * 32 + lane]);
-      if (OVF && c[u] < 0)
-      {
-        const float4 qu = ws.q[u * 32 + lane];
-        best = nn_dist2(g, lp, qu.x, qu.y, qu.z, st_rows, st_pts);
-      }
-      else
-        st_pts += static_cast<uint32_t>(max(c[u], 0));
-      if (best < lp.r2)  // (dead lanes and points beyond the slice keep best = r2)
-      {
-        // likelihood.cpp:128-133
-        const float dist = fsub(lp.match_dist_min, fmaxf(__fsqrt_rn(best), lp.match_dist_flat));
-        if (!(dist < 0.0f))
-        {
-          sum += nf_fx_term(fmul(dist, lp.match_weight), sh.fx_shift);
-          cnt++;
-        }
+        sum += nf_fx_term(t, sh.fx_shift);
+        cnt++;
       }
     }
     __syncwarp();  // the next trip overwrites q / best
@@ -994,12 +786,8 @@ __global__ void __launch_bounds__(kBlockThreads, MCL3DL_NF_MINB)
   }
   if (stats)
   {
-    const uint32_t r = warp_sum_u32(st_rows), q = warp_sum_u32(st_pts);
-    if (lane == 0)
-    {
-      atomicAdd(stats + 0, static_cast<unsigned long long>(r));
-      atomicAdd(stats + 1, static_cast<unsigned long long>(q));
-    }
+    stats_add(stats, 0, st_rows);
+    stats_add(stats, 1, st_pts);
   }
 }
 
@@ -1039,16 +827,8 @@ __global__ void __launch_bounds__(kBlockThreads, MCL3DL_NF_MINB)
     rn.w = 1.0f;
     if (live)
     {
-      const float4 a = __ldg(reinterpret_cast<const float4*>(poses + p));
-      const float4 b = __ldg(reinterpret_cast<const float4*>(poses + p) + 1);
-      pos.x = a.x;
-      pos.y = a.y;
-      pos.z = a.z;
       Q4 q;
-      q.x = b.x;
-      q.y = b.y;
-      q.z = b.z;
-      q.w = b.w;
+      load_pose(poses + p, pos, q);
       rn = qnormalized(q);  // state_6dof.h:217
     }
     if (!staged_ready)
@@ -1080,118 +860,25 @@ __global__ void __launch_bounds__(kBlockThreads, MCL3DL_NF_MINB)
         }
 #pragma unroll
         for (int u = 0; u < kNfU; ++u)
-          if (d[u] < lp.match_dist_min)
+        {
+          float t;
+          if (d[u] < lp.match_dist_min && lik_term(d[u], lp, t))  // the interpolated distance in place of sqrt(sqdist[0])
           {
-            // likelihood.cpp:128-133 with the interpolated distance in place of sqrt(sqdist[0])
-            const float dist = fsub(lp.match_dist_min, fmaxf(d[u], lp.match_dist_flat));
-            if (!(dist < 0.0f))
-            {
-              score = fadd(score, fmul(dist, lp.match_weight));
-              cnt++;
-            }
+            score = fadd(score, t);
+            cnt++;
           }
+        }
       }
     }
-    nf_reduce<TPP>(score, cnt, red_f, red_u);
+    particle_reduce<TPP>(score, cnt, red_f, red_u);
     if (live && l == 0)
       sink_store_lik(sink, out, p, (N == 0) ? 1.0f : score, cnt, write_beam_defaults);
   }
   if (!staged_ready)
     stage_wait(&bar);
   if (stats)
-  {
-    const uint32_t r = warp_sum_u32(st_rows);
-    if ((threadIdx.x & 31) == 0)
-      atomicAdd(stats + 0, static_cast<unsigned long long>(r) * 4ull);  // counted as 8-byte index entries: 32 B per eval
-  }
+    stats_add(stats, 0, st_rows * 4u);  // counted as 8-byte index entries: 32 B per eval
 }
-
-template <int TPP, bool STAGED>
-__global__ void __launch_bounds__(kBlockThreads)
-    beam_kernel(const mcl3dl_pose* __restrict__ poses, int P, const float4* __restrict__ scan, int N,
-                const float* __restrict__ origins, DdaGridDev g, mcl3dl_result* __restrict__ out,
-                uint8_t* __restrict__ status, int write_lik_defaults, unsigned long long* __restrict__ stats, RecordSink sink)
-{
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  __shared__ uint64_t bar;
-  __shared__ float red_f[kBlockThreads / 32];
-  __shared__ uint32_t red_u[3 * kBlockThreads / 32];
-  const float4* pts = scan;
-  if (STAGED && N > 0)
-  {
-    stage_tile(smem_raw, scan, static_cast<uint32_t>(N) * 16u, &bar);
-    pts = reinterpret_cast<const float4*>(smem_raw);
-  }
-  constexpr int PPB = kBlockThreads / TPP;
-  const int sub = threadIdx.x / TPP;
-  const int l = threadIdx.x % TPP;
-  const int n_groups = (P + PPB - 1) / PPB;
-  uint32_t st_steps = 0, st_occ = 0, st_tested = 0;
-  for (int grp = blockIdx.x; grp < n_groups; grp += gridDim.x)
-  {
-    const int p = grp * PPB + sub;
-    const bool live = p < P;
-    float unused = 0.0f;
-    uint32_t n_short = 0, n_hit = 0, n_long = 0;
-    if (live)
-    {
-      const float4 a = __ldg(reinterpret_cast<const float4*>(poses + p));
-      const float4 bq = __ldg(reinterpret_cast<const float4*>(poses + p) + 1);
-      F3 pos;
-      pos.x = a.x;
-      pos.y = a.y;
-      pos.z = a.z;
-      Q4 q;
-      q.x = bq.x;
-      q.y = bq.y;
-      q.z = bq.z;
-      q.w = bq.w;
-      const Q4 rn = qnormalized(q);
-      for (int j = l; j < N; j += TPP)
-      {
-        const float4 sp = pts[j];
-        F3 v;
-        v.x = sp.x;
-        v.y = sp.y;
-        v.z = sp.z;
-        const F3 end = transform_point(rn, pos, v);  // beam.cpp:138-139
-        const F3 begin = ray_origin(pos, q, origins, __float_as_uint(sp.w));
-        const int st = cast_ray(g, begin, end, st_steps, st_occ, st_tested);
-        n_short += (st == ST_SHORT);
-        n_hit += (st == ST_HIT);
-        n_long += (st == ST_LONG);
-        if (status)
-          status[static_cast<size_t>(p) * N + j] = static_cast<uint8_t>(st);
-      }
-    }
-    group_reduce<TPP>(unused, n_short, n_hit, n_long, red_f, red_u);
-    if (live && l == 0)
-    {
-      // beam.cpp:146-152: the same factor multiplied in sequentially, then the floor
-      float score = 1.0f;
-      if (N > 0)
-      {
-        const uint32_t k = n_short + (g.short_only ? 0u : n_long);
-        for (uint32_t i = 0; i < k; ++i) score = fmul(score, g.beam_likelihood);
-        if (score < g.beam_likelihood_min)
-          score = g.beam_likelihood_min;
-      }
-      sink_store_beam(sink, out, p, score, n_short, n_hit, n_long, write_lik_defaults);
-    }
-  }
-  if (stats)
-  {
-    const uint32_t a = warp_sum_u32(st_steps), b = warp_sum_u32(st_occ), c = warp_sum_u32(st_tested);
-    if ((threadIdx.x & 31) == 0)
-    {
-      atomicAdd(stats + 2, static_cast<unsigned long long>(a));
-      atomicAdd(stats + 3, static_cast<unsigned long long>(b));
-      atomicAdd(stats + 4, static_cast<unsigned long long>(c));
-    }
-  }
-}
-
-
 
 // ============================================================================================
 // Lane-per-particle mapping for the beam model ("pl" kernel).
@@ -1199,10 +886,10 @@ __global__ void __launch_bounds__(kBlockThreads)
 // A warp takes 32 consecutive particles (one per lane) and a chunk of consecutive rays; every lane
 // casts the SAME scan ray at the same time.  In tracking mode the 32 poses are within a few
 // decimetres of each other, so the lanes walk nearly the same voxels for nearly the same number of
-// steps: the occupancy words coalesce and the trip counts agree.  With
-// spread particles nothing is lost relative to the group mapping.  A CTA = one particle group x 8 chunks (8 warps); when a scan needs more than
-// 8 chunks to fill the chip, several CTAs share a particle group and the last one to finish (ticket
-// counter) folds the per-CTA partials in chunk order, so the result is still deterministic.
+// steps: the occupancy words coalesce and the trip counts agree.  A CTA = one particle group x 8 chunks
+// (8 warps); when a scan needs more than 8 chunks to fill the chip, several CTAs share a particle group and
+// the last one to finish (ticket counter) folds the per-CTA partials in chunk order, so the result is still
+// deterministic.
 constexpr int kPlWarps = kBlockThreads / 32;
 
 struct PlShape
@@ -1249,17 +936,7 @@ __global__ void __launch_bounds__(kBlockThreads, 4)
     q.x = q.y = q.z = 0.0f;
     q.w = 1.0f;
     if (live)
-    {
-      const float4 a = __ldg(reinterpret_cast<const float4*>(poses + p));
-      const float4 bq = __ldg(reinterpret_cast<const float4*>(poses + p) + 1);
-      pos.x = a.x;
-      pos.y = a.y;
-      pos.z = a.z;
-      q.x = bq.x;
-      q.y = bq.y;
-      q.z = bq.z;
-      q.w = bq.w;
-    }
+      load_pose(poses + p, pos, q);
     const Q4 rn = qnormalized(q);
     for (int j = j0; j < j1; ++j)
     {
@@ -1334,28 +1011,13 @@ __global__ void __launch_bounds__(kBlockThreads, 4)
       }
     }
     if (writer && live)
-    {
-      // beam.cpp:146-152: the same factor multiplied in sequentially, then the floor
-      float score = 1.0f;
-      if (N > 0)
-      {
-        const uint32_t k = a + (g.short_only ? 0u : c);
-        for (uint32_t i = 0; i < k; ++i) score = fmul(score, g.beam_likelihood);
-        if (score < g.beam_likelihood_min)
-          score = g.beam_likelihood_min;
-      }
-      sink_store_beam(sink, out, p, score, a, b, c, write_lik_defaults);
-    }
+      sink_store_beam(sink, out, p, beam_score(a, c, N, g), a, b, c, write_lik_defaults);
   }
   if (stats)
   {
-    const uint32_t x = warp_sum_u32(st_steps), y = warp_sum_u32(st_occ), z = warp_sum_u32(st_tested);
-    if (lane == 0)
-    {
-      atomicAdd(stats + 2, static_cast<unsigned long long>(x));
-      atomicAdd(stats + 3, static_cast<unsigned long long>(y));
-      atomicAdd(stats + 4, static_cast<unsigned long long>(z));
-    }
+    stats_add(stats, 2, st_steps);
+    stats_add(stats, 3, st_occ);
+    stats_add(stats, 4, st_tested);
   }
 }
 
@@ -1398,17 +1060,9 @@ __global__ void __launch_bounds__(kBlockThreads, 4)
     uint32_t n_short = 0, n_hit = 0, n_long = 0;
     if (live)
     {
-      const float4 a = __ldg(reinterpret_cast<const float4*>(poses + p));
-      const float4 bq = __ldg(reinterpret_cast<const float4*>(poses + p) + 1);
       F3 pos;
-      pos.x = a.x;
-      pos.y = a.y;
-      pos.z = a.z;
       Q4 q;
-      q.x = bq.x;
-      q.y = bq.y;
-      q.z = bq.z;
-      q.w = bq.w;
+      load_pose(poses + p, pos, q);
       const Q4 rn = qnormalized(q);
       const int j0 = chunk * ppl, j1 = min(N, j0 + ppl);
       for (int j = j0; j < j1; ++j)
@@ -1449,16 +1103,7 @@ __global__ void __launch_bounds__(kBlockThreads, 4)
         t[0] = 0;
         t[1] = 0;
         t[2] = 0;
-        // beam.cpp:146-152: the same factor multiplied in sequentially, then the floor
-        float score = 1.0f;
-        if (N > 0)
-        {
-          const uint32_t k = a + (g.short_only ? 0u : c);
-          for (uint32_t i = 0; i < k; ++i) score = fmul(score, g.beam_likelihood);
-          if (score < g.beam_likelihood_min)
-            score = g.beam_likelihood_min;
-        }
-        sink_store_beam(sink, out, p, score, a, b, c, write_lik_defaults);
+        sink_store_beam(sink, out, p, beam_score(a, c, N, g), a, b, c, write_lik_defaults);
       }
       if (lane == 0)
         tickets[group] = 0;
@@ -1476,13 +1121,9 @@ __global__ void __launch_bounds__(kBlockThreads, 4)
   }
   if (stats)
   {
-    const uint32_t x = warp_sum_u32(st_steps), y = warp_sum_u32(st_occ), z = warp_sum_u32(st_tested);
-    if (lane == 0)
-    {
-      atomicAdd(stats + 2, static_cast<unsigned long long>(x));
-      atomicAdd(stats + 3, static_cast<unsigned long long>(y));
-      atomicAdd(stats + 4, static_cast<unsigned long long>(z));
-    }
+    stats_add(stats, 2, st_steps);
+    stats_add(stats, 3, st_occ);
+    stats_add(stats, 4, st_tested);
   }
 }
 

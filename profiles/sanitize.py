@@ -1,7 +1,7 @@
 """Small end-to-end run for compute-sanitizer (memcheck / racecheck / initcheck / synccheck), covering every kernel the
-library ships: map build incl. the NN field, both likelihood kernel generations + the field mode, both beam kernels x
-both raycasters, the fused weight update, the resident particle set (predict / update / estimate / resample) and the
-scan preprocessing.
+library ships: map build incl. the NN field, the likelihood kernels with and without the NN field + the field mode, both
+beam kernels x both raycasters, the fused weight update, the resident particle set (predict / update / estimate /
+resample) and the scan preprocessing.
    compute-sanitizer --tool racecheck python profiles/sanitize.py"""
 import os
 import sys
@@ -12,8 +12,8 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from mcl_3dl_b200 import engine, synth  # noqa: E402
 
 s = synth.scene(20_000, 70, 96, 40, seed=3)
-for env in ({}, {"MCL3DL_MAPPING": "group"}, {"MCL3DL_NNF": "0"}, {"MCL3DL_BEAM": "dq"}, {"MCL3DL_BEAM": "pl"}):
-    for k in ("MCL3DL_MAPPING", "MCL3DL_NNF", "MCL3DL_BEAM"):
+for env in ({}, {"MCL3DL_NNF": "0"}, {"MCL3DL_BEAM": "dq"}, {"MCL3DL_BEAM": "pl"}):
+    for k in ("MCL3DL_NNF", "MCL3DL_BEAM"):
         os.environ.pop(k, None)
     os.environ.update(env)
     for use_dda in (True, False):
@@ -25,7 +25,7 @@ for env in ({}, {"MCL3DL_MAPPING": "group"}, {"MCL3DL_NNF": "0"}, {"MCL3DL_BEAM"
         st = eng.beam_status(s["particles"][:5], s["beam"], s["origins"])
         print(env, "dda" if use_dda else "kd", int(r["match_cnt"].sum()), int(r["n_hit"].sum()), st.shape)
         eng.close()
-for k in ("MCL3DL_MAPPING", "MCL3DL_NNF", "MCL3DL_BEAM"):
+for k in ("MCL3DL_NNF", "MCL3DL_BEAM"):
     os.environ.pop(k, None)
 eng = engine.Engine((0,))
 eng.set_map(s["map"], engine.LikParams(dist_weight=(1, 1, 5)), engine.beam_params_from_reference(num_points_default=40))

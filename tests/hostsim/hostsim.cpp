@@ -321,18 +321,12 @@ extern "C" int hostsim_measure_nf(const mcl3dl_point* map, size_t n, const mcl3d
   for (size_t p = 0; p < P; ++p)
   {
     F3 pos;
-    pos.x = poses[p].px;
-    pos.y = poses[p].py;
-    pos.z = poses[p].pz;
     Q4 q;
-    q.x = poses[p].qx;
-    q.y = poses[p].qy;
-    q.z = poses[p].qz;
-    q.w = poses[p].qw;
+    load_pose(poses + p, pos, q);
     const Q4 rn = qnormalized(q);
     mcl3dl_result r;
     std::memset(&r, 0, sizeof(r));
-    // beam: the per-ray body of beam_kernel / beam_kernel_pl
+    // beam: the per-ray body of beam_kernel_pl / beam_kernel_dq
     uint32_t a = 0, b = 0, c = 0, s0 = 0, s1 = 0, s2 = 0;
     for (size_t j = 0; j < n_beam; ++j)
     {
@@ -352,18 +346,11 @@ extern "C" int hostsim_measure_nf(const mcl3dl_point* map, size_t n, const mcl3d
     wk[2] += s0;
     wk[3] += s1;
     wk[4] += s2;
-    float score = 1.0f;
-    if (n_beam)
-    {
-      const uint32_t k = a + (m.dda.short_only ? 0u : c);
-      for (uint32_t i = 0; i < k; ++i) score = fmul(score, m.dda.beam_likelihood);
-      if (score < m.dda.beam_likelihood_min) score = m.dda.beam_likelihood_min;
-    }
-    r.score_beam = score;
+    r.score_beam = beam_score(a, c, static_cast<int>(n_beam), m.dda);
     r.n_short = a;
     r.n_hit = b;
     r.n_long = c;
-    // likelihood: the per-eval body of lik_kernel, summed in scan order
+    // likelihood: the per-eval body of the likelihood kernels, summed in scan order
     if (n_lik == 0)
     {
       r.score_like = 1.0f;
@@ -381,14 +368,11 @@ extern "C" int hostsim_measure_nf(const mcl3dl_point* map, size_t n, const mcl3d
         const F3 t = transform_point(rn, pos, v);
         const float sx = fmul(t.x, m.nn.wx), sy = fmul(t.y, m.nn.wy), sz = fmul(t.z, m.nn.wz);
         const float d2 = m.nn.field.dir ? nnf_dist2(m.nn, m.lik, sx, sy, sz, rows, npts) : nn_dist2(m.nn, m.lik, sx, sy, sz, rows, npts);
-        if (d2 < m.lik.r2)
+        float term;
+        if (d2 < m.lik.r2 && lik_term(__fsqrt_rn(d2), m.lik, term))
         {
-          const float dist = fsub(m.lik.match_dist_min, fmaxf(__fsqrt_rn(d2), m.lik.match_dist_flat));
-          if (!(dist < 0.0f))
-          {
-            sl = fadd(sl, fmul(dist, m.lik.match_weight));
-            cnt++;
-          }
+          sl = fadd(sl, term);
+          cnt++;
         }
       }
       r.score_like = sl;

@@ -27,11 +27,13 @@ def eng_mod():
 
 @pytest.fixture(params=["tuned", "group"])
 def eng(eng_mod, request, monkeypatch):
-    """Both kernel generations (csrc/kernels.cuh): the tuned default and the plain MCL3DL_MAPPING=group ones."""
+    """Both likelihood paths (csrc/kernels.cuh): `tuned` stages the NN field (lik_kernel_nf_pm / lik_kernel_nf);
+    `group` stages none (MCL3DL_NNF=0, as for a field above MCL3DL_NNF_MAX_MB): lik_kernel_wi, a group of TPP lanes per
+    particle searching the CSR windows.  The beam kernels are the same in both."""
     if request.param == "group":
-        monkeypatch.setenv("MCL3DL_MAPPING", "group")
+        monkeypatch.setenv("MCL3DL_NNF", "0")
     else:
-        monkeypatch.delenv("MCL3DL_MAPPING", raising=False)
+        monkeypatch.delenv("MCL3DL_NNF", raising=False)
     e = eng_mod.Engine((0,))
     yield e
     e.close()
@@ -39,7 +41,7 @@ def eng(eng_mod, request, monkeypatch):
 
 @pytest.fixture
 def eng_mod_engine_tuned(eng_mod, monkeypatch):
-    monkeypatch.delenv("MCL3DL_MAPPING", raising=False)
+    monkeypatch.delenv("MCL3DL_NNF", raising=False)
     e = eng_mod.Engine((0,))
     yield e
     e.close()
@@ -445,7 +447,7 @@ def test_wide_cells_of_the_nn_field(eng_mod, eng, cc):
     for use_dda in (True, False):  # the KD-tree caster's marching search reads the same lists
         cpu = run_both(eng_mod, eng, cc, s, (1, 1, 1), 8, dda_grid=0.2, use_dda=use_dda)
         info = eng.nn_field_info()
-        if os.environ.get("MCL3DL_MAPPING") != "group":  # (the plain kernels search the CSR windows: no field staged)
+        if os.environ.get("MCL3DL_NNF") != "0":  # (without the field the CSR windows are searched: none staged)
             assert info["bytes"] > 0 and info["wide_cells"] > 0
             assert not use_dda or info["overflow_cells"] == 0  # (the KD caster's larger search radius may overflow a few)
         want = cpu.measure(s["particles"], s["lik"], s["beam"], s["origins"])
@@ -492,7 +494,7 @@ def test_options_change_no_record(eng_mod, monkeypatch, use_dda):
     beam = eng_mod.beam_params_from_reference(num_points_default=24, dda_grid_size=0.2, use_raycast_using_dda=use_dda)
 
     def run(env, timing=False):
-        for k in ("MCL3DL_NEAR_K", "MCL3DL_NEAR_KD_K", "MCL3DL_ZEROCOPY_OUT", "MCL3DL_TIMING", "MCL3DL_MAPPING", "MCL3DL_NNF",
+        for k in ("MCL3DL_NEAR_K", "MCL3DL_NEAR_KD_K", "MCL3DL_ZEROCOPY_OUT", "MCL3DL_TIMING", "MCL3DL_NNF",
                   "MCL3DL_BEAM", "MCL3DL_BEAM_DQ_PPL"):
             monkeypatch.delenv(k, raising=False)
         for k, v in env.items():
@@ -515,13 +517,11 @@ def test_options_change_no_record(eng_mod, monkeypatch, use_dda):
     timed, _, t1 = run({"MCL3DL_NEAR_K": "1", "MCL3DL_ZEROCOPY_OUT": "100"}, timing=True)   # 300 particles > 100: bulk D2H copy
     assert timed.tobytes() == plain.tobytes()
     assert t1["lik_ms"] > 0.0 and t1["beam_ms"] > 0.0 and t1["h2d_ms"] > 0.0
-    def same(a, b):  # another kernel generation may sum a particle's likelihood terms in another order
+    def same(a, b):  # another likelihood kernel may sum a particle's likelihood terms in another order
         for f in ("match_cnt", "score_beam", "n_short", "n_hit", "n_long"):
             assert np.array_equal(a[f], b[f]), f
         assert np.allclose(a["score_like"], b["score_like"], rtol=2e-6, atol=1e-6)
-    group, _, _ = run({"MCL3DL_MAPPING": "group", "MCL3DL_NEAR_K": "3", "MCL3DL_NEAR_KD_K": "2"})
-    same(group, plain)
-    csr, _, _ = run({"MCL3DL_NNF": "0"})                      # the CSR-window kernels of round 1 (no NN field)
+    csr, _, _ = run({"MCL3DL_NNF": "0", "MCL3DL_NEAR_K": "3", "MCL3DL_NEAR_KD_K": "2"})  # the CSR-window kernel (no NN field)
     same(csr, plain)
     # both beam kernels (static CTA mapping / dynamic queue with several item sizes): integer tallies, so byte-identical
     for env in ({"MCL3DL_BEAM": "pl"}, {"MCL3DL_BEAM": "dq"}, {"MCL3DL_BEAM": "dq", "MCL3DL_BEAM_DQ_PPL": "1"},
