@@ -630,7 +630,8 @@ __device__ __forceinline__ float nnf_cand_d2(float qx, float qy, float qz, const
 // of its contributions in 2^-fx_shift fixed point].  The fields below the sum never carry (arrivals <= n_slices <
 // 2^arr_bits, matches <= N < 2^cnt_bits), and fx_shift keeps N contributions of at most match_dist_min * |match_weight|
 // each below a quarter of the sum field's range.  ok: the rounding of N terms stays below 2^-30 of that bound (scans of
-// up to a few thousand points); otherwise the particle-major kernel runs.
+// up to a few thousand points, and a bound whose fx_shift needs no clamp to +-120, e.g. not |match_weight| = 1e-36);
+// otherwise the particle-major kernel runs.
 struct NfPmShape
 {
   int slice, n_slices, fx_shift, arr_bits, cnt_bits;
@@ -656,8 +657,11 @@ inline NfPmShape nf_pm_shape(int N, int blocks, int slots, int unit, float match
   int e = 0;
   if (bound > 0.0)
     std::frexp(bound, &e);  // bound < 2^e
-  s.fx_shift = std::max(-120, std::min(120, sum_bits - 3 - e));
-  s.ok = sum_bits - 3 - nf_bit_width(N) >= 30;
+  const int k = sum_bits - 3 - e;
+  s.fx_shift = std::max(-120, std::min(120, k));
+  // a clamped scale (|match_weight| so small or large that 2^fx_shift leaves float's normal range) no longer fits the
+  // bound to the sum field, and the rounding of N terms is no longer below 2^-30 of the bound
+  s.ok = sum_bits - 3 - nf_bit_width(N) >= 30 && s.fx_shift == k;
   return s;
 }
 // one eval's contribution in fixed point (exact but for the bits below 2^-fx_shift: the scale is a power of two)

@@ -3,7 +3,9 @@ golden outputs of the reference's own sources.  Everything here needs an H100 (`
 
 Bars (BASELINE.json north_star): beam HIT/SHORT/LONG tallies and per-ray BeamStatus bit-exact;
 match counts bit-exact; likelihood scores within 1e-4 relative (the per-particle float sum is
-reduced in a different order than the reference's sequential loop).
+reduced in a different order than the reference's sequential loop).  LIK_RTOL is the bar against the oracle's serial
+float sum; the tight bar of each likelihood kernel, against the exact sum of the reference's per-point terms, lives in
+test_gpu_lik_exact.py.
 """
 import os
 

@@ -66,6 +66,25 @@ def test_long_scans_keep_the_particle_major_kernel(lib):
     assert not shape(lib, 1 << 16, 1024, 528)[5]
 
 
+@pytest.mark.parametrize("N,P,slots", [(512, 1024, 528), (1, 256, 528), (2047, 1024, 528), (96, 4097, 132)])
+def test_clamped_scales_keep_the_particle_major_kernel(lib, N, P, slots):
+    """fx_shift is clamped to +-120 (2^fx_shift stays a normal float).  Where the clamp binds, the N roundings to
+    2^-fx_shift are no longer below 2^-30 of the bound (match_weight = 1e-36: every term rounds to zero or one step),
+    so the shape must not report ok.  Every shape that does report ok, over |match_weight| from 1e-40 to 1e38, keeps
+    the headroom and rounding bounds of test_fixed_point_headroom."""
+    r = 0.2
+    assert not shape(lib, N, P, slots, r, 1e-36)[5] and not shape(lib, N, P, slots, r, -1e-36)[5]
+    for w in [s * 10.0 ** d for d in range(-40, 39) for s in (1.0, -1.0)]:
+        _, _, k, a, c, ok = shape(lib, N, P, slots, r, w)
+        assert ok or abs(w) < 1e-6, w  # the clamp binds only for tiny weights
+        if not ok:
+            continue
+        sum_bits = 64 - a - c
+        worst = Fraction(N) * Fraction(float(np.float32(r))) * Fraction(abs(float(np.float32(w)))) * (1 + Fraction(1, 1 << 20))
+        assert worst * (Fraction(2) ** k) < 2 ** (sum_bits - 2), w
+        assert Fraction(N, 2) / (worst * Fraction(2) ** k) <= Fraction(1, 1 << 30), w
+
+
 @pytest.mark.parametrize("seed", range(4))
 @pytest.mark.parametrize("P,N,slots", [(1024, 512, 528), (300, 97, 528), (65, 40, 3), (513, 33, 528), (256, 0, 528)])
 def test_fold_matches_serial(lib, seed, P, N, slots):
