@@ -552,6 +552,24 @@ int opt_in_smem(mcl3dl_engine* eng, DeviceCtx& c, K kernel, int bytes)
   return MCL3DL_OK;
 }
 
+// Launch with programmatic stream serialization (kernels.cuh: pdl_start): the kernel's launch and CTA dispatch overlap
+// the drain of the grid before it in the stream; the kernel itself waits for that grid before its first global read.
+template <typename... KArgs, typename... Args>
+cudaError_t launch_pdl(void (*kernel)(KArgs...), int grid, size_t smem, cudaStream_t st, Args... args)
+{
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(grid);
+  cfg.blockDim = dim3(kBlockThreads);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = st;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+}
+
 // CSR-window likelihood kernel (no NN field staged)
 template <int TPP>
 int launch_lik_wi_t(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_pose* poses, int P, const float4* scan, int N,
@@ -607,8 +625,8 @@ int launch_lik_nf_t(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_pose* poses, 
                              : (ovf ? lik_kernel_nf<TPP, false, true> : lik_kernel_nf<TPP, false, false>);
   if (staged)
     if (int rc = opt_in_smem(eng, c, kernel, kMaxStagedBytes / 2)) return rc;
-  kernel<<<grid, kBlockThreads, staged ? bytes : 0, st>>>(poses, P, scan, N, c.nn, eng->likdev, out, beam_defaults, c.stats_ptr(), sink);
-  CK(cudaGetLastError());
+  CK(launch_pdl(kernel, grid, staged ? bytes : 0, st, poses, P, scan, N, c.nn, eng->likdev, out, beam_defaults,
+                c.stats_ptr(), sink));
   eng->launches++;
   return MCL3DL_OK;
 }
@@ -628,9 +646,8 @@ int launch_lik_nf_pm(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_pose* poses,
   }
   auto* acc = static_cast<unsigned long long*>(c.d_lacc.p);
   const auto kernel = eng->nnf_overflow_cells != 0 ? lik_kernel_nf_pm<true> : lik_kernel_nf_pm<false>;
-  kernel<<<blocks * sh.n_slices, kBlockThreads, 0, st>>>(poses, P, scan, N, c.nn, eng->likdev, out, beam_defaults,
-                                                         c.stats_ptr(), sink, sh, acc);
-  CK(cudaGetLastError());
+  CK(launch_pdl(kernel, blocks * sh.n_slices, 0, st, poses, P, scan, N, c.nn, eng->likdev, out, beam_defaults,
+                c.stats_ptr(), sink, sh, acc));
   eng->launches++;
   return MCL3DL_OK;
 }

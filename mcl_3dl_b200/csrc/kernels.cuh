@@ -492,12 +492,35 @@ struct NfWarpSmem
   uint8_t own[kNfSlots];    // slot -> eval, for the pass's slots
 };
 
+// Segment cuts of lik_kernel_nf_pm, for profiles/lik_pm_anatomy.py only (the default, 0, is the whole kernel).  A cut
+// variant ends the chain after one segment and keeps that segment's results live with a store that never happens:
+//   1 return at entry (launch and drain of the same grid)   2 after the pose is normalised   3 after phase A
+//   4 after the owner table   5 after phase B   6 before the fold
+#ifndef MCL3DL_PM_CUT
+#define MCL3DL_PM_CUT 0
+#endif
+// Programmatic dependent launch (engine.cu: launch_pdl).  The NN-field likelihood kernels may start while the grid
+// before them in the stream drains: each lets the next such launch start once all of its CTAs run, and waits for the
+// grid before it to finish (and its stores to be visible) before its first global read, since that grid may have
+// written the poses or the scan.
+__device__ __forceinline__ void pdl_start()
+{
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+}
+
+__device__ __forceinline__ void pm_cut_sink(unsigned long long* acc, int p, bool live, uint32_t keep)
+{
+  if (live && keep == 0x7fc00001u)
+    acc[p] = keep;
+}
+
 // The candidate scan of one warp trip of the NN-field kernels (lik_kernel_nf, lik_kernel_nf_pm).  Phase A has left the
 // query of this lane's eval u (eval e = u * 32 + lane) in ws.q[e].xyz, and its candidate count c[u] (-1: overflow cell)
 // and first candidate s[u] from nnf_lookup; an eval without a query has c[u] = 0.  tot: the lane's candidates in all
 // (the sum of max(c[u], 0), counted in phase A: summed here, it costs a spill).  Returns each eval's best d^2 in d2[u]
 // (r2 when no map point is closer).  Every lane of the warp calls it: it shuffles and synchronises the whole warp.
-template <bool OVF>
+template <bool OVF, int CUT = 0>
 __device__ __forceinline__ void nf_warp_scan(NfWarpSmem& ws, const NnGridDev& g, const LikDev& lp, const int (&c)[kNfU],
                                              const uint32_t (&s)[kNfU], int tot, float (&d2)[kNfU], uint32_t& st_rows,
                                              uint32_t& st_pts)
@@ -531,6 +554,12 @@ __device__ __forceinline__ void nf_warp_scan(NfWarpSmem& ws, const NnGridDev& g,
 #pragma unroll
     for (int u = 0; u < kNfU; ++u) nnf_fill_owner(ws.own, lo, hi, b[u], max(c[u], 0), u * 32 + lane);
     __syncwarp();
+    if (CUT == 4)
+    {
+#pragma unroll
+      for (int u = 0; u < kNfU; ++u) d2[u] = __uint_as_float(ws.own[(u * 32 + lane) & (kNfSlots - 1)]);
+      return;
+    }
     for (int k = lo + lane; k < hi; k += 32 * kNfB)
     {
       int e[kNfB];
@@ -578,6 +607,7 @@ __global__ void __launch_bounds__(kBlockThreads, MCL3DL_NF_MINB)
   __shared__ float red_f[kBlockThreads / 32];
   __shared__ uint32_t red_u[kBlockThreads / 32];
   __shared__ NfWarpSmem nfw[kBlockThreads / 32];
+  pdl_start();
   if (STAGED && N > 0)
     stage_issue(smem_raw, scan, static_cast<uint32_t>(N) * 16u, &bar);
   constexpr int PPB = kBlockThreads / TPP;
@@ -698,6 +728,9 @@ __global__ void __launch_bounds__(kBlockThreads, MCL3DL_NF_MINB)
                      unsigned long long* __restrict__ stats, RecordSink sink, NfPmShape sh,
                      unsigned long long* __restrict__ acc)
 {
+  pdl_start();
+  if (MCL3DL_PM_CUT == 1)
+    return;
   __shared__ NfWarpSmem nfw[kBlockThreads / 32];
   const int lane = threadIdx.x & 31;
   const int group = (blockIdx.x / sh.n_slices) * (kBlockThreads / 32) + (threadIdx.x >> 5);
@@ -721,6 +754,14 @@ __global__ void __launch_bounds__(kBlockThreads, MCL3DL_NF_MINB)
     Q4 q;
     load_pose(poses + p, pos, q);
     rn = qnormalized(q);  // state_6dof.h:217
+  }
+  uint32_t keep = 0;  // MCL3DL_PM_CUT only
+  if (MCL3DL_PM_CUT == 2)
+  {
+    keep = __float_as_uint(rn.x) ^ __float_as_uint(rn.y) ^ __float_as_uint(rn.z) ^ __float_as_uint(rn.w) ^
+           __float_as_uint(pos.x) ^ __float_as_uint(pos.y) ^ __float_as_uint(pos.z);
+    pm_cut_sink(acc, p, live, keep);
+    return;
   }
   // every lane of the warp runs every trip (dead particles: no candidates), as in lik_kernel_nf
   for (int j0 = s0; j0 < s1; j0 += kNfU)
@@ -756,8 +797,21 @@ __global__ void __launch_bounds__(kBlockThreads, MCL3DL_NF_MINB)
       }
       ws.q[u * 32 + lane] = q;
     }
+    if (MCL3DL_PM_CUT == 3)
+    {
+#pragma unroll
+      for (int u = 0; u < kNfU; ++u) keep ^= s[u] ^ static_cast<uint32_t>(c[u]);
+      continue;
+    }
     float d2[kNfU];
-    nf_warp_scan<OVF>(ws, g, lp, c, s, tot, d2, st_rows, st_pts);
+    nf_warp_scan<OVF, MCL3DL_PM_CUT>(ws, g, lp, c, s, tot, d2, st_rows, st_pts);
+    if (MCL3DL_PM_CUT == 4 || MCL3DL_PM_CUT == 5)
+    {
+#pragma unroll
+      for (int u = 0; u < kNfU; ++u) keep ^= __float_as_uint(d2[u]);
+      __syncwarp();
+      continue;
+    }
     // ---- the owners: this lane's particle at points j0 .. j0 + kNfU - 1
 #pragma unroll
     for (int u = 0; u < kNfU; ++u)
@@ -770,6 +824,11 @@ __global__ void __launch_bounds__(kBlockThreads, MCL3DL_NF_MINB)
       }
     }
     __syncwarp();  // the next trip overwrites q / best
+  }
+  if (MCL3DL_PM_CUT >= 3)
+  {
+    pm_cut_sink(acc, p, live, keep ^ static_cast<uint32_t>(sum) ^ cnt);
+    return;
   }
   // ---- fold across the slices: one atomic per particle and slice, whose result tells the last slice
   if (live)
