@@ -296,7 +296,9 @@ int mcl3dl_particles_estimate(mcl3dl_engine*, const mcl3dl_pose* state_prev, flo
  * PointCloudUniformSampler::sample (point_cloud_uniform_sampler.h:56-74).  The prepared scans stay on the device for
  * mcl3dl_particles_measure_update_prepared; scan_get reads any stage back.  num_points are the values
  * setGlobalLocalizationStatus computed on the host (likelihood.cpp:63-77).  Departures: PCL's VoxelGrid is third-party
- * and unpinned (restated from its published algorithm; centroid float sums in input order, majority label); the
+ * and unpinned (restated from its published algorithm; centroid float sums in input order, majority label, lowest on
+ * ties); non-finite points are skipped by the VoxelGrid as for a cloud that is not dense, and more than INT32_MAX voxels
+ * by PCL's count leave the cloud unfiltered, as PCL does (without downsampling, non-finite points reach filter()); the
  * sampler's draws come from Philox-4x32-10 (the reference seeds from std::random_device: not reproducible either). */
 typedef struct
 {

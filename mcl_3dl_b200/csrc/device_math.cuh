@@ -31,6 +31,13 @@ __device__ __forceinline__ double dsub(double a, double b) { return __dsub_rn(a,
 __device__ __forceinline__ double dmul(double a, double b) { return __dmul_rn(a, b); }
 __device__ __forceinline__ double ddiv(double a, double b) { return __ddiv_rn(a, b); }
 
+// float -> unsigned int that orders like the float (for atomicMin / atomicMax bounding boxes)
+__device__ __forceinline__ uint32_t f2ord(float f)
+{
+  const uint32_t b = __float_as_uint(f);
+  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+
 // Vec3::dot, include/mcl_3dl/vec3.h:140-143: (x*x' + y*y') + z*z'
 __device__ __forceinline__ float dot3(const F3& a, const F3& b)
 {

@@ -30,11 +30,6 @@ constexpr int kMaxStagedBytes = 200 * 1024;
 constexpr int kMaxStagedSorted = 160 * 1024;  // the sorted kernel also holds ~26 KB of static shared memory
 
 // ---------------------------------------------------------------- device build kernels
-__device__ __forceinline__ uint32_t f2ord(float f)
-{
-  const uint32_t b = __float_as_uint(f);
-  return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
-}
 inline float ord2f(uint32_t o)
 {
   const uint32_t b = (o & 0x80000000u) ? (o & 0x7fffffffu) : ~o;
@@ -377,9 +372,10 @@ struct DeviceCtx
   std::vector<const void*> smem_opted;  // kernels already opted in to large dynamic shared memory on this device
   // resident particle set (mcl3dl_particles_*): two state buffers (resampling writes the other one), probabilities,
   // prefix sum + pstep, the packed poses / odometry-error factors the measurement kernels read
-  // scan preprocessing (mcl3dl_scan_prepare): raw cloud, sort keys / values (x2), flags + scan positions (x2), the
-  // downsampled cloud, the two clipped clouds, the two sampled scans, cub scratch, device-side counts
-  DevBuf s_raw, s_keys[2], s_vals[2], s_flags[2], s_pos[2], s_ds, s_clip[2], s_out[2], s_tmp, s_counts;
+  // scan preprocessing (mcl3dl_scan_prepare): raw cloud, sort keys / values (x2), (voxel, label) keys of the vote (x2),
+  // flags + scan positions (x2), the downsampled cloud, the two clipped clouds, the two sampled scans, cub scratch,
+  // device-side counts
+  DevBuf s_raw, s_keys[2], s_vals[2], s_key_label[2], s_flags[2], s_pos[2], s_ds, s_clip[2], s_out[2], s_tmp, s_counts;
   mcl3dl_scan_info s_info{};
   bool s_valid = false;
   DevBuf r_states[2], r_prob, r_accum, r_poses, r_extra, r_est;  // r_est: EstHeader + per-CTA partial sums
@@ -1563,8 +1559,8 @@ void mcl3dl_destroy(mcl3dl_engine* eng)
     free_buf(c.xchg);
     free_buf(c.x_ticket);
     for (DevBuf* b : {&c.r_states[0], &c.r_states[1], &c.r_prob, &c.r_accum, &c.r_poses, &c.r_extra, &c.r_est, &c.s_raw, &c.s_keys[0],
-                      &c.s_keys[1], &c.s_vals[0], &c.s_vals[1], &c.s_flags[0], &c.s_flags[1], &c.s_pos[0], &c.s_pos[1], &c.s_ds,
-                      &c.s_clip[0], &c.s_clip[1], &c.s_out[0], &c.s_out[1], &c.s_tmp, &c.s_counts})
+                      &c.s_keys[1], &c.s_vals[0], &c.s_vals[1], &c.s_key_label[0], &c.s_key_label[1], &c.s_flags[0],
+                      &c.s_flags[1], &c.s_pos[0], &c.s_pos[1], &c.s_ds, &c.s_clip[0], &c.s_clip[1], &c.s_out[0], &c.s_out[1], &c.s_tmp, &c.s_counts})
       free_buf(*b);
     for (DevBuf* b : {&c.nn_cell_start, &c.nn_pts, &c.nn_row3, &c.dda_occ, &c.dda_cell_start, &c.dda_pts, &c.raw_pts, &c.near_lik, &c.near_kd, &c.nnf_dir, &c.nnf_cand, &c.nnf_wide, &c.fld_cells, &c.d_poses,
                       &c.d_out, &c.d_status, &c.d_stats, &c.d_partial, &c.d_tickets, &c.d_tally, &c.d_queue, &c.d_lacc, &c.d_w, &c.d_post, &c.d_wpart, &c.d_wticket})
@@ -2117,59 +2113,53 @@ int mcl3dl_scan_prepare(mcl3dl_engine* eng, const mcl3dl_point* raw, size_t n_ra
   bool ds_done = false;
   if (downsample)
   {
-    // bounding box -> VoxelGrid lattice (getMinMax3D; min_b / max_b / div_b of voxel_grid.hpp)
-    uint32_t h_bbox[12];
-    for (int k = 0; k < 3; ++k)
-    {
-      h_bbox[k] = 0xffffffffu;
-      h_bbox[3 + k] = 0u;
-      h_bbox[6 + k] = 0xffffffffu;
-      h_bbox[9 + k] = 0u;
-    }
+    // bounding box of the finite points -> VoxelGrid lattice and PCL's overflow rule (scan_voxel_lattice)
+    uint32_t h_bbox[6] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u};
     if ((rc = reserve(eng, c.s_tmp, 4096)))
       return rc;
     uint32_t* bb = static_cast<uint32_t*>(c.s_tmp.p);
     CK(cudaMemcpyAsync(bb, h_bbox, sizeof(h_bbox), cudaMemcpyHostToDevice, st));
-    bbox_kernel<<<std::min(nb, c.sm_count * 8), 256, 0, st>>>(d_raw, n_raw, 1.0f, 1.0f, 1.0f, bb);
+    scan_bbox_kernel<<<std::min(nb, c.sm_count * 8), 256, 0, st>>>(d_raw, n, bb);
     CK(cudaGetLastError());
     eng->launches++;
     CK(cudaMemcpyAsync(h_bbox, bb, sizeof(h_bbox), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
+    const float mn[3] = {ord2f(h_bbox[0]), ord2f(h_bbox[1]), ord2f(h_bbox[2])};
+    const float mx[3] = {ord2f(h_bbox[3]), ord2f(h_bbox[4]), ord2f(h_bbox[5])};
     VoxelGridDev g{};
-    double cells = 1.0;
-    for (int k = 0; k < 3; ++k)
+    int end_bit = 0;
+    if (!(mn[0] <= mx[0]))
     {
-      g.inv_leaf[k] = 1.0f / sp->downsample[k];
-      const float mn = ord2f(h_bbox[k]), mx = ord2f(h_bbox[3 + k]);
-      g.min_b[k] = static_cast<int>(std::floor(mn * g.inv_leaf[k]));
-      const int max_b = static_cast<int>(std::floor(mx * g.inv_leaf[k]));
-      g.div_b[k] = max_b - g.min_b[k] + 1;
-      cells *= static_cast<double>(g.div_b[k]);
+      ds_done = true;  // no finite point: the voxel pass skips every point, the downsampled cloud is empty (counts[0] == 0)
     }
-    if (cells < 4294967295.0)  // (PCL itself refuses above INT_MAX voxels and returns the cloud unfiltered)
+    else if (scan_voxel_lattice(sp->downsample, mn, mx, g, end_bit))
     {
+      if ((rc = reserve(eng, c.s_key_label[0], cap * 8)) || (rc = reserve(eng, c.s_key_label[1], cap * 8)))
+        return rc;
       uint32_t *k0 = static_cast<uint32_t*>(c.s_keys[0].p), *k1 = static_cast<uint32_t*>(c.s_keys[1].p);
       uint32_t *v0 = static_cast<uint32_t*>(c.s_vals[0].p), *v1 = static_cast<uint32_t*>(c.s_vals[1].p);
+      uint64_t *kl0 = static_cast<uint64_t*>(c.s_key_label[0].p), *kl1 = static_cast<uint64_t*>(c.s_key_label[1].p);
       uint32_t *fl = static_cast<uint32_t*>(c.s_flags[0].p), *ps = static_cast<uint32_t*>(c.s_pos[0].p);
-      scan_key_kernel<<<nb, 256, 0, st>>>(d_raw, n, g, k0, v0);
-      size_t t_sort = 0, t_scan = 0;
-      int end_bit = 1;
-      while ((1.0 * (uint64_t(1) << end_bit)) < cells && end_bit < 32) ++end_bit;
+      scan_key_kernel<<<nb, 256, 0, st>>>(d_raw, n, g, k0, v0, kl0);
+      size_t t_sort = 0, t_sort_kl = 0, t_scan = 0;
       CK(cub::DeviceRadixSort::SortPairs(nullptr, t_sort, k0, k1, v0, v1, n, 0, end_bit, st));
+      CK(cub::DeviceRadixSort::SortKeys(nullptr, t_sort_kl, kl0, kl1, n, 0, 32 + end_bit, st));
       CK(cub::DeviceScan::ExclusiveSum(nullptr, t_scan, fl, ps, n, st));
-      if ((rc = reserve(eng, c.s_tmp, std::max(t_sort, t_scan) + 256)))
+      if ((rc = reserve(eng, c.s_tmp, std::max(std::max(t_sort, t_sort_kl), t_scan) + 256)))
         return rc;
       size_t tsz = c.s_tmp.cap;
       CK(cub::DeviceRadixSort::SortPairs(c.s_tmp.p, tsz, k0, k1, v0, v1, n, 0, end_bit, st));  // stable: input order inside a voxel
+      tsz = c.s_tmp.cap;
+      CK(cub::DeviceRadixSort::SortKeys(c.s_tmp.p, tsz, kl0, kl1, n, 0, 32 + end_bit, st));  // labels ascending inside a voxel
       scan_heads_kernel<<<nb, 256, 0, st>>>(k1, n, fl);
       tsz = c.s_tmp.cap;
       CK(cub::DeviceScan::ExclusiveSum(c.s_tmp.p, tsz, fl, ps, n, st));
-      scan_centroid_kernel<<<nb, 256, 0, st>>>(d_raw, k1, v1, fl, ps, n, static_cast<mcl3dl_point*>(c.s_ds.p), counts + 0);
+      scan_centroid_kernel<<<nb, 256, 0, st>>>(d_raw, k1, v1, kl1, fl, ps, n, g.cells, static_cast<mcl3dl_point*>(c.s_ds.p), counts + 0);
       CK(cudaGetLastError());
-      eng->launches += 5;
-      d_ds = static_cast<const mcl3dl_point*>(c.s_ds.p);
+      eng->launches += 6;
       ds_done = true;
     }
+    d_ds = static_cast<const mcl3dl_point*>(c.s_ds.p);
   }
   if (!ds_done)
   {
@@ -2178,8 +2168,8 @@ int mcl3dl_scan_prepare(mcl3dl_engine* eng, const mcl3dl_point* raw, size_t n_ra
     d_ds = static_cast<const mcl3dl_point*>(c.s_ds.p);
   }
   // clip (both models at once), compaction in order, then the uniform sample
-  const ClipDev ca{sp->lik_clip_near * sp->lik_clip_near, sp->lik_clip_far * sp->lik_clip_far, sp->lik_clip_z_min, sp->lik_clip_z_max};
-  const ClipDev cb{sp->beam_clip_near * sp->beam_clip_near, sp->beam_clip_far * sp->beam_clip_far, sp->beam_clip_z_min, sp->beam_clip_z_max};
+  const ClipDev ca = scan_clip_window(sp->lik_clip_near, sp->lik_clip_far, sp->lik_clip_z_min, sp->lik_clip_z_max);
+  const ClipDev cb = scan_clip_window(sp->beam_clip_near, sp->beam_clip_far, sp->beam_clip_z_min, sp->beam_clip_z_max);
   uint32_t *fa = static_cast<uint32_t*>(c.s_flags[0].p), *fb = static_cast<uint32_t*>(c.s_flags[1].p);
   uint32_t *pa = static_cast<uint32_t*>(c.s_pos[0].p), *pb = static_cast<uint32_t*>(c.s_pos[1].p);
   scan_clip_flags_kernel<<<nb, 256, 0, st>>>(d_ds, counts + 0, ca, cb, fa, fb, n);

@@ -2,11 +2,13 @@
 // raw cloud before every measurement (src/mcl_3dl.cpp:363-383):
 //   1. pcl::VoxelGrid downsample (leaf = params.downsample_x/y/z, :363-367).  PCL is a third-party dependency that is
 //      absent from the reference tree (PCL >= 1.8, version unpinned); restated from its published algorithm
-//      (pcl/filters/impl/voxel_grid.hpp: applyFilter): leaf index = floor(coord * float(1 / leaf)) - floor(min * ...),
-//      linear index x fastest, output in ascending voxel index, one centroid per occupied voxel (float sums; the label is
-//      the majority label of the voxel, lowest on ties, as PCL's CentroidPoint / AccumulatorLabel does).  PCL orders the
-//      points of one voxel with an unstable std::sort, so its float centroid sums are defined only up to summation order:
-//      the device sums in input order.  "Parity unpinned" for this piece (no reference test pins VoxelGrid output).
+//      (pcl/filters/impl/voxel_grid.hpp: applyFilter): non-finite points are skipped (the cloud is treated as not
+//      dense), the lattice comes from the finite points' bounding box, more than INT32_MAX voxels by PCL's own count
+//      leave the cloud unfiltered, leaf index = floor(coord * float(1 / leaf)) - floor(min * ...), linear index x
+//      fastest, output in ascending voxel index, one centroid per occupied voxel (float sums in input order; the label
+//      is the majority label of the voxel, lowest on ties, as PCL's CentroidPoint / AccumulatorLabel does).  PCL
+//      subtracts min_b in float, which equals the integer subtraction here while |coord / leaf| < 2^24.  "Parity
+//      unpinned" for this piece (no reference test pins VoxelGrid output).  Per-point pieces: scan_funcs.cuh.
 //   2. the models' filter(): clip by planar range^2 and z window, order kept
 //      (src/lidar_measurement_model_likelihood.cpp:79-103 == _beam.cpp:98-122) — exact, checked against the oracle;
 //   3. PointCloudUniformSampler::sample (point_cloud_random_samplers/point_cloud_uniform_sampler.h:56-74): `num` draws with
@@ -18,34 +20,66 @@
 #include <stdint.h>
 
 #include "../../include/mcl3dl_b200.h"
-#include "pf_funcs.cuh"
+#include "scan_funcs.cuh"
 
 namespace mcl3dl
 {
-struct VoxelGridDev
+// bounding box of the finite points (getMinMax3D of a cloud that is not dense): bbox[0..2] min, [3..5] max, in the
+// ordered-uint encoding; with no finite point the minimum stays +inf
+__global__ void scan_bbox_kernel(const mcl3dl_point* __restrict__ pts, uint32_t n, uint32_t* __restrict__ bbox)
 {
-  float inv_leaf[3];  // float(1 / leaf), Eigen::Array4f inverse_leaf_size_
-  int min_b[3];       // floor(min * inv_leaf)
-  int div_b[3];
-};
-
-__device__ __forceinline__ uint32_t voxel_key(const VoxelGridDev& g, float x, float y, float z)
-{
-  const int i = __float2int_rd(fmul(x, g.inv_leaf[0])) - g.min_b[0];
-  const int j = __float2int_rd(fmul(y, g.inv_leaf[1])) - g.min_b[1];
-  const int k = __float2int_rd(fmul(z, g.inv_leaf[2])) - g.min_b[2];
-  return static_cast<uint32_t>(i) + static_cast<uint32_t>(j) * g.div_b[0] + static_cast<uint32_t>(k) * g.div_b[0] * g.div_b[1];
+  float mn[3], mx[3];
+#pragma unroll
+  for (int k = 0; k < 3; ++k)
+  {
+    mn[k] = __int_as_float(0x7f800000);
+    mx[k] = __int_as_float(0xff800000);
+  }
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+  {
+    const mcl3dl_point p = pts[i];
+    if (!point_finite(p))
+      continue;
+    const float v[3] = {p.x, p.y, p.z};
+#pragma unroll
+    for (int k = 0; k < 3; ++k)
+    {
+      mn[k] = fminf(mn[k], v[k]);
+      mx[k] = fmaxf(mx[k], v[k]);
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < 3; ++k)
+  {
+    for (int o = 16; o > 0; o >>= 1)
+    {
+      mn[k] = fminf(mn[k], __shfl_xor_sync(0xffffffffu, mn[k], o));
+      mx[k] = fmaxf(mx[k], __shfl_xor_sync(0xffffffffu, mx[k], o));
+    }
+  }
+  if ((threadIdx.x & 31) == 0)
+  {
+#pragma unroll
+    for (int k = 0; k < 3; ++k)
+    {
+      atomicMin(bbox + k, f2ord(mn[k]));
+      atomicMax(bbox + 3 + k, f2ord(mx[k]));
+    }
+  }
 }
 
+// keys / values of the voxel sort (input index) and the (voxel, label) keys of the vote
 __global__ void scan_key_kernel(const mcl3dl_point* __restrict__ pts, uint32_t n, VoxelGridDev g, uint32_t* __restrict__ keys,
-                                uint32_t* __restrict__ vals)
+                                uint32_t* __restrict__ vals, uint64_t* __restrict__ key_label)
 {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n)
     return;
   const mcl3dl_point p = pts[i];
-  keys[i] = voxel_key(g, p.x, p.y, p.z);
+  const uint32_t key = voxel_key(g, p);
+  keys[i] = key;
   vals[i] = i;
+  key_label[i] = voxel_key_label(key, p.label);
 }
 
 // heads of the runs of equal keys (sorted): flag[i] = 1 where a voxel starts
@@ -56,67 +90,25 @@ __global__ void scan_heads_kernel(const uint32_t* __restrict__ keys, uint32_t n,
     flags[i] = (i == 0 || keys[i] != keys[i - 1]) ? 1u : 0u;
 }
 
-// one thread per voxel head: centroid of the run (input order: the sort is stable), majority label
+// one thread per voxel head: scan_voxel_point over the run.  keys / order: sorted by voxel, input order inside one;
+// key_label: sorted by (voxel, label), so the run covers the same positions.  The run of non-finite points (key ==
+// nonfinite_key, last) is no voxel.
 __global__ void scan_centroid_kernel(const mcl3dl_point* __restrict__ pts, const uint32_t* __restrict__ keys,
-                                     const uint32_t* __restrict__ order, const uint32_t* __restrict__ flags,
-                                     const uint32_t* __restrict__ pos /* exclusive scan of flags */, uint32_t n,
-                                     mcl3dl_point* __restrict__ out, uint32_t* __restrict__ n_out)
+                                     const uint32_t* __restrict__ order, const uint64_t* __restrict__ key_label,
+                                     const uint32_t* __restrict__ flags, const uint32_t* __restrict__ pos /* exclusive scan of flags */,
+                                     uint32_t n, uint32_t nonfinite_key, mcl3dl_point* __restrict__ out, uint32_t* __restrict__ n_out)
 {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n)
     return;
-  if (i == n - 1)
-    *n_out = pos[i] + flags[i];
-  if (!flags[i])
-    return;
   const uint32_t key = keys[i];
-  float sx = 0.0f, sy = 0.0f, sz = 0.0f;
-  uint32_t cnt = 0;
-  for (uint32_t j = i; j < n && keys[j] == key; ++j, ++cnt)
-  {
-    const mcl3dl_point p = pts[order[j]];
-    sx = fadd(sx, p.x);
-    sy = fadd(sy, p.y);
-    sz = fadd(sz, p.z);
-  }
-  // majority label, lowest label on ties (AccumulatorLabel: a std::map walked in key order, first maximum)
-  uint32_t best_label = 0xffffffffu, best_cnt = 0;
-  for (uint32_t j = i; j < i + cnt; ++j)
-  {
-    const uint32_t l = pts[order[j]].label;
-    uint32_t c = 0;
-    for (uint32_t k = i; k < i + cnt; ++k) c += pts[order[k]].label == l;
-    if (c > best_cnt || (c == best_cnt && l < best_label))
-    {
-      best_cnt = c;
-      best_label = l;
-    }
-  }
-  mcl3dl_point o;
-  const float fc = static_cast<float>(cnt);
-  o.x = fdiv(sx, fc);
-  o.y = fdiv(sy, fc);
-  o.z = fdiv(sz, fc);
-  o.label = best_label;
-  out[pos[i]] = o;
-}
-
-struct ClipDev
-{
-  float near_sq, far_sq, z_min, z_max;  // clip_near_sq_ = clip_near * clip_near (float), likelihood.cpp:59-60
-};
-
-// local_points_filter of filter(), likelihood.cpp:83-93 / beam.cpp:102-112: true = REMOVE
-__device__ __forceinline__ bool clip_removes(const ClipDev& c, const mcl3dl_point& p)
-{
-  const float r2 = fadd(fmul(p.x, p.x), fmul(p.y, p.y));
-  if (r2 > c.far_sq)
-    return true;
-  if (r2 < c.near_sq)
-    return true;
-  if (p.z < c.z_min || c.z_max < p.z)
-    return true;
-  return false;
+  if (i == n - 1)
+    *n_out = pos[i] + flags[i] - (key == nonfinite_key ? 1u : 0u);
+  if (!flags[i] || key == nonfinite_key)
+    return;
+  uint32_t cnt = 1;
+  while (i + cnt < n && keys[i + cnt] == key) ++cnt;
+  out[pos[i]] = scan_voxel_point(pts, order + i, key_label + i, cnt);
 }
 
 __global__ void scan_clip_flags_kernel(const mcl3dl_point* __restrict__ pts, const uint32_t* __restrict__ n_ptr, ClipDev a, ClipDev b,
@@ -144,7 +136,7 @@ __global__ void scan_compact_kernel(const mcl3dl_point* __restrict__ pts, const 
     out[pos[i]] = pts[i];
 }
 
-// PointCloudUniformSampler::sample: draw t takes clipped point floor(u * n), u from Philox (seed, stream, t)
+// PointCloudUniformSampler::sample: draw t takes clipped point scan_sample_index(seed, stream, t, n)
 __global__ void scan_sample_kernel(const mcl3dl_point* __restrict__ clipped, const uint32_t* __restrict__ n_ptr, uint32_t num,
                                    uint64_t seed, uint32_t stream, mcl3dl_point* __restrict__ out, uint32_t* __restrict__ n_out)
 {
@@ -154,10 +146,7 @@ __global__ void scan_sample_kernel(const mcl3dl_point* __restrict__ clipped, con
     *n_out = n ? num : 0u;  // an empty clipped cloud gives an empty sample (:62-63)
   if (t >= num || n == 0)
     return;
-  uint32_t c[4] = {t, stream, 0x5ca11ab1u, 0u};
-  philox4x32_10(c, static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32));
-  const uint32_t idx = static_cast<uint32_t>((static_cast<uint64_t>(c[0]) * n) >> 32);
-  out[t] = clipped[idx];
+  out[t] = clipped[scan_sample_index(seed, stream, t, n)];
 }
 
 }  // namespace mcl3dl
