@@ -421,10 +421,8 @@ struct mcl3dl_engine
   int timing = 0;               // the per-call timing events of mcl3dl_last_timing cost tens of us per update: off unless
                                 // mcl3dl_collect_timing(eng, 1) or MCL3DL_TIMING=1
   size_t zero_copy_max = 8192;  // the kernels of updates with <= this many particles per device store their records
-                                // straight into the pinned result block (no D2H copy launch); MCL3DL_ZEROCOPY_OUT
-  int update_one_sync = 1;  // mcl3dl_measure_update on ONE device: normalise from the device-side total, one host
-                            // synchronise instead of two (MCL3DL_UPDATE_ONE_SYNC=1; written without GPU time left in
-                            // round 1: off until the f2 parity tests have run with it)
+                                // (or their posterior and weight summaries) straight into the pinned result block (no
+                                // D2H copy launch); MCL3DL_ZEROCOPY_OUT
   int field_mode = 0;  // 1: the likelihood model reads the trilinear distance volume (opt-in, inexact; MCL3DL_LIK_MODE=field)
   size_t field_max_bytes = size_t(24) << 30;  // MCL3DL_FIELD_MAX_MB
   int beam_dq = 2;  // beam kernel: 2 = by job size, 1 = MCL3DL_BEAM=dq, 0 = MCL3DL_BEAM=pl
@@ -498,17 +496,22 @@ void free_buf(DevBuf& b)
   b.cap = 0;
 }
 
-// two zeroed ticket words for the last-CTA folds of the weight-update kernels (they leave them at zero)
-int weight_tickets(mcl3dl_engine* eng, DeviceCtx& c, unsigned int** out)
+// The weight update's grid for n particles and its scratch on one device: w_i, one slot set [nblk per-CTA partials |
+// folded partial] per pass (0, 1) and a zeroed ticket per pass for its last-CTA fold (the kernels leave it at zero)
+int weight_scratch(mcl3dl_engine* eng, DeviceCtx& c, size_t n, int pass, int* nblk, WeightPartial** slots, unsigned int** ticket)
 {
+  *nblk = static_cast<int>(std::min<size_t>((n + kBlockThreads - 1) / kBlockThreads, static_cast<size_t>(c.sm_count) * 4));
+  int rc;
+  if ((rc = reserve(eng, c.d_w, n * 4)) || (rc = reserve(eng, c.d_wpart, 2 * (*nblk + 1) * sizeof(WeightPartial))))
+    return rc;
   if (!c.d_wticket.p)
   {
-    const int rc = reserve(eng, c.d_wticket, 256);
-    if (rc != MCL3DL_OK)
+    if ((rc = reserve(eng, c.d_wticket, 256)))
       return rc;
     CK(cudaMemset(c.d_wticket.p, 0, 256));
   }
-  *out = static_cast<unsigned int*>(c.d_wticket.p);
+  *slots = static_cast<WeightPartial*>(c.d_wpart.p) + pass * (*nblk + 1);
+  *ticket = static_cast<unsigned int*>(c.d_wticket.p) + pass;
   return MCL3DL_OK;
 }
 
@@ -1448,8 +1451,6 @@ int mcl3dl_create(mcl3dl_engine** out, const int* device_ids, int n_devices)
     eng->zero_copy_max = static_cast<size_t>(std::max(std::atol(v), 0L));
   if (const char* v = std::getenv("MCL3DL_DIRECT_MIN_KB"))  // -1: never copy from / to the caller's page-locked arrays in place
     eng->direct_min_bytes = std::atoi(v) < 0 ? ~size_t(0) : static_cast<size_t>(std::atoi(v)) << 10;
-  if (const char* v = std::getenv("MCL3DL_UPDATE_ONE_SYNC"))
-    eng->update_one_sync = std::atoi(v) != 0;
   if (const char* v = std::getenv("MCL3DL_NNF"))
     eng->nnf = std::atoi(v) != 0;
   if (const char* v = std::getenv("MCL3DL_BEAM"))
@@ -1796,7 +1797,10 @@ int mcl3dl_last_timing(const mcl3dl_engine* eng, double* h2d_ms, double* lik_ms,
   return MCL3DL_OK;
 }
 
-static int validate_measure(mcl3dl_engine* eng, size_t P, size_t n_lik, size_t n_beam, size_t n_origins)
+// The arguments every measurement entry point shares.  `host_scans`: the scans are in host memory, so the beam labels,
+// which index the origins (origins[p.label], beam.cpp:142-145), are checked too.
+static int validate_measure(mcl3dl_engine* eng, size_t P, const mcl3dl_point* lik, size_t n_lik, const mcl3dl_point* beam,
+                            size_t n_beam, const float* origins, size_t n_origins, bool host_scans)
 {
   if (!eng)
     return MCL3DL_ERR_INVALID_ARG;
@@ -1808,6 +1812,11 @@ static int validate_measure(mcl3dl_engine* eng, size_t P, size_t n_lik, size_t n
     return MCL3DL_ERR_INVALID_ARG;  // that model's grid was never staged
   if (n_beam && n_origins == 0)
     return MCL3DL_ERR_INVALID_ARG;
+  if ((n_lik && !lik) || (n_beam && (!beam || !origins)))
+    return MCL3DL_ERR_INVALID_ARG;
+  for (size_t j = 0; host_scans && j < n_beam; ++j)
+    if (beam[j].label >= n_origins)
+      return MCL3DL_ERR_INVALID_ARG;
   return MCL3DL_OK;
 }
 
@@ -1853,14 +1862,136 @@ static int launch_models(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_pose* po
   return rc;
 }
 
+// One device's share of the particles of a host-array update and the layout of its pinned block: the inputs [poses |
+// likelihood scan | beam scan | origins | prior | extra] (16-byte sections, as in d_poses), then the outputs [posterior |
+// records | beam status | the WeightPartials of pass 1 and 2].  Absent sections have zero size.
+struct Share
+{
+  size_t p0, n;  // the particles [p0, p0 + n)
+  size_t o_lik, o_beam, o_org, o_prior, o_extra, in_bytes;
+  size_t o_post, o_rec, o_status, o_part, total;
+};
+
+static size_t pad16(size_t b) { return (b + 15) & ~size_t(15); }
+
+// Device d's block of P particles over G devices; per-particle sections in bytes per particle
+static Share share_of(size_t P, size_t G, size_t d, size_t pose_b, size_t n_lik, size_t n_beam, size_t n_origins,
+                      size_t prior_b, size_t extra_b, size_t post_b, size_t rec_b, size_t status_b)
+{
+  Share s;
+  s.p0 = P * d / G;
+  s.n = P * (d + 1) / G - s.p0;
+  s.o_lik = s.n * pose_b;
+  s.o_beam = s.o_lik + n_lik * 16;
+  s.o_org = s.o_beam + n_beam * 16;
+  s.o_prior = s.o_org + pad16(n_origins * 12);
+  s.o_extra = s.o_prior + pad16(s.n * prior_b);
+  s.in_bytes = s.o_extra + pad16(s.n * extra_b);
+  s.o_post = s.in_bytes;
+  s.o_rec = s.o_post + pad16(s.n * post_b);
+  s.o_status = s.o_rec + s.n * rec_b;
+  s.o_part = pad16(s.o_status + s.n * status_b);
+  s.total = s.o_part + 2 * sizeof(WeightPartial) + 64;
+  return s;
+}
+
+// The host inputs into their sections of the pinned block, then ONE H2D copy to d_poses.  Without `poses` the copy starts
+// at the likelihood scan (resident poses, or a page-locked pose array DMA-ed in place).  `timed`: ev[0] before the copy.
+static int stage_inputs(mcl3dl_engine* eng, DeviceCtx& c, const Share& s, const mcl3dl_pose* poses, const mcl3dl_point* lik,
+                        const mcl3dl_point* beam, const float* origins, size_t n_origins, const float* prior, const float* extra,
+                        bool timed)
+{
+  char* hp = static_cast<char*>(c.h_pinned);
+  if (poses) std::memcpy(hp, poses + s.p0, s.o_lik);
+  if (s.o_beam > s.o_lik) std::memcpy(hp + s.o_lik, lik, s.o_beam - s.o_lik);
+  if (s.o_org > s.o_beam) std::memcpy(hp + s.o_beam, beam, s.o_org - s.o_beam);
+  if (n_origins) std::memcpy(hp + s.o_org, origins, n_origins * 12);
+  if (prior) std::memcpy(hp + s.o_prior, prior + s.p0, s.n * 4);
+  if (extra) std::memcpy(hp + s.o_extra, extra + s.p0, s.n * 4);
+  if (timed) CK(cudaEventRecord(c.ev[0], c.stream));
+  const size_t from = poses ? 0 : s.o_lik;
+  if (s.in_bytes > from)
+    CK(cudaMemcpyAsync(static_cast<char*>(c.d_poses.p) + from, hp + from, s.in_bytes - from, cudaMemcpyHostToDevice, c.stream));
+  return MCL3DL_OK;
+}
+
+// Pass 1 of the weight update: w_i into d_w; the folded partial is left at *folded (and stored by the kernel at h_part)
+static int weight_pass1(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_result* rec, const float* prior, const float* extra,
+                        size_t n, size_t n_lik, WeightPartial* h_part, const WeightPartial** folded)
+{
+  int nblk;
+  WeightPartial* slots;
+  unsigned int* tk;
+  if (int rc = weight_scratch(eng, c, n, 0, &nblk, &slots, &tk))
+    return rc;
+  weight_kernel<<<nblk, kBlockThreads, 0, c.stream>>>(rec, prior, extra, static_cast<int>(n), static_cast<int>(n_lik),
+                                                      static_cast<float*>(c.d_w.p), slots, tk, h_part);
+  CK(cudaGetLastError());
+  eng->launches++;
+  *folded = slots + nblk;
+  return MCL3DL_OK;
+}
+
+// Pass 2: p_i = w_i / total into `post`, the total read from `pass1` on the device when given; folded as pass 1
+static int weight_pass2(mcl3dl_engine* eng, DeviceCtx& c, const WeightPartial* pass1, float total, size_t n, size_t index_offset,
+                        float* post, WeightPartial* h_part, const WeightPartial** folded)
+{
+  int nblk;
+  WeightPartial* slots;
+  unsigned int* tk;
+  if (int rc = weight_scratch(eng, c, n, 1, &nblk, &slots, &tk))
+    return rc;
+  normalize_kernel<<<nblk, kBlockThreads, 0, c.stream>>>(static_cast<const float*>(c.d_w.p), static_cast<int>(n), pass1, total,
+                                                         static_cast<int>(index_offset), post, slots, tk, h_part);
+  CK(cudaGetLastError());
+  eng->launches++;
+  *folded = slots + nblk;
+  return MCL3DL_OK;
+}
+
+// The weight update of ONE device: both passes, the total read on the device.  The folded partials come back to
+// h_part[0..1] and the posterior to h_post (if given): stored by the kernels up to zero_copy_max particles, else copied.
+static int fold_weights(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_result* rec, const float* prior, const float* extra,
+                        float* post, size_t n, size_t n_lik, size_t index_offset, WeightPartial* h_part, float* h_post)
+{
+  const bool zc = n <= eng->zero_copy_max;
+  const WeightPartial *f1, *f2;
+  int rc = weight_pass1(eng, c, rec, prior, extra, n, n_lik, zc ? h_part : nullptr, &f1);
+  if (rc != MCL3DL_OK)
+    return rc;
+  rc = weight_pass2(eng, c, f1, 0.0f, n, index_offset, zc && h_post ? h_post : post, zc ? h_part + 1 : nullptr, &f2);
+  if (rc != MCL3DL_OK)
+    return rc;
+  if (!zc)  // (behind both kernels, so that pass 2 does not wait for a copy)
+  {
+    CK(cudaMemcpyAsync(h_part, f1, sizeof(WeightPartial), cudaMemcpyDeviceToHost, c.stream));
+    if (h_post)
+      CK(cudaMemcpyAsync(h_post, post, n * 4, cudaMemcpyDeviceToHost, c.stream));
+    CK(cudaMemcpyAsync(h_part + 1, f2, sizeof(WeightPartial), cudaMemcpyDeviceToHost, c.stream));
+  }
+  return MCL3DL_OK;
+}
+
+// The summary from the partials of pass 1 and 2, folded over the devices
+static void make_summary(const WeightPartial& w1, const WeightPartial& w2, mcl3dl_update_summary* s)
+{
+  std::memset(s, 0, sizeof(*s));
+  s->weight_sum = static_cast<float>(w1.sum);
+  s->match_ratio_min = std::min(1.0f, w1.qmin);
+  s->match_ratio_max = std::max(0.0f, w1.qmax);
+  s->kept = s->weight_sum > 0.0f ? 1 : 0;
+  s->entropy = s->kept ? static_cast<float>(-w2.sum) : 0.0f;
+  s->max_index = s->kept && w2.best > -1.0f ? w2.best_i : 0;
+}
+
 int mcl3dl_measure_device(mcl3dl_engine* eng, const mcl3dl_pose* d_poses, size_t P, const mcl3dl_point* d_lik, size_t n_lik,
                           const mcl3dl_point* d_beam, size_t n_beam, const float* d_origins_xyz, size_t n_origins,
                           mcl3dl_result* d_out, void* cuda_stream)
 {
-  int rc = validate_measure(eng, P, n_lik, n_beam, n_origins);
+  int rc = validate_measure(eng, P, d_lik, n_lik, d_beam, n_beam, d_origins_xyz, n_origins, false);
   if (rc != MCL3DL_OK)
     return rc;
-  if (eng->devs.size() != 1 || (P && (!d_poses || !d_out)) || (n_lik && !d_lik) || (n_beam && (!d_beam || !d_origins_xyz)))
+  if (eng->devs.size() != 1 || (P && (!d_poses || !d_out)))
     return MCL3DL_ERR_INVALID_ARG;
   if (P == 0)
     return MCL3DL_OK;
@@ -1955,17 +2086,15 @@ int mcl3dl_particles_resample(mcl3dl_engine* eng, const float sigma_pos[3], cons
 }
 
 // The resident update with every input already on the device: pose pack -> both models -> prior * likelihood * odometry
-// term -> normalise; one synchronise.  `stage` = bytes of host inputs waiting in the pinned block for one H2D copy.
+// term -> normalise; one synchronise.  `s`: the pinned block's layout, whose inputs are already on their way up.
 static int resident_update(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_point* d_lik, size_t n_lik, const mcl3dl_point* d_beam,
-                           size_t n_beam, const float* d_org, size_t n_origins, float odom_err_lin_sigma, size_t pinned_off,
+                           size_t n_beam, const float* d_org, size_t n_origins, float odom_err_lin_sigma, const Share& s,
                            mcl3dl_update_summary* summary)
 {
   const size_t P = c.r_n;
   cudaStream_t st = c.stream;
-  int rc;
-  const int nblk = static_cast<int>(std::min<size_t>((P + kBlockThreads - 1) / kBlockThreads, static_cast<size_t>(c.sm_count) * 4));
-  if ((rc = reserve(eng, c.d_out, P * sizeof(mcl3dl_result))) || (rc = reserve(eng, c.d_w, P * 4)) ||
-      (rc = reserve(eng, c.d_wpart, 2 * (nblk + 1) * sizeof(WeightPartial))))
+  int rc = reserve(eng, c.d_out, P * sizeof(mcl3dl_result));
+  if (rc != MCL3DL_OK)
     return rc;
   // NormalLikelihood(sigma): a_ = float(1 / sqrt(2 pi s^2)), sq2_ = float(2 s^2) (include/mcl_3dl/nd.h:45-49)
   const bool with_odom = odom_err_lin_sigma > 0.0f;
@@ -1978,39 +2107,21 @@ static int resident_update(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_point*
                                                   with_odom ? static_cast<float*>(c.r_extra.p) : nullptr);
   CK(cudaGetLastError());
   eng->launches++;
+  mcl3dl_result* d_rec = static_cast<mcl3dl_result*>(c.d_out.p);
   rc = launch_models(eng, c, static_cast<const mcl3dl_pose*>(c.r_poses.p), P, d_lik, n_lik, d_beam, n_beam, d_org, n_origins,
-                     static_cast<mcl3dl_result*>(c.d_out.p), nullptr, st, false);
+                     d_rec, nullptr, st, false);
   if (rc != MCL3DL_OK)
     return rc;
   // prior * likelihood from the resident probabilities; the posterior is written over them (the weights were read
   // into d_w first); a vanished total leaves them untouched = the reference's "restore" (pf.h:274-278)
-  WeightPartial* parts = static_cast<WeightPartial*>(c.d_wpart.p);
-  WeightPartial* parts2 = parts + nblk + 1;
-  unsigned int* tk;
-  if ((rc = weight_tickets(eng, c, &tk)))
+  float* prob = static_cast<float*>(c.r_prob.p);
+  WeightPartial* h_part = reinterpret_cast<WeightPartial*>(static_cast<char*>(c.h_pinned) + s.o_part);
+  rc = fold_weights(eng, c, d_rec, prob, with_odom ? static_cast<const float*>(c.r_extra.p) : nullptr, prob, P, n_lik, 0, h_part,
+                    nullptr);
+  if (rc != MCL3DL_OK)
     return rc;
-  weight_kernel<<<nblk, kBlockThreads, 0, st>>>(static_cast<const mcl3dl_result*>(c.d_out.p), static_cast<const float*>(c.r_prob.p),
-                                               with_odom ? static_cast<const float*>(c.r_extra.p) : nullptr, static_cast<int>(P),
-                                               static_cast<int>(n_lik), static_cast<float*>(c.d_w.p), parts, tk, nullptr);
-  normalize_kernel_dev<<<nblk, kBlockThreads, 0, st>>>(static_cast<const float*>(c.d_w.p), static_cast<int>(P), parts + nblk, 0,
-                                                      static_cast<float*>(c.r_prob.p), parts2, tk + 1, nullptr);
-  CK(cudaGetLastError());
-  eng->launches += 2;
-  char* h_tot = static_cast<char*>(c.h_pinned) + pinned_off;
-  CK(cudaMemcpyAsync(h_tot, parts + nblk, sizeof(WeightPartial), cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(h_tot + sizeof(WeightPartial), parts2 + nblk, sizeof(WeightPartial), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
-  WeightPartial w1, w2;
-  std::memcpy(&w1, h_tot, sizeof(w1));
-  std::memcpy(&w2, h_tot + sizeof(w1), sizeof(w2));
-  std::memset(summary, 0, sizeof(*summary));
-  const float total_f = static_cast<float>(w1.sum);
-  summary->weight_sum = total_f;
-  summary->match_ratio_min = std::min(1.0f, w1.qmin);
-  summary->match_ratio_max = std::max(0.0f, w1.qmax);
-  summary->kept = total_f > 0.0f ? 1 : 0;
-  summary->entropy = summary->kept ? static_cast<float>(-w2.sum) : 0.0f;
-  summary->max_index = summary->kept ? w2.best_i : 0;
+  make_summary(h_part[0], h_part[1], summary);
   return MCL3DL_OK;
 }
 
@@ -2022,27 +2133,21 @@ int mcl3dl_particles_measure_update(mcl3dl_engine* eng, const mcl3dl_point* lik_
     return MCL3DL_ERR_INVALID_ARG;
   DeviceCtx& c = eng->devs[0];
   const size_t P = c.r_n;
-  int rc = validate_measure(eng, P, n_lik, n_beam, n_origins);
+  int rc = validate_measure(eng, P, lik_pts, n_lik, beam_pts, n_beam, origins_xyz, n_origins, true);
   if (rc != MCL3DL_OK)
     return rc;
-  if (P == 0 || (n_lik && !lik_pts) || (n_beam && (!beam_pts || !origins_xyz)))
+  if (P == 0)
     return MCL3DL_ERR_INVALID_ARG;
-  for (size_t j = 0; j < n_beam; ++j)
-    if (beam_pts[j].label >= n_origins)
-      return MCL3DL_ERR_INVALID_ARG;
   CK(cudaSetDevice(c.dev));
   // scans + origins up in one block (as in mcl3dl_measure); the poses come from the resident states
-  const size_t o_beam = n_lik * 16, o_org = o_beam + n_beam * 16, in_bytes = o_org + ((n_origins * 12 + 15) & ~size_t(15));
-  if ((rc = reserve_pinned(eng, c, in_bytes + 2 * sizeof(WeightPartial) + 64)) || (rc = reserve(eng, c.d_poses, in_bytes + 16)))
+  const Share s = share_of(P, 1, 0, 0, n_lik, n_beam, n_origins, 0, 0, 0, 0, 0);
+  if ((rc = reserve_pinned(eng, c, s.total)) || (rc = reserve(eng, c.d_poses, s.in_bytes)) ||
+      (rc = stage_inputs(eng, c, s, nullptr, lik_pts, beam_pts, origins_xyz, n_origins, nullptr, nullptr, false)))
     return rc;
-  char* hp = static_cast<char*>(c.h_pinned);
-  if (n_lik) std::memcpy(hp, lik_pts, n_lik * 16);
-  if (n_beam) std::memcpy(hp + o_beam, beam_pts, n_beam * 16);
-  if (n_origins) std::memcpy(hp + o_org, origins_xyz, n_origins * 12);
-  if (in_bytes) CK(cudaMemcpyAsync(c.d_poses.p, hp, in_bytes, cudaMemcpyHostToDevice, c.stream));
   const char* d_in = static_cast<const char*>(c.d_poses.p);
-  return resident_update(eng, c, reinterpret_cast<const mcl3dl_point*>(d_in), n_lik, reinterpret_cast<const mcl3dl_point*>(d_in + o_beam),
-                         n_beam, reinterpret_cast<const float*>(d_in + o_org), n_origins, odom_err_lin_sigma, in_bytes, summary);
+  return resident_update(eng, c, reinterpret_cast<const mcl3dl_point*>(d_in + s.o_lik), n_lik,
+                         reinterpret_cast<const mcl3dl_point*>(d_in + s.o_beam), n_beam,
+                         reinterpret_cast<const float*>(d_in + s.o_org), n_origins, odom_err_lin_sigma, s, summary);
 }
 
 int mcl3dl_particles_measure_update_prepared(mcl3dl_engine* eng, const float* origins_xyz, size_t n_origins, float odom_err_lin_sigma,
@@ -2054,23 +2159,22 @@ int mcl3dl_particles_measure_update_prepared(mcl3dl_engine* eng, const float* or
   if (!c.s_valid)
     return MCL3DL_ERR_INVALID_ARG;  // no mcl3dl_scan_prepare before
   const size_t P = c.r_n, n_lik = c.s_info.n_lik, n_beam = c.s_info.n_beam;
-  int rc = validate_measure(eng, P, n_lik, n_beam, n_origins);
+  const mcl3dl_point* d_lik = static_cast<const mcl3dl_point*>(c.s_out[0].p);
+  const mcl3dl_point* d_beam = static_cast<const mcl3dl_point*>(c.s_out[1].p);
+  int rc = validate_measure(eng, P, d_lik, n_lik, d_beam, n_beam, origins_xyz, n_origins, false);
   if (rc != MCL3DL_OK)
     return rc;
-  if (P == 0 || (n_beam && !origins_xyz))
+  if (P == 0)
     return MCL3DL_ERR_INVALID_ARG;
   CK(cudaSetDevice(c.dev));
-  const size_t in_bytes = (n_origins * 12 + 15) & ~size_t(15);
-  if ((rc = reserve_pinned(eng, c, in_bytes + 2 * sizeof(WeightPartial) + 64)) || (rc = reserve(eng, c.d_poses, in_bytes + 16)))
+  // only the origins go up; the scans are the prepared ones
+  const Share s = share_of(P, 1, 0, 0, 0, 0, n_origins, 0, 0, 0, 0, 0);
+  if ((rc = reserve_pinned(eng, c, s.total)) || (rc = reserve(eng, c.d_poses, s.in_bytes)) ||
+      (rc = stage_inputs(eng, c, s, nullptr, nullptr, nullptr, origins_xyz, n_origins, nullptr, nullptr, false)))
     return rc;
-  if (n_origins)
-  {
-    std::memcpy(c.h_pinned, origins_xyz, n_origins * 12);
-    CK(cudaMemcpyAsync(c.d_poses.p, c.h_pinned, in_bytes, cudaMemcpyHostToDevice, c.stream));
-  }
   // (beam labels are the raw cloud's, voted per voxel: the caller's origins must cover them, as in the node)
-  return resident_update(eng, c, static_cast<const mcl3dl_point*>(c.s_out[0].p), n_lik, static_cast<const mcl3dl_point*>(c.s_out[1].p),
-                         n_beam, static_cast<const float*>(c.d_poses.p), n_origins, odom_err_lin_sigma, in_bytes, summary);
+  return resident_update(eng, c, d_lik, n_lik, d_beam, n_beam, static_cast<const float*>(c.d_poses.p), n_origins, odom_err_lin_sigma,
+                         s, summary);
 }
 
 // ---- scan preprocessing on the device (scan_kernels.cuh)
@@ -2383,10 +2487,10 @@ int mcl3dl_measure_exchange_device(mcl3dl_engine* eng, const mcl3dl_pose* d_pose
                                    size_t n_lik, const mcl3dl_point* d_beam, size_t n_beam, const float* d_origins_xyz,
                                    size_t n_origins, void* cuda_stream, const mcl3dl_result** d_all_out)
 {
-  int rc = validate_measure(eng, P, n_lik, n_beam, n_origins);
+  int rc = validate_measure(eng, P, d_lik, n_lik, d_beam, n_beam, d_origins_xyz, n_origins, false);
   if (rc != MCL3DL_OK)
     return rc;
-  if (eng->devs.size() != 1 || !d_poses || (n_lik && !d_lik) || (n_beam && (!d_beam || !d_origins_xyz)))
+  if (eng->devs.size() != 1 || !d_poses)
     return MCL3DL_ERR_INVALID_ARG;
   DeviceCtx& c = eng->devs[0];
   if (!c.x_ready || P != c.x_local)
@@ -2429,75 +2533,59 @@ static int measure_host(mcl3dl_engine* eng, const mcl3dl_pose* poses, size_t P, 
                         const mcl3dl_point* beam_pts, size_t n_beam, const float* origins_xyz, size_t n_origins,
                         mcl3dl_result* out, uint8_t* status)
 {
-  int rc = validate_measure(eng, P, n_lik, n_beam, n_origins);
+  int rc = validate_measure(eng, P, lik_pts, n_lik, beam_pts, n_beam, origins_xyz, n_origins, true);
   if (rc != MCL3DL_OK)
     return rc;
-  if ((P && (!poses || (!out && !status))) || (n_lik && !lik_pts) || (n_beam && (!beam_pts || !origins_xyz)))
+  if (P && (!poses || (!out && !status)))
     return MCL3DL_ERR_INVALID_ARG;
-  for (size_t j = 0; j < n_beam; ++j)
-    if (beam_pts[j].label >= n_origins)  // origins[p.label], beam.cpp:142-145
-      return MCL3DL_ERR_INVALID_ARG;
   if (P == 0)
     return MCL3DL_OK;
   const size_t G = eng->devs.size();
-  std::vector<size_t> p0(G + 1);
-  for (size_t d = 0; d <= G; ++d) p0[d] = P * d / G;
+  std::vector<Share> sh(G);
+  const bool timed = eng->timing != 0;
+  // caller arrays inside a mcl3dl_host_alloc block are page-locked: a large pose array is DMA-ed from where it lies
+  // and the records land where the caller reads them, without the staging memcpy on either side
+  auto out_direct = [&](const Share& s) {
+    return out && eng->direct_min_bytes != ~size_t(0) && in_host_block(eng, out + s.p0, s.n * sizeof(mcl3dl_result));
+  };
   // enqueue everything on every device, then wait
   for (size_t d = 0; d < G; ++d)
   {
     DeviceCtx& c = eng->devs[d];
-    const size_t Pd = p0[d + 1] - p0[d];
-    if (Pd == 0)
+    const Share& s = sh[d] = share_of(P, G, d, sizeof(mcl3dl_pose), n_lik, n_beam, n_origins, 0, 0, 0, sizeof(mcl3dl_result),
+                                      status ? n_beam : 0);
+    if (s.n == 0)
       continue;
     CK(cudaSetDevice(c.dev));
     cudaStream_t st = c.stream;
-    const size_t b_poses = Pd * sizeof(mcl3dl_pose), b_lik = n_lik * 16, b_beam = n_beam * 16, b_org = (n_origins * 12 + 15) & ~size_t(15);
-    const size_t b_out = Pd * sizeof(mcl3dl_result), b_status = status ? Pd * n_beam : 0;
-    const size_t o_lik = b_poses, o_beam = o_lik + b_lik, o_org = o_beam + b_beam, o_out = o_org + b_org;
-    const size_t o_status = o_out + b_out;
-    rc = reserve_pinned(eng, c, o_status + b_status + 64);
-    if (rc != MCL3DL_OK) return rc;
-    // one staging block, one H2D copy: [poses | likelihood scan | beam scan | origins] (all 16-byte multiples)
-    if ((rc = reserve(eng, c.d_poses, o_out)) || (rc = reserve(eng, c.d_out, b_out)) || (rc = reserve(eng, c.d_status, b_status)))
+    const size_t b_rec = s.n * sizeof(mcl3dl_result), b_status = status ? s.n * n_beam : 0;
+    const bool poses_direct = s.o_lik >= eng->direct_min_bytes && in_host_block(eng, poses + s.p0, s.o_lik);
+    if ((rc = reserve_pinned(eng, c, s.total)) || (rc = reserve(eng, c.d_poses, s.in_bytes)) ||
+        (rc = reserve(eng, c.d_out, b_rec)) || (rc = reserve(eng, c.d_status, b_status)) ||
+        (rc = stage_inputs(eng, c, s, poses_direct ? nullptr : poses, lik_pts, beam_pts, origins_xyz, n_origins, nullptr,
+                           nullptr, timed)))
       return rc;
-    char* hp = static_cast<char*>(c.h_pinned);
-    // caller arrays inside a mcl3dl_host_alloc block are page-locked: a large pose array is DMA-ed from where it lies
-    // and the records land where the caller reads them, without the staging memcpy on either side
-    const bool poses_direct = b_poses >= eng->direct_min_bytes && in_host_block(eng, poses + p0[d], b_poses);
-    const bool out_direct = out && eng->direct_min_bytes != ~size_t(0) && in_host_block(eng, out + p0[d], b_out);
-    if (!poses_direct) std::memcpy(hp, poses + p0[d], b_poses);
-    if (b_lik) std::memcpy(hp + o_lik, lik_pts, b_lik);
-    if (b_beam) std::memcpy(hp + o_beam, beam_pts, b_beam);
-    if (n_origins) std::memcpy(hp + o_org, origins_xyz, n_origins * 12);
-    const bool timed = eng->timing != 0;
+    if (poses_direct)
+      CK(cudaMemcpyAsync(c.d_poses.p, poses + s.p0, s.o_lik, cudaMemcpyHostToDevice, st));
+    if (timed) CK(cudaEventRecord(c.ev[1], st));
     // small updates: the kernels store their records straight into the pinned block (cudaMallocHost memory is mapped
     // into the unified address space), which saves the D2H copy launch; large ones keep the bulk copy
-    const bool zc = !status && Pd <= eng->zero_copy_max;  // (per-ray status bytes would be scattered 1-byte PCIe writes)
-    if (timed) CK(cudaEventRecord(c.ev[0], st));
-    if (poses_direct)
-    {
-      CK(cudaMemcpyAsync(c.d_poses.p, poses + p0[d], b_poses, cudaMemcpyHostToDevice, st));
-      if (o_out > o_lik)
-        CK(cudaMemcpyAsync(static_cast<char*>(c.d_poses.p) + o_lik, hp + o_lik, o_out - o_lik, cudaMemcpyHostToDevice, st));
-    }
-    else
-      CK(cudaMemcpyAsync(c.d_poses.p, hp, o_out, cudaMemcpyHostToDevice, st));
-    const char* d_in = static_cast<const char*>(c.d_poses.p);
-    const mcl3dl_pose* d_poses = reinterpret_cast<const mcl3dl_pose*>(d_in);
-    const mcl3dl_point* d_lik = reinterpret_cast<const mcl3dl_point*>(d_in + o_lik);
-    const mcl3dl_point* d_beam = reinterpret_cast<const mcl3dl_point*>(d_in + o_beam);
-    const float* d_org = reinterpret_cast<const float*>(d_in + o_org);
-    if (timed) CK(cudaEventRecord(c.ev[1], st));
-    mcl3dl_result* h_out = out_direct ? out + p0[d] : reinterpret_cast<mcl3dl_result*>(hp + o_out);
+    const bool zc = !status && s.n <= eng->zero_copy_max;  // (per-ray status bytes would be scattered 1-byte PCIe writes)
+    char* hp = static_cast<char*>(c.h_pinned);
+    mcl3dl_result* h_out = out_direct(s) ? out + s.p0 : reinterpret_cast<mcl3dl_result*>(hp + s.o_rec);
     mcl3dl_result* k_out = zc ? h_out : static_cast<mcl3dl_result*>(c.d_out.p);
-    uint8_t* k_status = status ? static_cast<uint8_t*>(c.d_status.p) : nullptr;
-    rc = launch_models(eng, c, d_poses, Pd, d_lik, n_lik, d_beam, n_beam, d_org, n_origins, k_out, k_status, st, timed);
-    if (rc != MCL3DL_OK) return rc;
+    const char* d_in = static_cast<const char*>(c.d_poses.p);
+    rc = launch_models(eng, c, reinterpret_cast<const mcl3dl_pose*>(d_in), s.n, reinterpret_cast<const mcl3dl_point*>(d_in + s.o_lik),
+                       n_lik, reinterpret_cast<const mcl3dl_point*>(d_in + s.o_beam), n_beam,
+                       reinterpret_cast<const float*>(d_in + s.o_org), n_origins, k_out,
+                       status ? static_cast<uint8_t*>(c.d_status.p) : nullptr, st, timed);
+    if (rc != MCL3DL_OK)
+      return rc;
     if (timed) CK(cudaEventRecord(c.ev[5], st));
     if (!zc)
     {
-      CK(cudaMemcpyAsync(h_out, c.d_out.p, b_out, cudaMemcpyDeviceToHost, st));
-      if (b_status) CK(cudaMemcpyAsync(hp + o_status, c.d_status.p, b_status, cudaMemcpyDeviceToHost, st));
+      CK(cudaMemcpyAsync(h_out, c.d_out.p, b_rec, cudaMemcpyDeviceToHost, st));
+      if (b_status) CK(cudaMemcpyAsync(hp + s.o_status, c.d_status.p, b_status, cudaMemcpyDeviceToHost, st));
     }
     if (timed) CK(cudaEventRecord(c.ev[4], st));
   }
@@ -2505,19 +2593,17 @@ static int measure_host(mcl3dl_engine* eng, const mcl3dl_pose* poses, size_t P, 
   for (size_t d = 0; d < G; ++d)
   {
     DeviceCtx& c = eng->devs[d];
-    const size_t Pd = p0[d + 1] - p0[d];
-    if (Pd == 0)
+    const Share& s = sh[d];
+    if (s.n == 0)
       continue;
     CK(cudaSetDevice(c.dev));
     CK(cudaStreamSynchronize(c.stream));
-    const size_t o_out = Pd * sizeof(mcl3dl_pose) + n_lik * 16 + n_beam * 16 + ((n_origins * 12 + 15) & ~size_t(15));
-    const size_t o_status = o_out + Pd * sizeof(mcl3dl_result);
     const char* hp = static_cast<const char*>(c.h_pinned);
-    if (out && !(eng->direct_min_bytes != ~size_t(0) && in_host_block(eng, out + p0[d], Pd * sizeof(mcl3dl_result))))  // (else: already there)
-      std::memcpy(out + p0[d], hp + o_out, Pd * sizeof(mcl3dl_result));
-    if (status) std::memcpy(status + p0[d] * n_beam, hp + o_status, Pd * n_beam);
+    if (out && !out_direct(s))  // (else: already there)
+      std::memcpy(out + s.p0, hp + s.o_rec, s.n * sizeof(mcl3dl_result));
+    if (status) std::memcpy(status + s.p0 * n_beam, hp + s.o_status, s.n * n_beam);
     float ms_h2d = 0, ms_lik = 0, ms_beam = 0, ms_d2h = 0;
-    if (eng->timing)
+    if (timed)
     {
       CK(cudaEventElapsedTime(&ms_h2d, c.ev[0], c.ev[1]));
       CK(cudaEventElapsedTime(&ms_lik, c.ev[2], c.ev[3]));
@@ -2537,190 +2623,118 @@ int mcl3dl_measure_update(mcl3dl_engine* eng, const mcl3dl_pose* poses, size_t P
                           const float* prior, const float* extra, float* posterior, mcl3dl_result* records,
                           mcl3dl_update_summary* summary)
 {
-  int rc = validate_measure(eng, P, n_lik, n_beam, n_origins);
+  int rc = validate_measure(eng, P, lik_pts, n_lik, beam_pts, n_beam, origins_xyz, n_origins, true);
   if (rc != MCL3DL_OK)
     return rc;
-  if (!summary || (P && (!poses || !prior || !posterior)) || (n_lik && !lik_pts) || (n_beam && (!beam_pts || !origins_xyz)))
+  if (!summary || (P && (!poses || !prior || !posterior)))
     return MCL3DL_ERR_INVALID_ARG;
-  for (size_t j = 0; j < n_beam; ++j)
-    if (beam_pts[j].label >= n_origins)
-      return MCL3DL_ERR_INVALID_ARG;
-  std::memset(summary, 0, sizeof(*summary));
-  summary->match_ratio_min = 1.0f;
-  if (P == 0)
-    return MCL3DL_OK;
   const size_t G = eng->devs.size();
-  std::vector<size_t> p0(G + 1);
-  for (size_t d = 0; d <= G; ++d) p0[d] = P * d / G;
-  struct Lay
-  {
-    size_t o_lik, o_beam, o_org, o_prior, o_extra, in_bytes, o_post, o_rec, o_part, total;
-    int nblk;
-    bool zc;
-  };
-  std::vector<Lay> lay(G);
-  // One device: the total never leaves the device (normalize_kernel_dev reads pass 1's folded slot) and everything comes
-  // back after ONE synchronise; small updates store the posterior, the records and the two summaries straight into the
-  // pinned block (no D2H copy launches).  Several devices: the total is a sum over devices, so two host round trips.
-  const bool one_sync = eng->update_one_sync && G == 1;
-  // ---- pass 1 on every device: inputs up, both models, w_i and its reduction
+  std::vector<Share> sh(G);
+  // ---- pass 1 on every device: inputs up, both models, w_i and its reduction.  One device: the whole weight update,
+  // ONE synchronise.  Several devices: the total is a sum over devices, so pass 2 follows a host round trip.
   for (size_t d = 0; d < G; ++d)
   {
     DeviceCtx& c = eng->devs[d];
-    const size_t Pd = p0[d + 1] - p0[d];
-    if (Pd == 0)
+    const Share& s = sh[d] = share_of(P, G, d, sizeof(mcl3dl_pose), n_lik, n_beam, n_origins, 4, extra ? 4 : 0, 4,
+                                      records ? sizeof(mcl3dl_result) : 0, 0);
+    if (s.n == 0)
       continue;
     CK(cudaSetDevice(c.dev));
     cudaStream_t st = c.stream;
-    Lay& L = lay[d];
-    L.o_lik = Pd * sizeof(mcl3dl_pose);
-    L.o_beam = L.o_lik + n_lik * 16;
-    L.o_org = L.o_beam + n_beam * 16;
-    L.o_prior = L.o_org + ((n_origins * 12 + 15) & ~size_t(15));
-    L.o_extra = L.o_prior + ((Pd * 4 + 15) & ~size_t(15));
-    L.in_bytes = L.o_extra + (extra ? ((Pd * 4 + 15) & ~size_t(15)) : 0);
-    L.o_post = L.in_bytes;
-    L.o_rec = L.o_post + ((Pd * 4 + 15) & ~size_t(15));
-    L.o_part = (L.o_rec + (records ? Pd * sizeof(mcl3dl_result) : 0) + 15) & ~size_t(15);
-    L.total = L.o_part + 2 * sizeof(WeightPartial) + 64;
-    L.nblk = static_cast<int>(std::min<size_t>((Pd + kBlockThreads - 1) / kBlockThreads, static_cast<size_t>(c.sm_count) * 4));
-    L.zc = one_sync && Pd <= eng->zero_copy_max;
-    unsigned int* tk;
-    if ((rc = reserve_pinned(eng, c, L.total)) || (rc = reserve(eng, c.d_poses, L.in_bytes)) ||
-        (rc = reserve(eng, c.d_out, Pd * sizeof(mcl3dl_result))) || (rc = reserve(eng, c.d_w, Pd * 4)) ||
-        (rc = reserve(eng, c.d_post, Pd * 4)) || (rc = reserve(eng, c.d_wpart, 2 * (L.nblk + 1) * sizeof(WeightPartial))) ||
-        (rc = weight_tickets(eng, c, &tk)))
+    if ((rc = reserve_pinned(eng, c, s.total)) || (rc = reserve(eng, c.d_poses, s.in_bytes)) ||
+        (rc = reserve(eng, c.d_out, s.n * sizeof(mcl3dl_result))) || (rc = reserve(eng, c.d_post, s.n * 4)) ||
+        (rc = stage_inputs(eng, c, s, poses, lik_pts, beam_pts, origins_xyz, n_origins, prior, extra, false)))
       return rc;
-    char* hp = static_cast<char*>(c.h_pinned);
-    std::memcpy(hp, poses + p0[d], Pd * sizeof(mcl3dl_pose));
-    if (n_lik) std::memcpy(hp + L.o_lik, lik_pts, n_lik * 16);
-    if (n_beam) std::memcpy(hp + L.o_beam, beam_pts, n_beam * 16);
-    if (n_origins) std::memcpy(hp + L.o_org, origins_xyz, n_origins * 12);
-    std::memcpy(hp + L.o_prior, prior + p0[d], Pd * 4);
-    if (extra) std::memcpy(hp + L.o_extra, extra + p0[d], Pd * 4);
-    CK(cudaMemcpyAsync(c.d_poses.p, hp, L.in_bytes, cudaMemcpyHostToDevice, st));
     const char* d_in = static_cast<const char*>(c.d_poses.p);
-    // zero-copy: the model kernels store the records where the caller's copy is taken from (they are read again by
-    // weight_kernel over PCIe only when they live in host memory, so that is limited to the case the caller wants them)
-    mcl3dl_result* k_rec = (L.zc && records) ? reinterpret_cast<mcl3dl_result*>(hp + L.o_rec) : static_cast<mcl3dl_result*>(c.d_out.p);
-    rc = launch_models(eng, c, reinterpret_cast<const mcl3dl_pose*>(d_in), Pd, reinterpret_cast<const mcl3dl_point*>(d_in + L.o_lik),
-                       n_lik, reinterpret_cast<const mcl3dl_point*>(d_in + L.o_beam), n_beam,
-                       reinterpret_cast<const float*>(d_in + L.o_org), n_origins, static_cast<mcl3dl_result*>(c.d_out.p),
-                       nullptr, st, false);
-    (void)k_rec;
+    const float* d_prior = reinterpret_cast<const float*>(d_in + s.o_prior);
+    const float* d_extra = extra ? reinterpret_cast<const float*>(d_in + s.o_extra) : nullptr;
+    mcl3dl_result* d_rec = static_cast<mcl3dl_result*>(c.d_out.p);
+    char* hp = static_cast<char*>(c.h_pinned);
+    WeightPartial* h_part = reinterpret_cast<WeightPartial*>(hp + s.o_part);
+    rc = launch_models(eng, c, reinterpret_cast<const mcl3dl_pose*>(d_in), s.n, reinterpret_cast<const mcl3dl_point*>(d_in + s.o_lik),
+                       n_lik, reinterpret_cast<const mcl3dl_point*>(d_in + s.o_beam), n_beam,
+                       reinterpret_cast<const float*>(d_in + s.o_org), n_origins, d_rec, nullptr, st, false);
     if (rc != MCL3DL_OK)
       return rc;
-    WeightPartial* parts = static_cast<WeightPartial*>(c.d_wpart.p);
-    WeightPartial* h_part = reinterpret_cast<WeightPartial*>(hp + L.o_part);
-    weight_kernel<<<L.nblk, kBlockThreads, 0, st>>>(static_cast<const mcl3dl_result*>(c.d_out.p),
-                                                   reinterpret_cast<const float*>(d_in + L.o_prior),
-                                                   extra ? reinterpret_cast<const float*>(d_in + L.o_extra) : nullptr,
-                                                   static_cast<int>(Pd), static_cast<int>(n_lik), static_cast<float*>(c.d_w.p), parts,
-                                                   tk, L.zc ? h_part : nullptr);
-    CK(cudaGetLastError());
-    eng->launches += 1;
-    if (!L.zc)
-      CK(cudaMemcpyAsync(h_part, parts + L.nblk, sizeof(WeightPartial), cudaMemcpyDeviceToHost, st));
-    if (one_sync)
+    if (G == 1)
     {
-      // pass 2 right behind pass 1 (its partial slots live after pass 1's)
-      WeightPartial* parts2 = parts + L.nblk + 1;
-      float* k_post = L.zc ? reinterpret_cast<float*>(hp + L.o_post) : static_cast<float*>(c.d_post.p);
-      normalize_kernel_dev<<<L.nblk, kBlockThreads, 0, st>>>(static_cast<const float*>(c.d_w.p), static_cast<int>(Pd), parts + L.nblk,
-                                                            static_cast<int>(p0[d]), k_post, parts2, tk + 1,
-                                                            L.zc ? h_part + 1 : nullptr);
-      CK(cudaGetLastError());
-      eng->launches += 1;
-      if (!L.zc)
-      {
-        CK(cudaMemcpyAsync(hp + L.o_post, c.d_post.p, Pd * 4, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(h_part + 1, parts2 + L.nblk, sizeof(WeightPartial), cudaMemcpyDeviceToHost, st));
-      }
+      if ((rc = fold_weights(eng, c, d_rec, d_prior, d_extra, static_cast<float*>(c.d_post.p), s.n, n_lik, s.p0, h_part,
+                             reinterpret_cast<float*>(hp + s.o_post))))
+        return rc;
       if (records)
-        CK(cudaMemcpyAsync(hp + L.o_rec, c.d_out.p, Pd * sizeof(mcl3dl_result), cudaMemcpyDeviceToHost, st));
-    }
-  }
-  double total = 0.0;
-  float qmin = 1.0f, qmax = 0.0f;
-  for (size_t d = 0; d < G; ++d)
-  {
-    DeviceCtx& c = eng->devs[d];
-    if (p0[d + 1] == p0[d])
-      continue;
-    CK(cudaSetDevice(c.dev));
-    CK(cudaStreamSynchronize(c.stream));
-    WeightPartial wp;
-    std::memcpy(&wp, static_cast<const char*>(c.h_pinned) + lay[d].o_part, sizeof(wp));
-    total += wp.sum;  // device order: deterministic
-    qmin = std::min(qmin, wp.qmin);
-    qmax = std::max(qmax, wp.qmax);
-  }
-  const float total_f = static_cast<float>(total);
-  summary->weight_sum = total_f;
-  summary->match_ratio_min = qmin;
-  summary->match_ratio_max = qmax;
-  summary->kept = total_f > 0.0f ? 1 : 0;
-  // ---- pass 2 (several devices): normalise with the global total, entropy, arg max; only 4 B per particle come back
-  for (size_t d = 0; d < G && !one_sync; ++d)
-  {
-    DeviceCtx& c = eng->devs[d];
-    const size_t Pd = p0[d + 1] - p0[d];
-    if (Pd == 0)
-      continue;
-    CK(cudaSetDevice(c.dev));
-    cudaStream_t st = c.stream;
-    Lay& L = lay[d];
-    char* hp = static_cast<char*>(c.h_pinned);
-    WeightPartial* parts = static_cast<WeightPartial*>(c.d_wpart.p);
-    unsigned int* tk;
-    if ((rc = weight_tickets(eng, c, &tk)))
-      return rc;
-    if (summary->kept)
-    {
-      normalize_kernel<<<L.nblk, kBlockThreads, 0, st>>>(static_cast<const float*>(c.d_w.p), static_cast<int>(Pd), total_f,
-                                                        static_cast<int>(p0[d]), static_cast<float*>(c.d_post.p), parts, tk, nullptr);
-      CK(cudaGetLastError());
-      eng->launches += 1;
-      CK(cudaMemcpyAsync(hp + L.o_post, c.d_post.p, Pd * 4, cudaMemcpyDeviceToHost, st));
-      CK(cudaMemcpyAsync(hp + L.o_part + sizeof(WeightPartial), parts + L.nblk, sizeof(WeightPartial), cudaMemcpyDeviceToHost, st));
-    }
-    if (records)
-      CK(cudaMemcpyAsync(hp + L.o_rec, c.d_out.p, Pd * sizeof(mcl3dl_result), cudaMemcpyDeviceToHost, st));
-  }
-  double ent = 0.0;
-  float best = -1.0f;
-  uint32_t best_i = 0;
-  for (size_t d = 0; d < G; ++d)
-  {
-    DeviceCtx& c = eng->devs[d];
-    const size_t Pd = p0[d + 1] - p0[d];
-    if (Pd == 0)
-      continue;
-    CK(cudaSetDevice(c.dev));
-    if (!one_sync)
-      CK(cudaStreamSynchronize(c.stream));
-    const char* hp = static_cast<const char*>(c.h_pinned);
-    if (summary->kept)
-    {
-      std::memcpy(posterior + p0[d], hp + lay[d].o_post, Pd * 4);
-      WeightPartial wp;
-      std::memcpy(&wp, hp + lay[d].o_part + sizeof(WeightPartial), sizeof(wp));
-      ent += wp.sum;
-      if (wp.best > best)  // lower device = lower indices, so strict '>' keeps the first maximum
-      {
-        best = wp.best;
-        best_i = wp.best_i;
-      }
+        CK(cudaMemcpyAsync(hp + s.o_rec, d_rec, s.n * sizeof(mcl3dl_result), cudaMemcpyDeviceToHost, st));
     }
     else
     {
-      std::memcpy(posterior + p0[d], prior + p0[d], Pd * 4);  // "No Particle alive, restoring." pf.h:274-278
+      const WeightPartial* f1;
+      if ((rc = weight_pass1(eng, c, d_rec, d_prior, d_extra, s.n, n_lik, nullptr, &f1)))
+        return rc;
+      CK(cudaMemcpyAsync(h_part, f1, sizeof(WeightPartial), cudaMemcpyDeviceToHost, st));
+    }
+  }
+  WeightPartial w1 = weight_identity(), w2 = weight_identity();  // each pass folded over the devices, in device order
+  for (size_t d = 0; d < G; ++d)
+  {
+    DeviceCtx& c = eng->devs[d];
+    if (sh[d].n == 0)
+      continue;
+    CK(cudaSetDevice(c.dev));
+    CK(cudaStreamSynchronize(c.stream));
+    const WeightPartial& wp = *reinterpret_cast<const WeightPartial*>(static_cast<const char*>(c.h_pinned) + sh[d].o_part);
+    w1.sum += wp.sum;
+    w1.qmin = std::min(w1.qmin, wp.qmin);
+    w1.qmax = std::max(w1.qmax, wp.qmax);
+  }
+  const float total_f = static_cast<float>(w1.sum);
+  const bool kept = total_f > 0.0f;
+  // ---- pass 2 (several devices): normalise with the global total, entropy, arg max; only 4 B per particle come back
+  for (size_t d = 0; d < G && G > 1; ++d)
+  {
+    DeviceCtx& c = eng->devs[d];
+    const Share& s = sh[d];
+    if (s.n == 0)
+      continue;
+    CK(cudaSetDevice(c.dev));
+    cudaStream_t st = c.stream;
+    char* hp = static_cast<char*>(c.h_pinned);
+    if (kept)
+    {
+      const WeightPartial* f2;
+      if ((rc = weight_pass2(eng, c, nullptr, total_f, s.n, s.p0, static_cast<float*>(c.d_post.p), nullptr, &f2)))
+        return rc;
+      CK(cudaMemcpyAsync(hp + s.o_post, c.d_post.p, s.n * 4, cudaMemcpyDeviceToHost, st));
+      CK(cudaMemcpyAsync(hp + s.o_part + sizeof(WeightPartial), f2, sizeof(WeightPartial), cudaMemcpyDeviceToHost, st));
     }
     if (records)
-      std::memcpy(records + p0[d], hp + lay[d].o_rec, Pd * sizeof(mcl3dl_result));
+      CK(cudaMemcpyAsync(hp + s.o_rec, c.d_out.p, s.n * sizeof(mcl3dl_result), cudaMemcpyDeviceToHost, st));
   }
-  summary->entropy = summary->kept ? static_cast<float>(-ent) : 0.0f;
-  summary->max_index = best_i;
+  for (size_t d = 0; d < G; ++d)
+  {
+    DeviceCtx& c = eng->devs[d];
+    const Share& s = sh[d];
+    if (s.n == 0)
+      continue;
+    CK(cudaSetDevice(c.dev));
+    if (G > 1)
+      CK(cudaStreamSynchronize(c.stream));
+    const char* hp = static_cast<const char*>(c.h_pinned);
+    if (kept)
+    {
+      std::memcpy(posterior + s.p0, hp + s.o_post, s.n * 4);
+      const WeightPartial& wp = reinterpret_cast<const WeightPartial*>(hp + s.o_part)[1];
+      w2.sum += wp.sum;
+      if (wp.best > w2.best)  // lower device = lower indices, so strict '>' keeps the first maximum
+      {
+        w2.best = wp.best;
+        w2.best_i = wp.best_i;
+      }
+    }
+    else
+      std::memcpy(posterior + s.p0, prior + s.p0, s.n * 4);  // "No Particle alive, restoring." pf.h:274-278
+    if (records)
+      std::memcpy(records + s.p0, hp + s.o_rec, s.n * sizeof(mcl3dl_result));
+  }
+  make_summary(w1, w2, summary);
   return MCL3DL_OK;
 }
 

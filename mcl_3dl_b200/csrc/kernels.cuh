@@ -10,7 +10,7 @@
 //                     + RaycastUsingDDA / RaycastUsingKDTree:
 //       beam_kernel_pl    a lane owns a particle, a warp casts one chunk of rays; fixed CTA mapping
 //       beam_kernel_dq    the same lanes, (particle group, ray chunk) items pulled from a global queue
-//   weight_kernel / normalize_kernel*: the fused weight update; exchange_signal_kernel: the multi-GPU record exchange.
+//   weight_kernel / normalize_kernel: the fused weight update; exchange_signal_kernel: the multi-GPU record exchange.
 //
 // The per-thread arithmetic (transform, searches, ray casts, likelihood term, beam score) lives in device_funcs.cuh,
 // which tests/hostsim also compiles for the host.  Every reduction has a fixed order or sums integers, so results are
@@ -1198,6 +1198,18 @@ struct WeightPartial
   uint32_t best_i;  // its particle index (lowest index on ties)
 };
 
+// the identity of every fold of WeightPartials (device and host)
+__host__ __device__ __forceinline__ WeightPartial weight_identity()
+{
+  WeightPartial v;
+  v.sum = 0.0;
+  v.qmin = 1.0f;
+  v.qmax = 0.0f;
+  v.best = -1.0f;
+  v.best_i = 0xffffffffu;
+  return v;
+}
+
 // Per-CTA reduction into slots[blockIdx.x]; the LAST CTA to finish (ticket) then folds the slots in order into
 // slots[gridDim.x] (and into *host_copy, mapped pinned memory, when given): deterministic, and no separate finishing launch.
 __device__ __forceinline__ void weight_block_reduce(WeightPartial v, WeightPartial* slots, WeightPartial* sm, unsigned int* ticket,
@@ -1275,12 +1287,7 @@ __global__ void __launch_bounds__(kBlockThreads)
                   WeightPartial* __restrict__ host_copy)
 {
   __shared__ WeightPartial sm[kBlockThreads / 32];
-  WeightPartial v;
-  v.sum = 0.0;
-  v.qmin = 1.0f;
-  v.qmax = 0.0f;
-  v.best = -1.0f;
-  v.best_i = 0xffffffffu;
+  WeightPartial v = weight_identity();
   for (int i = blockIdx.x * kBlockThreads + threadIdx.x; i < P; i += gridDim.x * kBlockThreads)
   {
     const mcl3dl_result r = rec[i];
@@ -1299,49 +1306,18 @@ __global__ void __launch_bounds__(kBlockThreads)
   weight_block_reduce(v, partials, sm, ticket, host_copy);
 }
 
-// pass 2: p_i = w_i / sum (pf.h:266), entropy terms p ln p (pf.h:267-270), arg max
+// pass 2: p_i = w_i / total (pf.h:266), entropy terms p ln p (pf.h:267-270), arg max.  The total is pass 1's folded
+// slot when `pass1` is given (one device: no host round trip), else `total` (the sum over devices).  A non-positive
+// total ("No Particle alive", pf.h:274-278) leaves `post` unwritten; the caller restores the prior.
 __global__ void __launch_bounds__(kBlockThreads)
-    normalize_kernel(const float* __restrict__ w, int P, float total, int index_offset, float* __restrict__ post,
-                     WeightPartial* __restrict__ partials, unsigned int* __restrict__ ticket, WeightPartial* __restrict__ host_copy)
+    normalize_kernel(const float* __restrict__ w, int P, const WeightPartial* __restrict__ pass1, float total, int index_offset,
+                     float* __restrict__ post, WeightPartial* __restrict__ partials, unsigned int* __restrict__ ticket,
+                     WeightPartial* __restrict__ host_copy)
 {
   __shared__ WeightPartial sm[kBlockThreads / 32];
-  WeightPartial v;
-  v.sum = 0.0;
-  v.qmin = 1.0f;
-  v.qmax = 0.0f;
-  v.best = -1.0f;
-  v.best_i = 0xffffffffu;
-  for (int i = blockIdx.x * kBlockThreads + threadIdx.x; i < P; i += gridDim.x * kBlockThreads)
-  {
-    const float p = fdiv(w[i], total);
-    post[i] = p;
-    if (p > 0.0f)
-      v.sum = dadd(v.sum, static_cast<double>(fmul(p, logf(p))));
-    const uint32_t gi = static_cast<uint32_t>(index_offset + i);
-    if (p > v.best || (p == v.best && gi < v.best_i))
-    {
-      v.best = p;
-      v.best_i = gi;
-    }
-  }
-  weight_block_reduce(v, partials, sm, ticket, host_copy);
-}
-
-// pass 2 without a host round trip (one device): the total comes from pass 1's folded slot instead of a kernel
-// argument.  A non-positive total ("No Particle alive", pf.h:274-278) leaves `post` unwritten; the host restores the prior.
-__global__ void __launch_bounds__(kBlockThreads)
-    normalize_kernel_dev(const float* __restrict__ w, int P, const WeightPartial* __restrict__ pass1, int index_offset,
-                         float* __restrict__ post, WeightPartial* __restrict__ partials, unsigned int* __restrict__ ticket,
-                         WeightPartial* __restrict__ host_copy)
-{
-  __shared__ WeightPartial sm[kBlockThreads / 32];
-  const float total = __double2float_rn(pass1->sum);
-  WeightPartial v;
-  v.sum = 0.0;
-  v.qmin = 1.0f;
-  v.qmax = 0.0f;
-  v.best = -1.0f;
-  v.best_i = 0xffffffffu;
+  if (pass1)
+    total = __double2float_rn(pass1->sum);
+  WeightPartial v = weight_identity();
   if (total > 0.0f)
   {
     for (int i = blockIdx.x * kBlockThreads + threadIdx.x; i < P; i += gridDim.x * kBlockThreads)
