@@ -265,7 +265,10 @@ int mcl3dl_particles_measure_update(mcl3dl_engine*, const mcl3dl_point* lik_pts,
  * systematic pick from initial_p = initial_frac * pstep (the host draws initial_frac in [0, 1) with the node's engine),
  * noise on duplicates only, probability 1 / n.  Documented departures: the noise comes from a counter-based generator
  * (Philox-4x32-10 keyed by seed, output index and call count) instead of std::default_random_engine's stream, and
- * particles that tie in the accumulated probability are taken by lowest index instead of std::sort's order. */
+ * particles that tie in the accumulated probability are taken by lowest index instead of std::sort's order.  The call
+ * count starts at 1 on a new engine and is not reset by mcl3dl_particles_set.  Given the noise draws, the picks, the
+ * copies and the probabilities are exact; a duplicate differs from host arithmetic only through the device's logf /
+ * sinf / cosf (a few ulp of the noise). */
 int mcl3dl_particles_resample(mcl3dl_engine*, const float sigma_pos[3], const float sigma_rpy[3], float initial_frac,
                               uint64_t seed);
 
@@ -276,7 +279,10 @@ int mcl3dl_particles_resample(mcl3dl_engine*, const float sigma_pos[3], const fl
  *   state_prev == NULL: bias 1 for every particle (the node's branch for more particles than num_particles, :428-434);
  *   otherwise bias = NormalLikelihood(bias_var_dist)(|pos - prev.pos|) * NormalLikelihood(bias_var_ang)(angle) + 1e-6.
  * Sums are accumulated in double with a fixed tree (the reference: sequential float), so the values agree with the
- * reference to ~1e-5 relative.  Documented departures: the covariance always uses every particle (the reference
+ * reference to ~1e-5 relative.  Against the exact sums of the same float terms: with state_prev == NULL the weight
+ * sum, the mean position and the position block of cov equal float(exact ratio) (away from rounding boundaries), the
+ * mean rotation is within 1 ulp; the angle rows and the biased means carry the errors of the device's atan2f / asinf /
+ * acosf / expf (tests/test_gpu_pf_exact.py derives the bars).  Documented departures: the covariance always uses every particle (the reference
  * subsamples randomly above num_particles "to reduce calculation cost", and its expectation(1.0) / covariance(1.0) stop
  * early if the float running total of the probabilities passes 1.0 before the last particle). */
 typedef struct

@@ -2001,7 +2001,8 @@ int mcl3dl_measure_device(mcl3dl_engine* eng, const mcl3dl_pose* d_poses, size_t
   return launch_models(eng, c, d_poses, P, d_lik, n_lik, d_beam, n_beam, d_origins_xyz, n_origins, d_out, nullptr, st, false);
 }
 
-// ---- resident particle set (scope row f3; prepared, not yet run on hardware — see include/mcl3dl_b200.h)
+// ---- resident particle set (scope row f3; see include/mcl3dl_b200.h; tests/test_gpu_pf_exact.py holds it to its host
+// restatement)
 int mcl3dl_particles_set(mcl3dl_engine* eng, const mcl3dl_state* states, const float* prob, size_t n)
 {
   if (!eng || eng->devs.size() != 1 || !states || !prob || n == 0 || n >= (size_t(1) << 31))

@@ -131,7 +131,8 @@ __global__ void pf_resample_kernel(const PfState* __restrict__ in, const float* 
 // ---- pose estimate on the resident set (mcl3dl_particles_estimate): pf_->bias + expectationBiased + max + covariance
 // (src/mcl_3dl.cpp:428-452,704-724; pf.h:246-251,281-374).  Two passes of double sums with a fixed tree (lanes by
 // shuffles, warps and CTAs in order), so the result is deterministic; the reference sums sequentially in float, hence
-// agreement to ~1e-5 relative, not bitwise.
+// agreement to ~1e-5 relative, not bitwise.  Against the exact sums of the same float terms the bias-1 means, weight
+// sum and position covariance are float(exact ratio) away from rounding boundaries (tests/test_gpu_pf_exact.py).
 constexpr int kEstSums = 20;  // biased: w, w*pos(3), w*front(3), w*up(3); unbiased: the same ten with p
 constexpr int kCovSums = 22;  // p, 21 upper-triangle products p * d_j * d_k
 struct EstHeader

@@ -375,7 +375,7 @@ class Engine:
         self._check(self.L.mcl3dl_read_stats(self.h, C.byref(ws)))
         return ws.as_dict()
 
-    # ---- resident particle set (scope row f3; prepared, see include/mcl3dl_b200.h)
+    # ---- resident particle set (scope row f3; see include/mcl3dl_b200.h)
     def particles_set(self, states, prob):
         states = np.ascontiguousarray(states, dtype=STATE)
         prob = np.ascontiguousarray(prob, dtype=np.float32)

@@ -12,6 +12,7 @@ from mcl_3dl_b200 import synth
 
 HS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "hostsim")
 LikParams = real.LikParams
+SEQUENTIAL_SUMS = True  # the weight and estimate sums below add in particle order (the device folds a tree)
 beam_params_from_reference = real.beam_params_from_reference
 
 
@@ -64,11 +65,15 @@ class Engine:
         if total > 0:
             post = (w / total).astype(np.float32)
             nz = post > 0
-            summ["entropy"] = float(np.float32(-(post[nz] * np.log(post[nz]).astype(np.float32)).astype(np.float64).sum()))
+            lnp = np.log(post[nz].astype(np.float64)).astype(np.float32)      # logf correctly rounded
+            summ["entropy"] = float(np.float32(-(post[nz] * lnp).astype(np.float32).astype(np.float64).sum()))
             summ["max_index"] = int(np.argmax(post))
         else:
             post = prior.copy()
         return post, summ
+
+    def measure(self, poses, lik_pts=None, beam_pts=None, origins=None):
+        return self._records(poses, lik_pts, beam_pts, origins if origins is not None else np.zeros((0, 3)))[0]
 
     def measure_update(self, poses, lik_pts, beam_pts, origins, prior, extra_likelihood=None, want_records=False):
         rec, n_lik = self._records(poses, lik_pts, beam_pts, origins)
@@ -98,7 +103,8 @@ class Engine:
             a, sq2 = np.float32(1.0 / np.sqrt(2.0 * np.pi * s * s)), np.float32(s * s * 2.0)
             lin = self.states["odom_err_integ_lin"]
             x = np.sqrt((lin[:, 0] * lin[:, 0] + lin[:, 1] * lin[:, 1]).astype(np.float32) + lin[:, 2] * lin[:, 2]).astype(np.float32)
-            extra = (a * np.exp((-x * x / sq2).astype(np.float32)).astype(np.float32)).astype(np.float32)
+            e = np.exp((-x * x / sq2).astype(np.float32).astype(np.float64)).astype(np.float32)   # expf correctly rounded
+            extra = (a * e).astype(np.float32)
         rec, n_lik = self._records(poses, lik_pts, beam_pts, origins)
         self.prob, summ = self._update(rec, n_lik, self.prob, extra)
         return summ

@@ -116,11 +116,10 @@ extern "C" void hostsim_noise6(uint64_t seed, uint32_t index, uint32_t call, con
   pf_noise6(seed, index, call, sigma, org);
 }
 
-// The pose estimate (pf_kernels.cuh: pf_est_pass1/finish1/pass2/finish2) with the device's per-particle functions and
-// double sums in particle order (the kernels fold the same double terms with a fixed tree: equal to ~1e-16 relative).
-// out: mean_b pos[3] rot[4] | max_index | weight_sum_biased | cov[36]  (45 floats; max_index stored as float bits)
-extern "C" int hostsim_pf_estimate(const float* probs, const PfState* states, size_t n, const mcl3dl_pose* prev, float bias_var_dist,
-                                   float bias_var_ang, float* mean_pos, float* mean_rot, uint32_t* max_index, float* wsum, float* cov)
+namespace
+{
+// mcl3dl_particles_estimate's BiasDev for `prev` (nullptr: the constant bias 1)
+BiasDev bias_of(const mcl3dl_pose* prev, float bias_var_dist, float bias_var_ang)
 {
   BiasDev b{};
   if (prev)
@@ -138,6 +137,75 @@ extern "C" int hostsim_pf_estimate(const float* probs, const PfState* states, si
     b.ang_a = static_cast<float>(1.0 / std::sqrt(2.0 * M_PI * sa * sa));
     b.ang_sq2 = static_cast<float>(sa * sa * 2.0);
   }
+  return b;
+}
+}  // namespace
+
+// The float terms pf_est_pass1_kernel adds in double, per particle, in its column order: terms[20 i + k] = w, w * pos(3),
+// w * front(3), w * up(3), p, p * pos(3), p * front(3), p * up(3), with w = fmul(p, pf_bias).  bias[i] = pf_bias.
+extern "C" int hostsim_pf_est_terms(const float* probs, const PfState* states, size_t n, const mcl3dl_pose* prev, float bias_var_dist,
+                                    float bias_var_ang, float* bias, float* terms)
+{
+  const BiasDev b = bias_of(prev, bias_var_dist, bias_var_ang);
+  for (size_t i = 0; i < n; ++i)
+  {
+    const float p = probs[i];
+    bias[i] = pf_bias(states[i], b);
+    const float w = __fmul_rn(p, bias[i]);
+    float t[9];
+    pf_mean_terms(states[i], t);
+    float* o = terms + 20 * i;
+    o[0] = w;
+    o[10] = p;
+    for (int k = 0; k < 9; ++k)
+    {
+      o[1 + k] = __fmul_rn(t[k], w);
+      o[11 + k] = __fmul_rn(t[k], p);
+    }
+  }
+  return 0;
+}
+
+// pf_est_finish1_kernel's derivations from the twenty column sums v: the biased mean (pos, rot) and the centre of the
+// covariance (e_pos, e_rpy)
+extern "C" void hostsim_pf_est_finish(const double* v, float* mean_pos, float* mean_rot, float* e_pos, float* e_rpy)
+{
+  for (int a = 0; a < 3; ++a)
+  {
+    mean_pos[a] = static_cast<float>(v[1 + a] / v[0]);
+    e_pos[a] = static_cast<float>(v[11 + a] / v[10]);
+  }
+  pf_quat_from_front_up(v + 4, v + 7, mean_rot);
+  float qu[4];
+  pf_quat_from_front_up(v + 14, v + 17, qu);
+  pf_rpy(qu, e_rpy);
+}
+
+// The float terms pf_est_pass2_kernel adds in double for the centre (e_pos, e_rpy): terms[22 i] = p, then the 21
+// upper-triangle products fmul(fmul(fmul(1, d_j), d_k), p); d[6 i + j] = pf_cov_diff
+extern "C" int hostsim_pf_cov_terms(const float* probs, const PfState* states, size_t n, const float* e_pos, const float* e_rpy,
+                                    float* d, float* terms)
+{
+  for (size_t i = 0; i < n; ++i)
+  {
+    float* di = d + 6 * i;
+    pf_cov_diff(states[i], e_pos, e_rpy, di);
+    float* o = terms + 22 * i;
+    o[0] = probs[i];
+    int t = 1;
+    for (int j = 0; j < 6; ++j)
+      for (int k = j; k < 6; ++k) o[t++] = __fmul_rn(__fmul_rn(__fmul_rn(1.0f, di[j]), di[k]), probs[i]);
+  }
+  return 0;
+}
+
+// The pose estimate (pf_kernels.cuh: pf_est_pass1/finish1/pass2/finish2) with the device's per-particle functions and
+// double sums in particle order (the kernels fold the same double terms with a fixed tree: equal to ~1e-16 relative).
+// out: mean_b pos[3] rot[4] | max_index | weight_sum_biased | cov[36]  (45 floats; max_index stored as float bits)
+extern "C" int hostsim_pf_estimate(const float* probs, const PfState* states, size_t n, const mcl3dl_pose* prev, float bias_var_dist,
+                                   float bias_var_ang, float* mean_pos, float* mean_rot, uint32_t* max_index, float* wsum, float* cov)
+{
+  const BiasDev b = bias_of(prev, bias_var_dist, bias_var_ang);
   double v[20] = {0};
   float best = -1.0f;
   uint32_t best_i = 0;
