@@ -325,6 +325,34 @@ int mcl3dl_scan_get(mcl3dl_engine*, int which, mcl3dl_point* out, size_t capacit
 int mcl3dl_particles_measure_update_prepared(mcl3dl_engine*, const float* origins_xyz, size_t n_origins,
                                              float odom_err_integ_lin_sigma, mcl3dl_update_summary* summary);
 
+/* ---- Matched / unmatched output (src/mcl_3dl.cpp:761-805): the scan transformed by the pose estimate e
+ * (State6DOF::transform, normalised rotation) and split by kdtree_->radiusSearch(p, unmatch_output_dist, id, sqdist, 1)
+ * on the map index ChunkedKdtree(chunk_length, max_search_radius):
+ *   unmatched: no map point within unmatch_output_dist (the search radius);
+ *   matched:   the nearest one has sqdist < match_output_dist^2 (squared in double, :777);
+ *   neither:   every other point.
+ * Both clouds keep input order and carry the transformed xyz; the label passes through.  Distances are those of the
+ * likelihood search (dist_weight rescale, float L2), and which map points a query sees follows the chunk rule of
+ * ChunkedKdtree exactly: its own chunk's sub-cloud, halo copies included (chunked_kdtree.h:124-263), which matters
+ * because the radius is larger than max_search_radius.  Departures: a non-finite transformed point is unmatched (the
+ * reference gets there through floor(NaN) -> INT_MIN on x86, a chunk that does not exist); FLANN's eps is not emulated
+ * (the search is exact, as every search of this engine).
+ * pts == NULL: the downsampled cloud of the last mcl3dl_scan_prepare (single-device engines; n is ignored).
+ * matched / unmatched: host arrays with room for every input point, either may be NULL (count only).  Synchronous; on
+ * multi-device engines host clouds run on device 0.  Errors: INVALID_ARG for a null engine, pose, params or count
+ * pointer, a map staged without likelihood params, chunk_length <= 0, float(unmatch_output_dist) > chunk_length (the
+ * reference throws, chunked_kdtree.h:224-225) or pts == NULL without a prepared scan; NO_MAP before set_map. */
+typedef struct
+{
+  double match_output_dist;   /* Parameters::match_output_dist_   (node default 0.1) */
+  double unmatch_output_dist; /* Parameters::unmatch_output_dist_ (node default 0.5): the search radius */
+  float chunk_length;         /* ChunkedKdtree(map_chunk_, max_search_radius), src/mcl_3dl.cpp:1327 */
+  float max_search_radius;
+} mcl3dl_match_params;
+int mcl3dl_match_output(mcl3dl_engine*, const mcl3dl_pose* pose, const mcl3dl_point* pts, size_t n,
+                        const mcl3dl_match_params*, mcl3dl_point* matched, size_t* n_matched,
+                        mcl3dl_point* unmatched, size_t* n_unmatched);
+
 /* Record exchange over peer memory for the one-process-per-GPU layout (SURVEY §8e: particles sharded, ONE gather of the
  * 24-byte records, then the unchanged weight update of include/mcl_3dl/pf.h:252-279 on the full array).  There is no
  * collective call and no copy: the two measurement kernels store each particle's record straight into slot `rank` of

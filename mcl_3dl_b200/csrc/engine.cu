@@ -19,6 +19,7 @@
 #include <cub/iterator/transform_input_iterator.cuh>
 
 #include "kernels.cuh"
+#include "match_funcs.cuh"
 #include "pf_kernels.cuh"
 #include "scan_kernels.cuh"
 
@@ -346,7 +347,7 @@ struct DeviceCtx
   NnGridDev nn{};
   DdaGridDev dda{};
   KdRayDev kd{};
-  DevBuf raw_pts;  // map points in original order (KD-tree raycaster only)
+  DevBuf raw_pts;  // map points in original order (with a likelihood grid: KD-tree raycaster, matched / unmatched output)
   DevBuf near_lik, near_kd;  // near-field bits (MCL3DL_NEAR_BITS builds)
   DevBuf nnf_dir, nnf_cand, nnf_wide;  // NN field: directory, candidate lists, side table of the wide cells
   DevBuf fld_cells;          // field mode: 8 corner distances per lattice cell
@@ -378,6 +379,12 @@ struct DeviceCtx
   DevBuf s_raw, s_keys[2], s_vals[2], s_key_label[2], s_flags[2], s_pos[2], s_ds, s_clip[2], s_out[2], s_tmp, s_counts;
   mcl3dl_scan_info s_info{};
   bool s_valid = false;
+  // matched / unmatched output (mcl3dl_match_output), kept apart from the prepared scans it may read: host cloud,
+  // transformed cloud, flags + scan positions per output, cub scratch; the page-locked block the compaction writes
+  // both clouds and their counts into
+  DevBuf m_in, m_tf, m_flags[2], m_pos[2], m_tmp;
+  void* m_host = nullptr;
+  size_t m_host_cap = 0;
   DevBuf r_states[2], r_prob, r_accum, r_poses, r_extra, r_est;  // r_est: EstHeader + per-CTA partial sums
   size_t r_n = 0;
   int r_cur = 0;
@@ -1284,6 +1291,15 @@ int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_point* h_
     eng->info.nn_origin[1] = g.oy;
     eng->info.nn_origin[2] = g.oz;
   }
+  // ---- the raw points by original index (the KD-tree raycaster's colliding point; the chunk rule of
+  // mcl3dl_match_output): keep the upload wherever there is a likelihood grid
+  free_buf(c.raw_pts);
+  if (eng->has_lik)
+  {
+    c.raw_pts = d_pts;
+    d_pts = DevBuf();
+    c.map_bytes += n * 16;
+  }
 
   // ---- KD-tree raycaster: marches over the likelihood grid; needs the raw points by original index
   if (eng->has_beam && !eng->beam.use_raycast_using_dda)
@@ -1299,11 +1315,7 @@ int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_point* h_
     CKB(build_near_field(eng, c, st, pts, n32, wx, wy, wz, c.kd.r1_pad, eng->near_kd_k, sc_min, sc_max, c.near_kd, c.kd.near, 1));
     c.near_kd_r = c.kd.r1_pad;
 #endif
-    free_buf(c.raw_pts);
-    c.raw_pts = d_pts;  // keep the upload
-    d_pts = DevBuf();
     c.kd.raw_pts = static_cast<const float4*>(c.raw_pts.p);
-    c.map_bytes += n * 16;
   }
   // ---- DDA grid: updatePointCloud, raycast_using_dda.h:162-190
   if (eng->has_beam && eng->beam.use_raycast_using_dda)
@@ -1561,8 +1573,11 @@ void mcl3dl_destroy(mcl3dl_engine* eng)
     free_buf(c.x_ticket);
     for (DevBuf* b : {&c.r_states[0], &c.r_states[1], &c.r_prob, &c.r_accum, &c.r_poses, &c.r_extra, &c.r_est, &c.s_raw, &c.s_keys[0],
                       &c.s_keys[1], &c.s_vals[0], &c.s_vals[1], &c.s_key_label[0], &c.s_key_label[1], &c.s_flags[0],
-                      &c.s_flags[1], &c.s_pos[0], &c.s_pos[1], &c.s_ds, &c.s_clip[0], &c.s_clip[1], &c.s_out[0], &c.s_out[1], &c.s_tmp, &c.s_counts})
+                      &c.s_flags[1], &c.s_pos[0], &c.s_pos[1], &c.s_ds, &c.s_clip[0], &c.s_clip[1], &c.s_out[0], &c.s_out[1], &c.s_tmp, &c.s_counts,
+                      &c.m_in, &c.m_tf, &c.m_flags[0], &c.m_flags[1], &c.m_pos[0], &c.m_pos[1], &c.m_tmp})
       free_buf(*b);
+    if (c.m_host)
+      cudaFreeHost(c.m_host);
     for (DevBuf* b : {&c.nn_cell_start, &c.nn_pts, &c.nn_row3, &c.dda_occ, &c.dda_cell_start, &c.dda_pts, &c.raw_pts, &c.near_lik, &c.near_kd, &c.nnf_dir, &c.nnf_cand, &c.nnf_wide, &c.fld_cells, &c.d_poses,
                       &c.d_out, &c.d_status, &c.d_stats, &c.d_partial, &c.d_tickets, &c.d_tally, &c.d_queue, &c.d_lacc, &c.d_w, &c.d_post, &c.d_wpart, &c.d_wticket})
       free_buf(*b);
@@ -2326,6 +2341,98 @@ int mcl3dl_scan_get(mcl3dl_engine* eng, int which, mcl3dl_point* out, size_t cap
   CK(cudaSetDevice(c.dev));
   CK(cudaMemcpyAsync(out, src[which]->p, static_cast<size_t>(n[which]) * 16, cudaMemcpyDeviceToHost, c.stream));
   CK(cudaStreamSynchronize(c.stream));
+  return MCL3DL_OK;
+}
+
+int mcl3dl_match_output(mcl3dl_engine* eng, const mcl3dl_pose* pose, const mcl3dl_point* pts, size_t n, const mcl3dl_match_params* mp,
+                        mcl3dl_point* matched, size_t* n_matched, mcl3dl_point* unmatched, size_t* n_unmatched)
+{
+  if (!eng || !pose || !mp || !n_matched || !n_unmatched)
+    return MCL3DL_ERR_INVALID_ARG;
+  if (!eng->has_map)
+    return MCL3DL_ERR_NO_MAP;
+  // radiusSearch takes the radius as a float and throws above the chunk length (chunked_kdtree.h:218-225)
+  const float r = static_cast<float>(mp->unmatch_output_dist);
+  if (!eng->has_lik || !(mp->chunk_length > 0.0f) || r > mp->chunk_length)
+    return MCL3DL_ERR_INVALID_ARG;
+  DeviceCtx& c = eng->devs[0];
+  const mcl3dl_point* src = pts;
+  size_t cnt = n;
+  if (!pts)
+  {
+    if (eng->devs.size() != 1 || !c.s_valid)
+      return MCL3DL_ERR_INVALID_ARG;
+    src = static_cast<const mcl3dl_point*>(c.s_ds.p);
+    cnt = c.s_info.n_downsampled;
+  }
+  if (cnt >= (size_t(1) << 30))
+    return MCL3DL_ERR_INVALID_ARG;
+  *n_matched = 0;
+  *n_unmatched = 0;
+  if (cnt == 0)
+    return MCL3DL_OK;
+  CK(cudaSetDevice(c.dev));
+  cudaStream_t st = c.stream;
+  const uint32_t n32 = static_cast<uint32_t>(cnt);
+  int rc;
+  if ((rc = reserve(eng, c.m_tf, cnt * 16)) || (pts && (rc = reserve(eng, c.m_in, cnt * 16))))
+    return rc;
+  for (int k = 0; k < 2; ++k)
+    if ((rc = reserve(eng, c.m_flags[k], cnt * 4)) || (rc = reserve(eng, c.m_pos[k], cnt * 4)))
+      return rc;
+  // page-locked result block: [2 counts | 56 B pad | matched cloud | unmatched cloud], written by the compaction itself so
+  // that one synchronise ends the call
+  const size_t host_bytes = 64 + 2 * cnt * 16;
+  if (host_bytes > c.m_host_cap)
+  {
+    if (c.m_host)
+      CK(cudaFreeHost(c.m_host));
+    c.m_host = nullptr;
+    c.m_host_cap = 0;
+    CK(cudaMallocHost(&c.m_host, host_bytes));
+    c.m_host_cap = host_bytes;
+  }
+  if (pts)
+  {
+    CK(cudaMemcpyAsync(c.m_in.p, pts, cnt * 16, cudaMemcpyHostToDevice, st));
+    src = static_cast<const mcl3dl_point*>(c.m_in.p);
+  }
+  MatchDev m{};
+  m.raw_pts = static_cast<const float4*>(c.raw_pts.p);
+  m.r2 = static_cast<float>(static_cast<double>(r) * static_cast<double>(r));
+  m.rpad = r * 1.0001f + 1e-6f;
+  m.match_sq = mp->match_output_dist * mp->match_output_dist;
+  m.chunk_length = mp->chunk_length;
+  m.pos_to_chunk = static_cast<float>(1.0 / static_cast<double>(mp->chunk_length));
+  m.max_search_radius = mp->max_search_radius;
+  uint32_t* f[2] = {static_cast<uint32_t*>(c.m_flags[0].p), static_cast<uint32_t*>(c.m_flags[1].p)};
+  uint32_t* ps[2] = {static_cast<uint32_t*>(c.m_pos[0].p), static_cast<uint32_t*>(c.m_pos[1].p)};
+  mcl3dl_point* tf = static_cast<mcl3dl_point*>(c.m_tf.p);
+  const int nb = static_cast<int>((cnt + 255) / 256);
+  match_classify_kernel<<<nb, 256, 0, st>>>(src, n32, *pose, c.nn, m, tf, f[0], f[1]);
+  CK(cudaGetLastError());
+  size_t t_scan = 0;
+  CK(cub::DeviceScan::ExclusiveSum(nullptr, t_scan, f[0], ps[0], n32, st));
+  if ((rc = reserve(eng, c.m_tmp, t_scan + 256)))
+    return rc;
+  char* hp = static_cast<char*>(c.m_host);
+  uint32_t* h_counts = reinterpret_cast<uint32_t*>(hp);
+  mcl3dl_point* h_out[2] = {reinterpret_cast<mcl3dl_point*>(hp + 64), reinterpret_cast<mcl3dl_point*>(hp + 64 + cnt * 16)};
+  for (int k = 0; k < 2; ++k)
+  {
+    size_t tsz = c.m_tmp.cap;
+    CK(cub::DeviceScan::ExclusiveSum(c.m_tmp.p, tsz, f[k], ps[k], n32, st));
+    scan_compact_kernel<<<nb, 256, 0, st>>>(tf, f[k], ps[k], n32, h_out[k], h_counts + k);
+  }
+  CK(cudaGetLastError());
+  eng->launches += 5;
+  CK(cudaStreamSynchronize(st));
+  *n_matched = h_counts[0];
+  *n_unmatched = h_counts[1];
+  if (matched)
+    std::memcpy(matched, h_out[0], *n_matched * 16);
+  if (unmatched)
+    std::memcpy(unmatched, h_out[1], *n_unmatched * 16);
   return MCL3DL_OK;
 }
 

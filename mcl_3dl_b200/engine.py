@@ -86,6 +86,12 @@ class ScanInfo(C.Structure):
         return {k: int(getattr(self, k)) for k, _ in self._fields_}
 
 
+class MatchParams(C.Structure):
+    """mcl3dl_match_params (Engine.match_output fills it; its defaults are the node's)."""
+    _fields_ = [("match_output_dist", C.c_double), ("unmatch_output_dist", C.c_double), ("chunk_length", C.c_float),
+                ("max_search_radius", C.c_float)]
+
+
 class Estimate(C.Structure):
     """mcl3dl_estimate"""
     _fields_ = [("mean_biased", C.c_float * 8), ("max_state", C.c_float * 8), ("max_index", C.c_uint32),
@@ -108,7 +114,7 @@ EXPORTED_SYMBOLS = ["mcl3dl_measure_update", "mcl3dl_collect_stats", "mcl3dl_rea
                     "mcl3dl_exchange_create", "mcl3dl_exchange_open", "mcl3dl_measure_exchange_device", "mcl3dl_exchange_current",
                     "mcl3dl_particles_set", "mcl3dl_particles_get", "mcl3dl_particles_predict",
                     "mcl3dl_particles_measure_update", "mcl3dl_particles_resample", "mcl3dl_particles_estimate", "mcl3dl_scan_prepare", "mcl3dl_scan_get",
-                    "mcl3dl_particles_measure_update_prepared"]
+                    "mcl3dl_particles_measure_update_prepared", "mcl3dl_match_output"]
 
 _LIBS = {}
 
@@ -160,6 +166,7 @@ def load_library(path=None):
     L.mcl3dl_scan_prepare.argtypes = [vp, vp, sz, vp, vp]
     L.mcl3dl_scan_get.argtypes = [vp, C.c_int, vp, sz, C.POINTER(sz)]
     L.mcl3dl_particles_measure_update_prepared.argtypes = [vp, vp, sz, C.c_float, vp]
+    L.mcl3dl_match_output.argtypes = [vp, vp, vp, sz, vp, vp, C.POINTER(sz), vp, C.POINTER(sz)]
     L.mcl3dl_exchange_create.argtypes = [vp, sz, C.c_int, C.c_int, vp]
     L.mcl3dl_exchange_open.argtypes = [vp, vp]
     L.mcl3dl_measure_exchange_device.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp, sz, vp, C.POINTER(vp)]
@@ -424,6 +431,24 @@ class Engine:
         if n.value:
             self._check(self.L.mcl3dl_scan_get(self.h, which, _ptr(out), len(out), C.byref(n)))
         return out
+
+    def match_output(self, pose, pts=None, match_dist=0.1, unmatch_dist=0.5, chunk_length=20.0, max_search_radius=0.2):
+        """The node's matched / unmatched clouds (include/mcl3dl_b200.h: mcl3dl_match_output) -> (matched, unmatched) as
+        POINT arrays of the transformed points.  pts=None: the downsampled cloud of the last scan_prepare."""
+        pose = np.ascontiguousarray(pose, dtype=POSE).reshape(1)
+        mp = MatchParams(match_dist, unmatch_dist, chunk_length, max_search_radius)
+        if pts is not None:
+            pts = np.ascontiguousarray(pts, dtype=POINT)
+            cap = len(pts)
+        else:  # the prepared cloud's size (no prepared scan: the call below reports the error)
+            n_ds = C.c_size_t(0)
+            cap = n_ds.value if self.L.mcl3dl_scan_get(self.h, 0, None, 0, C.byref(n_ds)) == 0 else 0
+        out = [np.zeros(cap, dtype=POINT), np.zeros(cap, dtype=POINT)]
+        n = [C.c_size_t(0), C.c_size_t(0)]
+        self._check(self.L.mcl3dl_match_output(self.h, _ptr(pose), _ptr(pts) if pts is not None else None,
+                                               len(pts) if pts is not None else 0, C.byref(mp), _ptr(out[0]),
+                                               C.byref(n[0]), _ptr(out[1]), C.byref(n[1])))
+        return out[0][:n[0].value].copy(), out[1][:n[1].value].copy()
 
     def particles_measure_update_prepared(self, origins, odom_err_integ_lin_sigma=0.0):
         origins = np.ascontiguousarray(origins if origins is not None else np.zeros((0, 3)), dtype=np.float32).reshape(-1, 3)

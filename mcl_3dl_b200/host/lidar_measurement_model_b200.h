@@ -232,6 +232,37 @@ public:
                                           origins.size(), odom_err_integ_lin_sigma, summary),
           "mcl3dl_particles_measure_update");
   }
+  // The node's matched / unmatched output (src/mcl_3dl.cpp:761-805) in one engine call: pc_local_full transformed by
+  // the pose estimate e, split by the map index's radius search (mcl3dl_match_output); pc_local_full == nullptr takes
+  // the downsampled cloud of the last mcl3dl_scan_prepare.  The clouds are filled as the node fills them.
+  void matchOutput(ChunkedKdtree<PointType>::Ptr& kdtree, const State6DOF& e, const Cloud::ConstPtr& pc_local_full,
+                   double match_dist, double unmatch_dist, float chunk_length, float max_search_radius,
+                   pcl::PointCloud<pcl::PointXYZ>& matched, pcl::PointCloud<pcl::PointXYZ>& unmatched)
+  {
+    stageMap(kdtree);
+    std::vector<mcl3dl_point> in;
+    size_t cap = 0;
+    if (pc_local_full)
+    {
+      pack(pc_local_full, in);
+      cap = in.size();
+    }
+    else
+    {
+      check(mcl3dl_scan_get(engine_, 0, nullptr, 0, &cap), "mcl3dl_scan_get");
+    }
+    std::vector<mcl3dl_point> m(cap), u(cap);
+    const mcl3dl_pose pose = toPose(e);
+    const mcl3dl_match_params mp{match_dist, unmatch_dist, chunk_length, max_search_radius};
+    size_t n_m = 0, n_u = 0;
+    check(mcl3dl_match_output(engine_, &pose, pc_local_full ? in.data() : nullptr, in.size(), &mp, m.data(), &n_m, u.data(),
+                              &n_u),
+          "mcl3dl_match_output");
+    matched.points.clear();
+    unmatched.points.clear();
+    for (size_t i = 0; i < n_m; ++i) matched.points.emplace_back(m[i].x, m[i].y, m[i].z);
+    for (size_t i = 0; i < n_u; ++i) unmatched.points.emplace_back(u[i].x, u[i].y, u[i].z);
+  }
   void checked(int rc, const char* what) const { check(rc, what); }
   size_t likPoints() const { return lik_cloud_ ? lik_cloud_->size() : 0; }
   mcl3dl_engine* engine() { return engine_; }
