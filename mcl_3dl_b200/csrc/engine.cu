@@ -11,6 +11,7 @@
 #include <limits>
 #include <string>
 #include <type_traits>
+#include <utility>
 #include <vector>
 
 #include <cub/device/device_radix_sort.cuh>
@@ -331,14 +332,87 @@ __global__ void dda_gather_kernel(const mcl3dl_point* __restrict__ pts, uint32_t
   out[k] = __ldg(reinterpret_cast<const float4*>(pts) + order[k]);  // xyz + label bits, map order kept by the stable sort
 }
 
-struct DevBuf
+// Memory the engine owns: device memory (cudaMalloc) or a page-locked host block (cudaMallocHost).  Move-only; the
+// destructor frees it.
+template <bool kPinned>
+struct Buf
 {
   void* p = nullptr;
   size_t cap = 0;
-};
+  Buf() = default;
+  Buf(Buf&& o) noexcept : p(std::exchange(o.p, nullptr)), cap(std::exchange(o.cap, 0)) {}
+  Buf& operator=(Buf&& o) noexcept
+  {
+    if (this != &o)
+    {
+      release();
+      p = std::exchange(o.p, nullptr);
+      cap = std::exchange(o.cap, 0);
+    }
+    return *this;
+  }
+  ~Buf() { release(); }
+  // At least `bytes` (device memory: at least 256 B).  Grows only, by a new allocation: the contents are not kept.
+  cudaError_t reserve(size_t bytes)
+  {
+    if (p && bytes <= cap)
+      return cudaSuccess;
+    if (const cudaError_t e = release())
+      return e;
+    const size_t want = kPinned ? bytes : std::max<size_t>(bytes, 256);
+    if (const cudaError_t e = kPinned ? cudaMallocHost(&p, want) : cudaMalloc(&p, want))
+      return e;
+    cap = want;
+    return cudaSuccess;
+  }
 
+ private:
+  cudaError_t release()
+  {
+    const cudaError_t e = !p ? cudaSuccess : kPinned ? cudaFreeHost(p) : cudaFree(p);
+    p = nullptr;
+    cap = 0;
+    return e;
+  }
+};
+using DevBuf = Buf<false>;
+using PinnedBuf = Buf<true>;
+
+// Everything the engine holds on one device.  Not copyable or movable (the engine keeps its contexts where they were
+// constructed); the destructor releases it all.
 struct DeviceCtx
 {
+  DeviceCtx() = default;
+  DeviceCtx(const DeviceCtx&) = delete;
+  DeviceCtx& operator=(const DeviceCtx&) = delete;
+  ~DeviceCtx()
+  {
+    cudaSetDevice(dev);
+    for (cudaStream_t s : {stream, side})
+      if (s)
+        cudaStreamSynchronize(s);
+    xchg_close();
+    for (cudaEvent_t e : ev)
+      if (e)
+        cudaEventDestroy(e);
+    for (cudaEvent_t e : {ev_fork, ev_join, ev_b0, ev_b1})
+      if (e)
+        cudaEventDestroy(e);
+    for (cudaStream_t s : {side, stream})
+      if (s)
+        cudaStreamDestroy(s);
+  }  // then the buffer members free themselves, on this device
+  void xchg_close()
+  {
+    for (void*& o : x_opened)
+      if (o)
+      {
+        cudaIpcCloseMemHandle(o);
+        o = nullptr;
+      }
+    x_ready = false;
+  }
+
   int dev = 0;
   cudaStream_t stream = nullptr;
   int sm_count = 132;
@@ -351,14 +425,14 @@ struct DeviceCtx
   DevBuf near_lik, near_kd;  // near-field bits (MCL3DL_NEAR_BITS builds)
   DevBuf nnf_dir, nnf_cand, nnf_wide;  // NN field: directory, candidate lists, side table of the wide cells
   DevBuf fld_cells;          // field mode: 8 corner distances per lattice cell
-  cudaPitchedPtr fld_nodes{};  // field mode: node volume (cudaMalloc3D)
+  DevBuf fld_mem;              // field mode: node volume (cudaMalloc3D), the owner of fld_nodes.ptr
+  cudaPitchedPtr fld_nodes{};
   bool fld_nodes_valid = false;
   float near_kd_r = 0.0f;            // radius the KD field was built for
   size_t map_bytes = 0;
   // per-update I/O
   DevBuf d_poses /* whole input block of the host path */, d_out, d_status;
-  void* h_pinned = nullptr;
-  size_t h_pinned_cap = 0;
+  PinnedBuf h_pinned;
   cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   // the two models are independent (disjoint fields of the record): the beam kernel runs on a side stream,
   // forked from / joined to the caller's stream with events
@@ -368,8 +442,6 @@ struct DeviceCtx
   DevBuf d_partial, d_tickets;  // lane-per-particle kernels: per-CTA partials + per-group ticket counters
   DevBuf d_tally, d_queue;      // dynamic-queue beam kernel: per-particle integer tallies, item counter (left at zero)
   DevBuf d_lacc;                // point-major likelihood kernel: per-particle accumulators (left at zero)
-  size_t tally_zeroed = 0;
-  size_t tickets_zeroed = 0;
   std::vector<const void*> smem_opted;  // kernels already opted in to large dynamic shared memory on this device
   // resident particle set (mcl3dl_particles_*): two state buffers (resampling writes the other one), probabilities,
   // prefix sum + pstep, the packed poses / odometry-error factors the measurement kernels read
@@ -383,8 +455,7 @@ struct DeviceCtx
   // transformed cloud, flags + scan positions per output, cub scratch; the page-locked block the compaction writes
   // both clouds and their counts into
   DevBuf m_in, m_tf, m_flags[2], m_pos[2], m_tmp;
-  void* m_host = nullptr;
-  size_t m_host_cap = 0;
+  PinnedBuf m_host;
   DevBuf r_states[2], r_prob, r_accum, r_poses, r_extra, r_est;  // r_est: EstHeader + per-CTA partial sums
   size_t r_n = 0;
   int r_cur = 0;
@@ -468,55 +539,34 @@ namespace
     }                                                                                                \
   } while (0)
 
-int reserve(mcl3dl_engine* eng, DevBuf& b, size_t bytes)
+template <bool kPinned>
+int reserve(mcl3dl_engine* eng, Buf<kPinned>& b, size_t bytes)
 {
-  if (bytes <= b.cap && b.p)
-    return MCL3DL_OK;
-  if (b.p)
-    CK(cudaFree(b.p));
-  b.p = nullptr;
-  b.cap = 0;
-  const size_t want = std::max<size_t>(bytes, 256);
-  CK(cudaMalloc(&b.p, want));
-  b.cap = want;
+  CK(b.reserve(bytes));
   return MCL3DL_OK;
 }
 
-int reserve_pinned(mcl3dl_engine* eng, DeviceCtx& c, size_t bytes)
+// Scratch that the kernels leave at zero (tickets, counters, accumulators): when the buffer grows, its whole new capacity
+// is zeroed on `st`, ahead of the kernels that read it there.
+int reserve_zeroed(mcl3dl_engine* eng, DevBuf& b, size_t bytes, cudaStream_t st)
 {
-  if (bytes <= c.h_pinned_cap)
+  if (b.p && bytes <= b.cap)
     return MCL3DL_OK;
-  if (c.h_pinned)
-    CK(cudaFreeHost(c.h_pinned));
-  c.h_pinned = nullptr;
-  c.h_pinned_cap = 0;
-  CK(cudaMallocHost(&c.h_pinned, bytes));
-  c.h_pinned_cap = bytes;
+  if (int rc = reserve(eng, b, bytes))
+    return rc;
+  CK(cudaMemsetAsync(b.p, 0, b.cap, st));
   return MCL3DL_OK;
-}
-
-void free_buf(DevBuf& b)
-{
-  if (b.p)
-    cudaFree(b.p);
-  b.p = nullptr;
-  b.cap = 0;
 }
 
 // The weight update's grid for n particles and its scratch on one device: w_i, one slot set [nblk per-CTA partials |
-// folded partial] per pass (0, 1) and a zeroed ticket per pass for its last-CTA fold (the kernels leave it at zero)
+// folded partial] per pass (0, 1) and a zeroed ticket per pass for its last-CTA fold
 int weight_scratch(mcl3dl_engine* eng, DeviceCtx& c, size_t n, int pass, int* nblk, WeightPartial** slots, unsigned int** ticket)
 {
   *nblk = static_cast<int>(std::min<size_t>((n + kBlockThreads - 1) / kBlockThreads, static_cast<size_t>(c.sm_count) * 4));
   int rc;
-  if ((rc = reserve(eng, c.d_w, n * 4)) || (rc = reserve(eng, c.d_wpart, 2 * (*nblk + 1) * sizeof(WeightPartial))))
+  if ((rc = reserve(eng, c.d_w, n * 4)) || (rc = reserve(eng, c.d_wpart, 2 * (*nblk + 1) * sizeof(WeightPartial))) ||
+      (rc = reserve_zeroed(eng, c.d_wticket, 256, c.stream)))
     return rc;
-  if (!c.d_wticket.p)
-  {
-    if ((rc = reserve(eng, c.d_wticket, 256)))
-      return rc;
-    CK(cudaMemset(c.d_wticket.p, 0, 256));
-  }
   *slots = static_cast<WeightPartial*>(c.d_wpart.p) + pass * (*nblk + 1);
   *ticket = static_cast<unsigned int*>(c.d_wticket.p) + pass;
   return MCL3DL_OK;
@@ -643,13 +693,8 @@ int launch_lik_nf_pm(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_pose* poses,
                      const NfPmShape& sh)
 {
   // one accumulator per particle; zeroed once, the kernel leaves it at zero
-  const size_t bytes = static_cast<size_t>(P) * 8;
-  if (bytes > c.d_lacc.cap || !c.d_lacc.p)
-  {
-    if (int rc = reserve(eng, c.d_lacc, bytes))
-      return rc;
-    CK(cudaMemsetAsync(c.d_lacc.p, 0, c.d_lacc.cap, st));
-  }
+  if (int rc = reserve_zeroed(eng, c.d_lacc, static_cast<size_t>(P) * 8, st))
+    return rc;
   auto* acc = static_cast<unsigned long long*>(c.d_lacc.p);
   const auto kernel = eng->nnf_overflow_cells != 0 ? lik_kernel_nf_pm<true> : lik_kernel_nf_pm<false>;
   CK(launch_pdl(kernel, blocks * sh.n_slices, 0, st, poses, P, scan, N, c.nn, eng->likdev, out, beam_defaults,
@@ -692,10 +737,12 @@ int stage_field(mcl3dl_engine* eng, DeviceCtx& c, const float* host_nodes)
   if (n_cells * 32 > eng->field_max_bytes)
     return MCL3DL_ERR_TOO_LARGE;
   cudaStream_t st = c.stream;
-  if (!c.fld_nodes.ptr)
+  if (!c.fld_mem.p)
   {
     const cudaExtent ext = make_cudaExtent(static_cast<size_t>(nnx) * sizeof(float), nny, nnz);
     CK(cudaMalloc3D(&c.fld_nodes, ext));
+    c.fld_mem.p = c.fld_nodes.ptr;
+    c.fld_mem.cap = c.fld_nodes.pitch * nny * nnz;
   }
   int rc = reserve(eng, c.fld_cells, n_cells * 32);
   if (rc != MCL3DL_OK)
@@ -802,14 +849,7 @@ int prepare_pl_scratch(mcl3dl_engine* eng, DeviceCtx& c, size_t P, const PlShape
   int rc = reserve(eng, c.d_partial, std::max<size_t>(P, 1) * sh.cb * 12);
   if (rc != MCL3DL_OK)
     return rc;
-  if (groups * 4 > c.d_tickets.cap || !c.d_tickets.p)
-  {
-    rc = reserve(eng, c.d_tickets, std::max<size_t>(groups * 4, 4096));
-    if (rc != MCL3DL_OK)
-      return rc;
-    CK(cudaMemsetAsync(c.d_tickets.p, 0, c.d_tickets.cap, st));  // the kernels leave them at zero afterwards
-  }
-  return MCL3DL_OK;
+  return reserve_zeroed(eng, c.d_tickets, std::max<size_t>(groups * 4, 4096), st);
 }
 
 int launch_beam_pl(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_pose* poses, size_t P, const mcl3dl_point* scan, size_t N,
@@ -843,25 +883,10 @@ int launch_beam_dq(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_pose* poses, s
   ppl = std::min<size_t>(std::max<size_t>(ppl, 1), 16);
   const int n_chunks = static_cast<int>(std::max<size_t>((N + ppl - 1) / ppl, 1));
   int rc;
-  const size_t tally_bytes = std::max<size_t>(P, 1) * 12, ticket_bytes = std::max<size_t>(groups * 4, 4096);
-  if (tally_bytes > c.d_tally.cap || !c.d_tally.p)
-  {
-    if ((rc = reserve(eng, c.d_tally, tally_bytes)))
-      return rc;
-    CK(cudaMemsetAsync(c.d_tally.p, 0, c.d_tally.cap, st));  // the kernel leaves them at zero afterwards
-  }
-  if (ticket_bytes > c.d_tickets.cap || !c.d_tickets.p)
-  {
-    if ((rc = reserve(eng, c.d_tickets, ticket_bytes)))
-      return rc;
-    CK(cudaMemsetAsync(c.d_tickets.p, 0, c.d_tickets.cap, st));
-  }
-  if (!c.d_queue.p)
-  {
-    if ((rc = reserve(eng, c.d_queue, 256)))
-      return rc;
-    CK(cudaMemsetAsync(c.d_queue.p, 0, 256, st));
-  }
+  if ((rc = reserve_zeroed(eng, c.d_tally, std::max<size_t>(P, 1) * 12, st)) ||
+      (rc = reserve_zeroed(eng, c.d_tickets, std::max<size_t>(groups * 4, 4096), st)) ||
+      (rc = reserve_zeroed(eng, c.d_queue, 256, st)))
+    return rc;
   const auto kernel = eng->beam.use_raycast_using_dda ? beam_kernel_dq<false> : beam_kernel_dq<true>;
   kernel<<<grid, kBlockThreads, 0, st>>>(poses, static_cast<int>(P), reinterpret_cast<const float4*>(scan), static_cast<int>(N),
                                          origins, c.dda, c.kd, c.nn, out, status, lik_defaults, c.stats_ptr(),
@@ -1000,90 +1025,63 @@ int build_nn_field(mcl3dl_engine* eng, DeviceCtx& c, cudaStream_t st, const mcl3
     return MCL3DL_OK;
   DevBuf d_bits, d_tot, d_tmp;
   int rc = MCL3DL_OK;
-  auto cleanup = [&]() {
-    free_buf(d_bits);
-    free_buf(d_tot);
-    free_buf(d_tmp);
-  };
-#define CKF(call)                                                                  \
-  do                                                                               \
-  {                                                                                \
-    cudaError_t e__ = (call);                                                      \
-    if (e__ != cudaSuccess)                                                        \
-    {                                                                              \
-      eng->err = std::string(#call) + ": " + cudaGetErrorString(e__);              \
-      cleanup();                                                                   \
-      return MCL3DL_ERR_CUDA;                                                      \
-    }                                                                              \
-  } while (0)
   const uint32_t wide_cap = static_cast<uint32_t>(std::min<size_t>(n_cells, size_t(1) << 18));
   const size_t sum_at = (n_cells + 5) & ~size_t(1);  // 64-bit grand total, 8-byte aligned behind the tail words
   if ((rc = reserve(eng, d_bits, bits_bytes)) || (rc = reserve(eng, d_tot, (sum_at + 2) * 4)) ||
       (rc = reserve(eng, c.nnf_dir, n_cells * sizeof(uint2))) || (rc = reserve(eng, c.nnf_wide, static_cast<size_t>(wide_cap) * sizeof(uint4))))
-  {
-    cleanup();
     return rc;
-  }
-  CKF(cudaMemsetAsync(d_bits.p, 0, bits_bytes, st));
+  CK(cudaMemsetAsync(d_bits.p, 0, bits_bytes, st));
   near_mark_kernel<<<(n + 255) / 256, 256, 0, st>>>(pts, n, g.wx, g.wy, g.wz, lay, static_cast<uint32_t*>(d_bits.p), 2);
   const unsigned blocks = static_cast<unsigned>((n_cells * 8 + 255) / 256);
   uint2* dir = static_cast<uint2*>(c.nnf_dir.p);
   uint32_t* tot = static_cast<uint32_t*>(d_tot.p);
-  CKF(cudaMemsetAsync(tot + n_cells, 0, 16, st));  // [n_cells]: scan tail, [n_cells + 2] wide cells, [n_cells + 3] overflow cells
+  CK(cudaMemsetAsync(tot + n_cells, 0, 16, st));  // [n_cells]: scan tail, [n_cells + 2] wide cells, [n_cells + 3] overflow cells
   f.wide = static_cast<const uint4*>(c.nnf_wide.p);
   nnf_count_kernel<<<blocks, 256, 0, st>>>(g, f, static_cast<const uint32_t*>(d_bits.p), lay.pitch, dir, tot, n_cells,
                                            static_cast<uint4*>(c.nnf_wide.p), wide_cap, tot + n_cells + 2);
-  CKF(cudaGetLastError());
+  CK(cudaGetLastError());
   // exclusive scan of the per-cell totals (in place); the grand total sizes the candidate array.  A candidate index
   // must stay below 2^31 (bit 31 of a directory entry marks wide / overflow cells): the total is first summed in 64 bits.
   cub::TransformInputIterator<unsigned long long, WidenU32, const uint32_t*> wide_in(tot, WidenU32());
   unsigned long long* d_sum = reinterpret_cast<unsigned long long*>(tot + sum_at);
   size_t tmp_bytes = 0, tmp_sum = 0;
-  CKF(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, tot, tot, static_cast<int>(n_cells + 1), st));
-  CKF(cub::DeviceReduce::Sum(nullptr, tmp_sum, wide_in, d_sum, static_cast<int>(n_cells), st));
+  CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, tot, tot, static_cast<int>(n_cells + 1), st));
+  CK(cub::DeviceReduce::Sum(nullptr, tmp_sum, wide_in, d_sum, static_cast<int>(n_cells), st));
   if ((rc = reserve(eng, d_tmp, std::max(tmp_bytes, tmp_sum))))
-  {
-    cleanup();
     return rc;
-  }
   tmp_sum = d_tmp.cap;
-  CKF(cub::DeviceReduce::Sum(d_tmp.p, tmp_sum, wide_in, d_sum, static_cast<int>(n_cells), st));
+  CK(cub::DeviceReduce::Sum(d_tmp.p, tmp_sum, wide_in, d_sum, static_cast<int>(n_cells), st));
   unsigned long long sum64 = 0;
-  CKF(cudaMemcpyAsync(&sum64, d_sum, 8, cudaMemcpyDeviceToHost, st));
-  CKF(cudaStreamSynchronize(st));
+  CK(cudaMemcpyAsync(&sum64, d_sum, 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
   if (sum64 >= (1ull << 31))
   {
-    cleanup();
-    free_buf(c.nnf_dir);
-    free_buf(c.nnf_wide);
+    c.nnf_dir = DevBuf();
+    c.nnf_wide = DevBuf();
     return MCL3DL_OK;
   }
   tmp_bytes = d_tmp.cap;
-  CKF(cub::DeviceScan::ExclusiveSum(d_tmp.p, tmp_bytes, tot, tot, static_cast<int>(n_cells + 1), st));
+  CK(cub::DeviceScan::ExclusiveSum(d_tmp.p, tmp_bytes, tot, tot, static_cast<int>(n_cells + 1), st));
   uint32_t tail[4] = {0, 0, 0, 0};
-  CKF(cudaMemcpyAsync(tail, tot + n_cells, sizeof(tail), cudaMemcpyDeviceToHost, st));
-  CKF(cudaStreamSynchronize(st));
+  CK(cudaMemcpyAsync(tail, tot + n_cells, sizeof(tail), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
   const uint32_t total = tail[0];
   eng->nnf_wide_cells = std::min<uint32_t>(tail[2], wide_cap);
   eng->nnf_overflow_cells = tail[3];
   const size_t cand_bytes = static_cast<size_t>(total) * sizeof(float4);
   if (n_cells * 8 + cand_bytes > eng->nnf_max_bytes)
   {
-    cleanup();
-    free_buf(c.nnf_dir);
-    free_buf(c.nnf_wide);
+    c.nnf_dir = DevBuf();
+    c.nnf_wide = DevBuf();
     return MCL3DL_OK;
   }
   if ((rc = reserve(eng, c.nnf_cand, std::max<size_t>(cand_bytes, 16))))
-  {
-    cleanup();
     return rc;
-  }
   nnf_base_kernel<<<static_cast<unsigned>((n_cells + 255) / 256), 256, 0, st>>>(dir, tot, n_cells, static_cast<uint4*>(c.nnf_wide.p));
   nnf_fill_kernel<<<blocks, 256, 0, st>>>(g, f, static_cast<const uint32_t*>(d_bits.p), lay.pitch, dir,
                                           static_cast<float4*>(c.nnf_cand.p), n_cells);
-  CKF(cudaGetLastError());
-  CKF(cudaStreamSynchronize(st));
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(st));
   eng->launches += 4;
   f.dir = dir;
   f.cand = static_cast<const float4*>(c.nnf_cand.p);
@@ -1091,9 +1089,7 @@ int build_nn_field(mcl3dl_engine* eng, DeviceCtx& c, cudaStream_t st, const mcl3
   eng->nnf_bytes = n_cells * 8 + cand_bytes + static_cast<size_t>(wide_cap) * sizeof(uint4);
   eng->nnf_cands = total;
   c.map_bytes += eng->nnf_bytes;
-  cleanup();
   return MCL3DL_OK;
-#undef CKF
 }
 
 // Build both grids on one device from the uploaded points.
@@ -1101,56 +1097,38 @@ int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_point* h_
 {
   CK(cudaSetDevice(c.dev));
   cudaStream_t st = c.stream;
-  cudaEvent_t e0, e1;
-  CK(cudaEventCreate(&e0));
-  CK(cudaEventCreate(&e1));
-  DevBuf d_pts, d_bbox, d_keys, d_vals, d_keys2, d_vals2, d_tmp;
+  cudaEvent_t e0 = c.ev[0], e1 = c.ev[1];  // build time: the per-update timing events, unused between calls
+  DevBuf d_pts, d_bbox, d_keys[2], d_vals[2], d_tmp;  // keys / values: [0] per point, [1] sorted by cell
   int rc = MCL3DL_OK;
-  auto cleanup = [&]() {
-    free_buf(d_pts);
-    free_buf(d_bbox);
-    free_buf(d_keys);
-    free_buf(d_vals);
-    free_buf(d_keys2);
-    free_buf(d_vals2);
-    free_buf(d_tmp);
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-  };
-#define CKB(x)            \
-  do                      \
-  {                       \
-    rc = (x);             \
-    if (rc != MCL3DL_OK)  \
-    {                     \
-      cleanup();          \
-      return rc;          \
-    }                     \
-  } while (0)
-#define CKC(call)                                                                       \
-  do                                                                                    \
-  {                                                                                     \
-    cudaError_t e__ = (call);                                                           \
-    if (e__ != cudaSuccess)                                                             \
-    {                                                                                   \
-      eng->err = std::string(#call) + ": " + cudaGetErrorString(e__);                   \
-      cleanup();                                                                        \
-      return MCL3DL_ERR_CUDA;                                                           \
-    }                                                                                   \
-  } while (0)
-
   const uint32_t n32 = static_cast<uint32_t>(n);
   const int tb = 256;
   const int nb = static_cast<int>((n + tb - 1) / tb);
-  CKB(reserve(eng, d_pts, n * sizeof(mcl3dl_point)));
-  CKB(reserve(eng, d_bbox, 12 * sizeof(uint32_t)));
-  CKB(reserve(eng, d_keys, n * 4));
-  CKB(reserve(eng, d_vals, n * 4));
-  CKB(reserve(eng, d_keys2, n * 4));
-  CKB(reserve(eng, d_vals2, n * 4));
-  CKC(cudaMemcpyAsync(d_pts.p, h_pts, n * sizeof(mcl3dl_point), cudaMemcpyHostToDevice, st));
-  CKC(cudaEventRecord(e0, st));
+  if ((rc = reserve(eng, d_pts, n * sizeof(mcl3dl_point))) || (rc = reserve(eng, d_bbox, 12 * sizeof(uint32_t))) ||
+      (rc = reserve(eng, d_keys[0], n * 4)) || (rc = reserve(eng, d_vals[0], n * 4)) || (rc = reserve(eng, d_keys[1], n * 4)) ||
+      (rc = reserve(eng, d_vals[1], n * 4)))
+    return rc;
+  CK(cudaMemcpyAsync(d_pts.p, h_pts, n * sizeof(mcl3dl_point), cudaMemcpyHostToDevice, st));
+  CK(cudaEventRecord(e0, st));
   const mcl3dl_point* pts = static_cast<const mcl3dl_point*>(d_pts.p);
+  uint32_t* keys[2] = {static_cast<uint32_t*>(d_keys[0].p), static_cast<uint32_t*>(d_keys[1].p)};
+  uint32_t* vals[2] = {static_cast<uint32_t*>(d_vals[0].p), static_cast<uint32_t*>(d_vals[1].p)};
+  // CSR order of a grid, once its key kernel has written the (cell, point) pairs to keys[0] / vals[0] and the per-cell
+  // counts to cell_start[1 .. cells]: the pairs sorted by cell into keys[1] / vals[1] (stable: map order inside a cell),
+  // then the inclusive scan that turns the counts into each cell's first index
+  auto sort_csr = [&](size_t cells, uint32_t* cell_start) -> int {
+    int end_bit = 1;
+    while ((size_t(1) << end_bit) < cells && end_bit < 32) ++end_bit;
+    size_t tmp_sort = 0, tmp_scan = 0;
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, keys[0], keys[1], vals[0], vals[1], n32, 0, end_bit, st));
+    CK(cub::DeviceScan::InclusiveSum(nullptr, tmp_scan, cell_start, cell_start, static_cast<int>(cells + 1), st));
+    if (int r = reserve(eng, d_tmp, std::max(tmp_sort, tmp_scan)))
+      return r;
+    size_t tsz = d_tmp.cap;
+    CK(cub::DeviceRadixSort::SortPairs(d_tmp.p, tsz, keys[0], keys[1], vals[0], vals[1], n32, 0, end_bit, st));
+    tsz = d_tmp.cap;
+    CK(cub::DeviceScan::InclusiveSum(d_tmp.p, tsz, cell_start, cell_start, static_cast<int>(cells + 1), st));
+    return MCL3DL_OK;
+  };
 
   // ---- bounding boxes (raw: pcl::getMinMax3D, raycast_using_dda.h:175; rescaled: likelihood grid)
   uint32_t h_bbox[12];
@@ -1161,15 +1139,15 @@ int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_point* h_
     h_bbox[6 + k] = 0xffffffffu;
     h_bbox[9 + k] = 0u;
   }
-  CKC(cudaMemcpyAsync(d_bbox.p, h_bbox, sizeof(h_bbox), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(d_bbox.p, h_bbox, sizeof(h_bbox), cudaMemcpyHostToDevice, st));
   const float wx = eng->has_lik ? eng->lik.dist_weight[0] : 1.0f;
   const float wy = eng->has_lik ? eng->lik.dist_weight[1] : 1.0f;
   const float wz = eng->has_lik ? eng->lik.dist_weight[2] : 1.0f;
   bbox_kernel<<<std::min(nb, c.sm_count * 8), tb, 0, st>>>(pts, n, wx, wy, wz, static_cast<uint32_t*>(d_bbox.p));
-  CKC(cudaGetLastError());
+  CK(cudaGetLastError());
   eng->launches++;
-  CKC(cudaMemcpyAsync(h_bbox, d_bbox.p, sizeof(h_bbox), cudaMemcpyDeviceToHost, st));
-  CKC(cudaStreamSynchronize(st));
+  CK(cudaMemcpyAsync(h_bbox, d_bbox.p, sizeof(h_bbox), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
   float raw_min[3], raw_max[3], sc_min[3], sc_max[3];
   for (int k = 0; k < 3; ++k)
   {
@@ -1188,10 +1166,7 @@ int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_point* h_
     // (1 % margin: the float cell function can be off by ~1e-7 x cells-per-axis, and the kernels rely on <= 3)
     const float cell = std::max(eng->lik.match_dist_min * eng->nn_cell_factor, eng->likdev.rpad * 1.01f);
     if (!(cell > 0.0f))
-    {
-      cleanup();
       return MCL3DL_ERR_INVALID_ARG;
-    }
     g.inv_cell = 1.0f / cell;
     g.wx = wx;
     g.wy = wy;
@@ -1206,10 +1181,7 @@ int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_point* h_
       total *= dims[k];
     }
     if (total >= (int64_t(1) << 31))
-    {
-      cleanup();
       return MCL3DL_ERR_TOO_LARGE;
-    }
     g.nx = dims[0];
     g.ny = dims[1];
     g.nz = dims[2];
@@ -1217,37 +1189,23 @@ int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_point* h_
     g.oy = org[1];
     g.oz = org[2];
     const size_t cells = static_cast<size_t>(total);
-    CKB(reserve(eng, c.nn_cell_start, (cells + 1) * 4));
-    CKB(reserve(eng, c.nn_pts, n * 16));
-    CKC(cudaMemsetAsync(c.nn_cell_start.p, 0, (cells + 1) * 4, st));
-    nn_key_kernel<<<nb, tb, 0, st>>>(pts, n32, g, static_cast<uint32_t*>(d_keys.p), static_cast<uint32_t*>(d_vals.p),
-                                     static_cast<uint32_t*>(c.nn_cell_start.p));
-    CKC(cudaGetLastError());
+    if ((rc = reserve(eng, c.nn_cell_start, (cells + 1) * 4)) || (rc = reserve(eng, c.nn_pts, n * 16)))
+      return rc;
+    uint32_t* cell_start = static_cast<uint32_t*>(c.nn_cell_start.p);
+    CK(cudaMemsetAsync(cell_start, 0, (cells + 1) * 4, st));
+    nn_key_kernel<<<nb, tb, 0, st>>>(pts, n32, g, keys[0], vals[0], cell_start);
+    CK(cudaGetLastError());
     eng->launches++;
-    size_t tmp_sort = 0, tmp_scan = 0;
-    int end_bit = 1;
-    while ((int64_t(1) << end_bit) < total && end_bit < 32) ++end_bit;
-    CKC(cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, static_cast<uint32_t*>(d_keys.p),
-                                        static_cast<uint32_t*>(d_keys2.p), static_cast<uint32_t*>(d_vals.p),
-                                        static_cast<uint32_t*>(d_vals2.p), n32, 0, end_bit, st));
-    CKC(cub::DeviceScan::InclusiveSum(nullptr, tmp_scan, static_cast<uint32_t*>(c.nn_cell_start.p),
-                                      static_cast<uint32_t*>(c.nn_cell_start.p), static_cast<int>(cells + 1), st));
-    CKB(reserve(eng, d_tmp, std::max(tmp_sort, tmp_scan)));
-    size_t tsz = d_tmp.cap;
-    CKC(cub::DeviceRadixSort::SortPairs(d_tmp.p, tsz, static_cast<uint32_t*>(d_keys.p), static_cast<uint32_t*>(d_keys2.p),
-                                        static_cast<uint32_t*>(d_vals.p), static_cast<uint32_t*>(d_vals2.p), n32, 0,
-                                        end_bit, st));
-    tsz = d_tmp.cap;
-    CKC(cub::DeviceScan::InclusiveSum(d_tmp.p, tsz, static_cast<uint32_t*>(c.nn_cell_start.p),
-                                      static_cast<uint32_t*>(c.nn_cell_start.p), static_cast<int>(cells + 1), st));
-    nn_gather_kernel<<<nb, tb, 0, st>>>(pts, n32, static_cast<uint32_t*>(d_vals2.p), wx, wy, wz,
-                                        static_cast<float4*>(c.nn_pts.p));
-    CKC(cudaGetLastError());
+    if ((rc = sort_csr(cells, cell_start)))
+      return rc;
+    nn_gather_kernel<<<nb, tb, 0, st>>>(pts, n32, vals[1], wx, wy, wz, static_cast<float4*>(c.nn_pts.p));
+    CK(cudaGetLastError());
     eng->launches += 3;
-    g.cell_start = static_cast<const uint32_t*>(c.nn_cell_start.p);
+    g.cell_start = cell_start;
     g.pts = static_cast<const float4*>(c.nn_pts.p);
 #if MCL3DL_NEAR_BITS
-    CKB(build_near_field(eng, c, st, pts, n32, wx, wy, wz, eng->likdev.rpad, eng->near_k, sc_min, sc_max, c.near_lik, g.near, 0));
+    if ((rc = build_near_field(eng, c, st, pts, n32, wx, wy, wz, eng->likdev.rpad, eng->near_k, sc_min, sc_max, c.near_lik, g.near, 0)))
+      return rc;
 #endif
     // NN field: exact for the likelihood radius and, with the KD-tree raycaster, for its marching radius as well
     {
@@ -1261,8 +1219,8 @@ int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_point* h_
         radius = std::max(radius, eng->nnf_kd_r2 ? tmp.r2_pad : tmp.r1_pad);
       }
       g.field = NnFieldDev{};
-      if (eng->nnf)
-        CKB(build_nn_field(eng, c, st, pts, n32, g, radius, sc_min, sc_max));
+      if (eng->nnf && (rc = build_nn_field(eng, c, st, pts, n32, g, radius, sc_min, sc_max)))
+        return rc;
     }
     // window table of the CSR-window kernel (lik_kernel_wi): only when the field is not staged
     size_t row3_total = 0;
@@ -1270,15 +1228,16 @@ int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_point* h_
     if (!g.field.dir)
     {
       row3_total = static_cast<size_t>(g.nz) * g.nx * g.nyp;
-      CKB(reserve(eng, c.nn_row3, (row3_total + 2) * sizeof(uint2)));
+      if ((rc = reserve(eng, c.nn_row3, (row3_total + 2) * sizeof(uint2))))
+        return rc;
       g.row3 = static_cast<const uint2*>(c.nn_row3.p);
       nn_row3_kernel<<<static_cast<unsigned>((row3_total + 255) / 256), 256, 0, st>>>(g, static_cast<uint2*>(c.nn_row3.p), row3_total);
-      CKC(cudaGetLastError());
+      CK(cudaGetLastError());
       eng->launches++;
     }
     else
     {
-      free_buf(c.nn_row3);
+      c.nn_row3 = DevBuf();
       g.row3 = nullptr;
     }
     c.nn = g;
@@ -1293,26 +1252,24 @@ int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_point* h_
   }
   // ---- the raw points by original index (the KD-tree raycaster's colliding point; the chunk rule of
   // mcl3dl_match_output): keep the upload wherever there is a likelihood grid
-  free_buf(c.raw_pts);
   if (eng->has_lik)
   {
-    c.raw_pts = d_pts;
-    d_pts = DevBuf();
+    c.raw_pts = std::move(d_pts);
     c.map_bytes += n * 16;
   }
+  else
+    c.raw_pts = DevBuf();
 
   // ---- KD-tree raycaster: marches over the likelihood grid; needs the raw points by original index
   if (eng->has_beam && !eng->beam.use_raycast_using_dda)
   {
     if (!eng->has_lik)
-    {
-      cleanup();
       return MCL3DL_ERR_INVALID_ARG;
-    }
     fill_dda_scalars(eng->beam, c.dda);
     fill_kd_scalars(eng->beam, c.kd);
 #if MCL3DL_NEAR_BITS
-    CKB(build_near_field(eng, c, st, pts, n32, wx, wy, wz, c.kd.r1_pad, eng->near_kd_k, sc_min, sc_max, c.near_kd, c.kd.near, 1));
+    if ((rc = build_near_field(eng, c, st, pts, n32, wx, wy, wz, c.kd.r1_pad, eng->near_kd_k, sc_min, sc_max, c.near_kd, c.kd.near, 1)))
+      return rc;
     c.near_kd_r = c.kd.r1_pad;
 #endif
     c.kd.raw_pts = static_cast<const float4*>(c.raw_pts.p);
@@ -1323,10 +1280,7 @@ int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_point* h_
     DdaGridDev g{};
     fill_dda_scalars(eng->beam, g);
     if (!(g.grid > 0.0))
-    {
-      cleanup();
       return MCL3DL_ERR_INVALID_ARG;
-    }
     int64_t total = 1;
     int dims[3];
     for (int k = 0; k < 3; ++k)
@@ -1337,10 +1291,7 @@ int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_point* h_
       total *= dims[k];
     }
     if (total >= (int64_t(1) << 31))  // `int point_total` (:176)
-    {
-      cleanup();
       return MCL3DL_ERR_TOO_LARGE;
-    }
     g.nx = dims[0];
     g.ny = dims[1];
     g.nz = dims[2];
@@ -1352,35 +1303,21 @@ int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_point* h_
     g.max_z = raw_max[2];
     const size_t cells = static_cast<size_t>(total);
     const size_t occ_words = (cells + 31) / 32 + 1;
-    CKB(reserve(eng, c.dda_cell_start, (cells + 2) * 4));
-    CKB(reserve(eng, c.dda_occ, occ_words * 4));
-    CKB(reserve(eng, c.dda_pts, n * 16));
-    CKC(cudaMemsetAsync(c.dda_cell_start.p, 0, (cells + 2) * 4, st));
-    CKC(cudaMemsetAsync(c.dda_occ.p, 0, occ_words * 4, st));
-    dda_key_kernel<<<nb, tb, 0, st>>>(pts, n32, g, static_cast<uint32_t*>(d_keys.p), static_cast<uint32_t*>(d_vals.p),
-                                      static_cast<uint32_t*>(c.dda_cell_start.p), static_cast<uint32_t*>(c.dda_occ.p));
-    CKC(cudaGetLastError());
-    size_t tmp_sort = 0, tmp_scan = 0;
-    int end_bit = 1;
-    while ((int64_t(1) << end_bit) < total && end_bit < 32) ++end_bit;
-    CKC(cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, static_cast<uint32_t*>(d_keys.p),
-                                        static_cast<uint32_t*>(d_keys2.p), static_cast<uint32_t*>(d_vals.p),
-                                        static_cast<uint32_t*>(d_vals2.p), n32, 0, end_bit, st));
-    CKC(cub::DeviceScan::InclusiveSum(nullptr, tmp_scan, static_cast<uint32_t*>(c.dda_cell_start.p),
-                                      static_cast<uint32_t*>(c.dda_cell_start.p), static_cast<int>(cells + 1), st));
-    CKB(reserve(eng, d_tmp, std::max(tmp_sort, tmp_scan)));
-    size_t tsz = d_tmp.cap;
-    CKC(cub::DeviceRadixSort::SortPairs(d_tmp.p, tsz, static_cast<uint32_t*>(d_keys.p), static_cast<uint32_t*>(d_keys2.p),
-                                        static_cast<uint32_t*>(d_vals.p), static_cast<uint32_t*>(d_vals2.p), n32, 0,
-                                        end_bit, st));
-    tsz = d_tmp.cap;
-    CKC(cub::DeviceScan::InclusiveSum(d_tmp.p, tsz, static_cast<uint32_t*>(c.dda_cell_start.p),
-                                      static_cast<uint32_t*>(c.dda_cell_start.p), static_cast<int>(cells + 1), st));
-    dda_gather_kernel<<<nb, tb, 0, st>>>(pts, n32, static_cast<uint32_t*>(d_vals2.p), static_cast<float4*>(c.dda_pts.p));
-    CKC(cudaGetLastError());
+    if ((rc = reserve(eng, c.dda_cell_start, (cells + 2) * 4)) || (rc = reserve(eng, c.dda_occ, occ_words * 4)) ||
+        (rc = reserve(eng, c.dda_pts, n * 16)))
+      return rc;
+    uint32_t* cell_start = static_cast<uint32_t*>(c.dda_cell_start.p);
+    CK(cudaMemsetAsync(cell_start, 0, (cells + 2) * 4, st));
+    CK(cudaMemsetAsync(c.dda_occ.p, 0, occ_words * 4, st));
+    dda_key_kernel<<<nb, tb, 0, st>>>(pts, n32, g, keys[0], vals[0], cell_start, static_cast<uint32_t*>(c.dda_occ.p));
+    CK(cudaGetLastError());
+    if ((rc = sort_csr(cells, cell_start)))
+      return rc;
+    dda_gather_kernel<<<nb, tb, 0, st>>>(pts, n32, vals[1], static_cast<float4*>(c.dda_pts.p));
+    CK(cudaGetLastError());
     eng->launches += 4;
     g.occ = static_cast<const uint32_t*>(c.dda_occ.p);
-    g.cell_start = static_cast<const uint32_t*>(c.dda_cell_start.p);
+    g.cell_start = cell_start;
     g.pts = static_cast<const float4*>(c.dda_pts.p);
     c.dda = g;
     c.map_bytes += (cells + 2) * 4 + occ_words * 4 + n * 16;
@@ -1391,16 +1328,13 @@ int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_point* h_
       eng->info.dda_max[k] = raw_max[k];
     }
   }
-  CKC(cudaEventRecord(e1, st));
-  CKC(cudaStreamSynchronize(st));
+  CK(cudaEventRecord(e1, st));
+  CK(cudaStreamSynchronize(st));
   float ms = 0;
-  CKC(cudaEventElapsedTime(&ms, e0, e1));
+  CK(cudaEventElapsedTime(&ms, e0, e1));
   eng->info.build_ms = std::max(eng->info.build_ms, static_cast<double>(ms));
   eng->info.device_bytes = c.map_bytes;
-  cleanup();
   return MCL3DL_OK;
-#undef CKB
-#undef CKC
 }
 }  // namespace
 
@@ -1481,7 +1415,7 @@ int mcl3dl_create(mcl3dl_engine** out, const int* device_ids, int n_devices)
     eng->nnf_max_bytes = static_cast<size_t>(std::max(std::atol(v), 1L)) << 20;
   if (const char* o = std::getenv("MCL3DL_OVERLAP"))
     eng->overlap = std::atoi(o) != 0;
-  eng->devs.resize(n_devices);
+  eng->devs = std::vector<DeviceCtx>(n_devices);  // at its final size: a context never moves
   for (int i = 0; i < n_devices; ++i)
   {
     DeviceCtx& c = eng->devs[i];
@@ -1523,8 +1457,6 @@ int mcl3dl_create(mcl3dl_engine** out, const int* device_ids, int n_devices)
   return MCL3DL_OK;
 }
 
-static void xchg_close(DeviceCtx& c);
-
 int mcl3dl_host_alloc(mcl3dl_engine* eng, size_t bytes, void** out)
 {
   if (!eng || !out || bytes == 0 || eng->devs.empty())
@@ -1563,42 +1495,7 @@ void mcl3dl_destroy(mcl3dl_engine* eng)
 {
   if (!eng)
     return;
-  for (DeviceCtx& c : eng->devs)
-  {
-    cudaSetDevice(c.dev);
-    if (c.stream)
-      cudaStreamSynchronize(c.stream);
-    xchg_close(c);
-    free_buf(c.xchg);
-    free_buf(c.x_ticket);
-    for (DevBuf* b : {&c.r_states[0], &c.r_states[1], &c.r_prob, &c.r_accum, &c.r_poses, &c.r_extra, &c.r_est, &c.s_raw, &c.s_keys[0],
-                      &c.s_keys[1], &c.s_vals[0], &c.s_vals[1], &c.s_key_label[0], &c.s_key_label[1], &c.s_flags[0],
-                      &c.s_flags[1], &c.s_pos[0], &c.s_pos[1], &c.s_ds, &c.s_clip[0], &c.s_clip[1], &c.s_out[0], &c.s_out[1], &c.s_tmp, &c.s_counts,
-                      &c.m_in, &c.m_tf, &c.m_flags[0], &c.m_flags[1], &c.m_pos[0], &c.m_pos[1], &c.m_tmp})
-      free_buf(*b);
-    if (c.m_host)
-      cudaFreeHost(c.m_host);
-    for (DevBuf* b : {&c.nn_cell_start, &c.nn_pts, &c.nn_row3, &c.dda_occ, &c.dda_cell_start, &c.dda_pts, &c.raw_pts, &c.near_lik, &c.near_kd, &c.nnf_dir, &c.nnf_cand, &c.nnf_wide, &c.fld_cells, &c.d_poses,
-                      &c.d_out, &c.d_status, &c.d_stats, &c.d_partial, &c.d_tickets, &c.d_tally, &c.d_queue, &c.d_lacc, &c.d_w, &c.d_post, &c.d_wpart, &c.d_wticket})
-      free_buf(*b);
-    if (c.fld_nodes.ptr)
-      cudaFree(c.fld_nodes.ptr);
-    if (c.h_pinned)
-      cudaFreeHost(c.h_pinned);
-    for (auto& e : c.ev)
-      if (e)
-        cudaEventDestroy(e);
-    for (cudaEvent_t e : {c.ev_fork, c.ev_join, c.ev_b0, c.ev_b1})
-      if (e)
-        cudaEventDestroy(e);
-    if (c.side)
-    {
-      cudaStreamSynchronize(c.side);
-      cudaStreamDestroy(c.side);
-    }
-    if (c.stream)
-      cudaStreamDestroy(c.stream);
-  }
+  eng->devs.clear();  // each context waits for its streams before it releases anything
   for (auto& b : eng->host_blocks)  // (blocks the caller did not return; its pointers into them dangle from here on)
     cudaFreeHost(b.first);
   delete eng;
@@ -1638,11 +1535,8 @@ int mcl3dl_set_map(mcl3dl_engine* eng, const mcl3dl_point* pts, size_t n, uint64
     if (rc != MCL3DL_OK)
       return rc;
     c.fld_nodes_valid = false;  // a volume of the previous map is stale
-    if (c.fld_nodes.ptr)
-    {
-      cudaFree(c.fld_nodes.ptr);
-      c.fld_nodes = cudaPitchedPtr{};
-    }
+    c.fld_mem = DevBuf();
+    c.fld_nodes = cudaPitchedPtr{};
     if (eng->field_mode && eng->has_lik && (rc = stage_field(eng, c, nullptr)) != MCL3DL_OK)
       return rc;
   }
@@ -1916,7 +1810,7 @@ static int stage_inputs(mcl3dl_engine* eng, DeviceCtx& c, const Share& s, const 
                         const mcl3dl_point* beam, const float* origins, size_t n_origins, const float* prior, const float* extra,
                         bool timed)
 {
-  char* hp = static_cast<char*>(c.h_pinned);
+  char* hp = static_cast<char*>(c.h_pinned.p);
   if (poses) std::memcpy(hp, poses + s.p0, s.o_lik);
   if (s.o_beam > s.o_lik) std::memcpy(hp + s.o_lik, lik, s.o_beam - s.o_lik);
   if (s.o_org > s.o_beam) std::memcpy(hp + s.o_beam, beam, s.o_org - s.o_beam);
@@ -2131,7 +2025,7 @@ static int resident_update(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_point*
   // prior * likelihood from the resident probabilities; the posterior is written over them (the weights were read
   // into d_w first); a vanished total leaves them untouched = the reference's "restore" (pf.h:274-278)
   float* prob = static_cast<float*>(c.r_prob.p);
-  WeightPartial* h_part = reinterpret_cast<WeightPartial*>(static_cast<char*>(c.h_pinned) + s.o_part);
+  WeightPartial* h_part = reinterpret_cast<WeightPartial*>(static_cast<char*>(c.h_pinned.p) + s.o_part);
   rc = fold_weights(eng, c, d_rec, prob, with_odom ? static_cast<const float*>(c.r_extra.p) : nullptr, prob, P, n_lik, 0, h_part,
                     nullptr);
   if (rc != MCL3DL_OK)
@@ -2157,7 +2051,7 @@ int mcl3dl_particles_measure_update(mcl3dl_engine* eng, const mcl3dl_point* lik_
   CK(cudaSetDevice(c.dev));
   // scans + origins up in one block (as in mcl3dl_measure); the poses come from the resident states
   const Share s = share_of(P, 1, 0, 0, n_lik, n_beam, n_origins, 0, 0, 0, 0, 0);
-  if ((rc = reserve_pinned(eng, c, s.total)) || (rc = reserve(eng, c.d_poses, s.in_bytes)) ||
+  if ((rc = reserve(eng, c.h_pinned, s.total)) || (rc = reserve(eng, c.d_poses, s.in_bytes)) ||
       (rc = stage_inputs(eng, c, s, nullptr, lik_pts, beam_pts, origins_xyz, n_origins, nullptr, nullptr, false)))
     return rc;
   const char* d_in = static_cast<const char*>(c.d_poses.p);
@@ -2185,7 +2079,7 @@ int mcl3dl_particles_measure_update_prepared(mcl3dl_engine* eng, const float* or
   CK(cudaSetDevice(c.dev));
   // only the origins go up; the scans are the prepared ones
   const Share s = share_of(P, 1, 0, 0, 0, 0, n_origins, 0, 0, 0, 0, 0);
-  if ((rc = reserve_pinned(eng, c, s.total)) || (rc = reserve(eng, c.d_poses, s.in_bytes)) ||
+  if ((rc = reserve(eng, c.h_pinned, s.total)) || (rc = reserve(eng, c.d_poses, s.in_bytes)) ||
       (rc = stage_inputs(eng, c, s, nullptr, nullptr, nullptr, origins_xyz, n_origins, nullptr, nullptr, false)))
     return rc;
   // (beam labels are the raw cloud's, voted per voxel: the caller's origins must cover them, as in the node)
@@ -2223,7 +2117,7 @@ int mcl3dl_scan_prepare(mcl3dl_engine* eng, const mcl3dl_point* raw, size_t n_ra
     if (info) *info = c.s_info;
     return MCL3DL_OK;
   }
-  if ((rc = reserve_pinned(eng, c, 256)))
+  if ((rc = reserve(eng, c.h_pinned, 256)))
     return rc;
   CK(cudaMemcpyAsync(c.s_raw.p, raw, n_raw * 16, cudaMemcpyHostToDevice, st));
   const mcl3dl_point* d_raw = static_cast<const mcl3dl_point*>(c.s_raw.p);
@@ -2311,9 +2205,9 @@ int mcl3dl_scan_prepare(mcl3dl_engine* eng, const mcl3dl_point* raw, size_t n_ra
   CK(cudaGetLastError());
   eng->launches += 5;
   uint32_t h_counts[5];
-  CK(cudaMemcpyAsync(c.h_pinned, counts, sizeof(h_counts), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(c.h_pinned.p, counts, sizeof(h_counts), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
-  std::memcpy(h_counts, c.h_pinned, sizeof(h_counts));
+  std::memcpy(h_counts, c.h_pinned.p, sizeof(h_counts));
   c.s_info.n_downsampled = h_counts[0];
   c.s_info.n_lik_clipped = h_counts[1];
   c.s_info.n_beam_clipped = h_counts[2];
@@ -2382,16 +2276,8 @@ int mcl3dl_match_output(mcl3dl_engine* eng, const mcl3dl_pose* pose, const mcl3d
       return rc;
   // page-locked result block: [2 counts | 56 B pad | matched cloud | unmatched cloud], written by the compaction itself so
   // that one synchronise ends the call
-  const size_t host_bytes = 64 + 2 * cnt * 16;
-  if (host_bytes > c.m_host_cap)
-  {
-    if (c.m_host)
-      CK(cudaFreeHost(c.m_host));
-    c.m_host = nullptr;
-    c.m_host_cap = 0;
-    CK(cudaMallocHost(&c.m_host, host_bytes));
-    c.m_host_cap = host_bytes;
-  }
+  if ((rc = reserve(eng, c.m_host, 64 + 2 * cnt * 16)))
+    return rc;
   if (pts)
   {
     CK(cudaMemcpyAsync(c.m_in.p, pts, cnt * 16, cudaMemcpyHostToDevice, st));
@@ -2415,7 +2301,7 @@ int mcl3dl_match_output(mcl3dl_engine* eng, const mcl3dl_pose* pose, const mcl3d
   CK(cub::DeviceScan::ExclusiveSum(nullptr, t_scan, f[0], ps[0], n32, st));
   if ((rc = reserve(eng, c.m_tmp, t_scan + 256)))
     return rc;
-  char* hp = static_cast<char*>(c.m_host);
+  char* hp = static_cast<char*>(c.m_host.p);
   uint32_t* h_counts = reinterpret_cast<uint32_t*>(hp);
   mcl3dl_point* h_out[2] = {reinterpret_cast<mcl3dl_point*>(hp + 64), reinterpret_cast<mcl3dl_point*>(hp + 64 + cnt * 16)};
   for (int k = 0; k < 2; ++k)
@@ -2451,7 +2337,7 @@ int mcl3dl_particles_estimate(mcl3dl_engine* eng, const mcl3dl_pose* prev, float
   const size_t part_doubles = static_cast<size_t>(grid) * (kEstSums + 2);
   const size_t hdr = (sizeof(EstHeader) + 255) & ~size_t(255);
   int rc;
-  if ((rc = reserve(eng, c.r_est, hdr + part_doubles * sizeof(double))) || (rc = reserve_pinned(eng, c, sizeof(EstHeader) + sizeof(PfState) + 64)))
+  if ((rc = reserve(eng, c.r_est, hdr + part_doubles * sizeof(double))) || (rc = reserve(eng, c.h_pinned, sizeof(EstHeader) + sizeof(PfState) + 64)))
     return rc;
   BiasDev b{};
   if (prev)
@@ -2481,7 +2367,7 @@ int mcl3dl_particles_estimate(mcl3dl_engine* eng, const mcl3dl_pose* prev, float
   pf_est_finish2_kernel<<<1, 32, 0, st>>>(parts, grid, h);
   CK(cudaGetLastError());
   eng->launches += 4;
-  char* hp = static_cast<char*>(c.h_pinned);
+  char* hp = static_cast<char*>(c.h_pinned.p);
   CK(cudaMemcpyAsync(hp, h, sizeof(EstHeader), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   EstHeader hh;
@@ -2510,17 +2396,6 @@ int mcl3dl_particles_estimate(mcl3dl_engine* eng, const mcl3dl_pose* prev, float
 static size_t xchg_flags_offset(size_t n_local, int world)
 {
   return (2 * static_cast<size_t>(world) * n_local * sizeof(mcl3dl_result) + 255) & ~size_t(255);  // two arrays, by step parity
-}
-
-static void xchg_close(DeviceCtx& c)
-{
-  for (void*& o : c.x_opened)
-    if (o)
-    {
-      cudaIpcCloseMemHandle(o);
-      o = nullptr;
-    }
-  c.x_ready = false;
 }
 
 int mcl3dl_exchange_create(mcl3dl_engine* eng, size_t n_local, int world, int rank, void* ipc_handle_out)
@@ -2575,7 +2450,7 @@ int mcl3dl_exchange_open(mcl3dl_engine* eng, const void* ipc_handles /* world x 
       if (e != cudaSuccess)
       {
         eng->err = std::string("cudaIpcOpenMemHandle: ") + cudaGetErrorString(e);
-        xchg_close(c);
+        c.xchg_close();
         return MCL3DL_ERR_CUDA;
       }
       c.x_opened[g] = base;
@@ -2668,7 +2543,7 @@ static int measure_host(mcl3dl_engine* eng, const mcl3dl_pose* poses, size_t P, 
     cudaStream_t st = c.stream;
     const size_t b_rec = s.n * sizeof(mcl3dl_result), b_status = status ? s.n * n_beam : 0;
     const bool poses_direct = s.o_lik >= eng->direct_min_bytes && in_host_block(eng, poses + s.p0, s.o_lik);
-    if ((rc = reserve_pinned(eng, c, s.total)) || (rc = reserve(eng, c.d_poses, s.in_bytes)) ||
+    if ((rc = reserve(eng, c.h_pinned, s.total)) || (rc = reserve(eng, c.d_poses, s.in_bytes)) ||
         (rc = reserve(eng, c.d_out, b_rec)) || (rc = reserve(eng, c.d_status, b_status)) ||
         (rc = stage_inputs(eng, c, s, poses_direct ? nullptr : poses, lik_pts, beam_pts, origins_xyz, n_origins, nullptr,
                            nullptr, timed)))
@@ -2679,7 +2554,7 @@ static int measure_host(mcl3dl_engine* eng, const mcl3dl_pose* poses, size_t P, 
     // small updates: the kernels store their records straight into the pinned block (cudaMallocHost memory is mapped
     // into the unified address space), which saves the D2H copy launch; large ones keep the bulk copy
     const bool zc = !status && s.n <= eng->zero_copy_max;  // (per-ray status bytes would be scattered 1-byte PCIe writes)
-    char* hp = static_cast<char*>(c.h_pinned);
+    char* hp = static_cast<char*>(c.h_pinned.p);
     mcl3dl_result* h_out = out_direct(s) ? out + s.p0 : reinterpret_cast<mcl3dl_result*>(hp + s.o_rec);
     mcl3dl_result* k_out = zc ? h_out : static_cast<mcl3dl_result*>(c.d_out.p);
     const char* d_in = static_cast<const char*>(c.d_poses.p);
@@ -2706,7 +2581,7 @@ static int measure_host(mcl3dl_engine* eng, const mcl3dl_pose* poses, size_t P, 
       continue;
     CK(cudaSetDevice(c.dev));
     CK(cudaStreamSynchronize(c.stream));
-    const char* hp = static_cast<const char*>(c.h_pinned);
+    const char* hp = static_cast<const char*>(c.h_pinned.p);
     if (out && !out_direct(s))  // (else: already there)
       std::memcpy(out + s.p0, hp + s.o_rec, s.n * sizeof(mcl3dl_result));
     if (status) std::memcpy(status + s.p0 * n_beam, hp + s.o_status, s.n * n_beam);
@@ -2749,7 +2624,7 @@ int mcl3dl_measure_update(mcl3dl_engine* eng, const mcl3dl_pose* poses, size_t P
       continue;
     CK(cudaSetDevice(c.dev));
     cudaStream_t st = c.stream;
-    if ((rc = reserve_pinned(eng, c, s.total)) || (rc = reserve(eng, c.d_poses, s.in_bytes)) ||
+    if ((rc = reserve(eng, c.h_pinned, s.total)) || (rc = reserve(eng, c.d_poses, s.in_bytes)) ||
         (rc = reserve(eng, c.d_out, s.n * sizeof(mcl3dl_result))) || (rc = reserve(eng, c.d_post, s.n * 4)) ||
         (rc = stage_inputs(eng, c, s, poses, lik_pts, beam_pts, origins_xyz, n_origins, prior, extra, false)))
       return rc;
@@ -2757,7 +2632,7 @@ int mcl3dl_measure_update(mcl3dl_engine* eng, const mcl3dl_pose* poses, size_t P
     const float* d_prior = reinterpret_cast<const float*>(d_in + s.o_prior);
     const float* d_extra = extra ? reinterpret_cast<const float*>(d_in + s.o_extra) : nullptr;
     mcl3dl_result* d_rec = static_cast<mcl3dl_result*>(c.d_out.p);
-    char* hp = static_cast<char*>(c.h_pinned);
+    char* hp = static_cast<char*>(c.h_pinned.p);
     WeightPartial* h_part = reinterpret_cast<WeightPartial*>(hp + s.o_part);
     rc = launch_models(eng, c, reinterpret_cast<const mcl3dl_pose*>(d_in), s.n, reinterpret_cast<const mcl3dl_point*>(d_in + s.o_lik),
                        n_lik, reinterpret_cast<const mcl3dl_point*>(d_in + s.o_beam), n_beam,
@@ -2788,7 +2663,7 @@ int mcl3dl_measure_update(mcl3dl_engine* eng, const mcl3dl_pose* poses, size_t P
       continue;
     CK(cudaSetDevice(c.dev));
     CK(cudaStreamSynchronize(c.stream));
-    const WeightPartial& wp = *reinterpret_cast<const WeightPartial*>(static_cast<const char*>(c.h_pinned) + sh[d].o_part);
+    const WeightPartial& wp = *reinterpret_cast<const WeightPartial*>(static_cast<const char*>(c.h_pinned.p) + sh[d].o_part);
     w1.sum += wp.sum;
     w1.qmin = std::min(w1.qmin, wp.qmin);
     w1.qmax = std::max(w1.qmax, wp.qmax);
@@ -2804,7 +2679,7 @@ int mcl3dl_measure_update(mcl3dl_engine* eng, const mcl3dl_pose* poses, size_t P
       continue;
     CK(cudaSetDevice(c.dev));
     cudaStream_t st = c.stream;
-    char* hp = static_cast<char*>(c.h_pinned);
+    char* hp = static_cast<char*>(c.h_pinned.p);
     if (kept)
     {
       const WeightPartial* f2;
@@ -2825,7 +2700,7 @@ int mcl3dl_measure_update(mcl3dl_engine* eng, const mcl3dl_pose* poses, size_t P
     CK(cudaSetDevice(c.dev));
     if (G > 1)
       CK(cudaStreamSynchronize(c.stream));
-    const char* hp = static_cast<const char*>(c.h_pinned);
+    const char* hp = static_cast<const char*>(c.h_pinned.p);
     if (kept)
     {
       std::memcpy(posterior + s.p0, hp + s.o_post, s.n * 4);
@@ -2875,7 +2750,9 @@ int mcl3dl_collect_stats(mcl3dl_engine* eng, int enable)
     int rc = reserve(eng, c.d_stats, 5 * sizeof(unsigned long long));
     if (rc != MCL3DL_OK)
       return rc;
-    CK(cudaMemset(c.d_stats.p, 0, 5 * sizeof(unsigned long long)));
+    // every call restarts the counters: done before the call returns, so ahead of any later kernel on any stream
+    CK(cudaMemsetAsync(c.d_stats.p, 0, 5 * sizeof(unsigned long long), c.stream));
+    CK(cudaStreamSynchronize(c.stream));
     c.stats_on = enable != 0;
   }
   return MCL3DL_OK;
