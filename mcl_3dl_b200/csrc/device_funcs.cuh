@@ -605,13 +605,92 @@ __device__ __forceinline__ int nnf_lookup(const NnFieldDev& f, float qx, float q
   return nnf_slot(f, d, (vx & 1) | ((vy & 1) << 1) | ((vz & 1) << 2), start);
 }
 
-// Warp-cooperative candidate scan (kernels.cuh: lik_kernel_nf, phase B).  The candidate lists of a warp's evals are laid
-// end to end in one list of (eval, candidate) slots; the list of eval `e` occupies slots [base, base + count).  A pass
-// covers slots [lo, hi): name `e` as the owner of its slots in that range (own[slot - lo]).
+// Warp-cooperative candidate scan (kernels.cuh: nf_warp_scan, phase B).  The candidate lists of a warp's evals are laid
+// end to end in one list of (eval, candidate) slots, lane after lane and within a lane u = 0 .. U - 1, so the list of
+// eval e = u * 32 + lane occupies slots [base, base + count) and is the o-th list in slot order, o = lane * U + u (its
+// ordinal).  A pass covers slots [lo, hi), and the owner table own[slot - lo] names the eval whose list holds the slot.
+// The table is built without a loop over list lengths.  Every list that reaches into the pass marks its first slot in
+// the pass with its ordinal, on a cleared table.  Each slot of the pass lies in a list, and the pass's first slot is
+// always marked, so the largest mark at or before a slot is the ordinal of the slot's list (a cleared byte, 0, never
+// raises the maximum).  A warp-wide inclusive max-scan over the pass's bytes gives every slot its ordinal, and the
+// ordinals are turned back into evals as the bytes are stored.
+
+// The serial fill the table replaced: a loop over each list's slots in the pass, naming its eval (own[slot - lo] = e).
+// The kernels no longer call it; the host models of the scan keep it as the definition the table must equal.
 __device__ __forceinline__ void nnf_fill_owner(uint8_t* own, int lo, int hi, int base, int count, int e)
 {
   const int a = max(base, lo), b = min(base + count, hi);
   for (int i = a; i < b; ++i) own[i - lo] = static_cast<uint8_t>(e);
+}
+
+// The byte permute, 16x2 three-way maximum and leading-zero count of the table build.  tests/hostsim compiles this file
+// for the host, where they are restated here bit for bit (the selector uses the low 3 bits of each nibble).
+__device__ __forceinline__ uint32_t nnf_prmt(uint32_t x, uint32_t y, uint32_t sel)
+{
+#ifdef MCL3DL_HOSTSIM
+  const unsigned long long v = (static_cast<unsigned long long>(y) << 32) | x;
+  uint32_t r = 0;
+  for (int i = 0; i < 4; ++i) r |= static_cast<uint32_t>((v >> (8 * ((sel >> (4 * i)) & 7u))) & 0xffu) << (8 * i);
+  return r;
+#else
+  return __byte_perm(x, y, sel);
+#endif
+}
+__device__ __forceinline__ uint32_t nnf_max3_u16x2(uint32_t a, uint32_t b, uint32_t c)
+{
+#ifdef MCL3DL_HOSTSIM
+  uint32_t r = 0;
+  for (int h = 0; h < 32; h += 16)
+    r |= std::max(std::max((a >> h) & 0xffffu, (b >> h) & 0xffffu), (c >> h) & 0xffffu) << h;
+  return r;
+#else
+  return __vimax3_u16x2(a, b, c);
+#endif
+}
+__device__ __forceinline__ int nnf_clz(uint32_t w)
+{
+#ifdef MCL3DL_HOSTSIM
+  return w == 0u ? 32 : __builtin_clz(w);
+#else
+  return __clz(static_cast<int>(w));
+#endif
+}
+
+// where the list marks its ordinal (relative to lo), or -1 when it has no slot in the pass
+__device__ __forceinline__ int nnf_owner_mark(int lo, int hi, int base, int count)
+{
+  const int s = max(base, lo);
+  return s < min(base + count, hi) ? s - lo : -1;  // (count <= 0: never)
+}
+
+// the largest mark among 16 consecutive table bytes (a lane's share of the scan).  Marks grow with the slot, so it is the
+// last non-zero byte: the highest non-zero byte of the last non-zero word.
+__device__ __forceinline__ uint32_t nnf_owner_run_max(uint4 r)
+{
+  uint32_t w = r.x;
+  w = r.y ? r.y : w;
+  w = r.z ? r.z : w;
+  w = r.w ? r.w : w;
+  return w >> ((31 - nnf_clz(w)) & 24);  // w = 0: the shift is 24, and 0 stays 0
+}
+
+// inclusive prefix maximum of the 4 bytes of w, in slot order (low byte first), seeded with `run`, the running maximum of
+// the slots before w in both 16-bit halves; returns the bytes and leaves the last one in both halves of `run`.  The
+// bytes are widened to 16-bit pairs for the hardware 16x2 three-way maximum, one instruction per pair.
+__device__ __forceinline__ uint32_t nnf_owner_scan_word(uint32_t w, uint32_t& run)
+{
+  uint32_t a = nnf_prmt(w, 0u, 0x4140u);  // slots 0, 1
+  a = nnf_max3_u16x2(a, a << 16, run);
+  uint32_t b = nnf_prmt(w, 0u, 0x4342u);  // slots 2, 3
+  b = nnf_max3_u16x2(b, b << 16, nnf_prmt(a, 0u, 0x3232u));
+  run = nnf_prmt(b, 0u, 0x3232u);
+  return nnf_prmt(a, b, 0x6420u);
+}
+
+// ordinals o = lane * U + u back to evals e = u * 32 + lane, in each byte of w (U = 1 << u_shift, 32 * U <= 256)
+__device__ __forceinline__ uint32_t nnf_owner_evals(uint32_t w, int u_shift)
+{
+  return ((w >> u_shift) & 0x1f1f1f1fu) | ((w << 5) & (((1u << u_shift) - 1u) * 0x20202020u));
 }
 
 // flann::L2_Simple of one candidate: sequential float accumulate of squared differences

@@ -473,6 +473,8 @@ __global__ void __launch_bounds__(kBlockThreads, 4)
 constexpr int kNfU = MCL3DL_NF_U;
 constexpr int kNfEvals = 32 * kNfU;  // evals of one warp per trip; eval e = u * 32 + lane
 static_assert(kNfEvals <= 256, "phase B names an eval by one byte");
+constexpr int kNfUShift = kNfU == 1 ? 0 : kNfU == 2 ? 1 : kNfU == 4 ? 2 : 3;
+static_assert((1 << kNfUShift) == kNfU, "the owner table turns ordinals into evals by shifts: kNfU is a power of two");
 // phase B: candidate loads in flight per lane, and (eval, candidate) slots per pass (longer flattened lists take passes)
 #ifndef MCL3DL_NF_B
 #define MCL3DL_NF_B 4
@@ -547,12 +549,45 @@ __device__ __forceinline__ void nf_warp_scan(NfWarpSmem& ws, const NnGridDev& g,
     ws.q[u * 32 + lane].w = __uint_as_float(s[u] - static_cast<uint32_t>(b[u]));  // slot + .w = candidate index
     ws.best[u * 32 + lane] = __float_as_uint(lp.r2);
   }
-  // ---- phase B: kNfB candidates per lane in flight, folded into their evals' bests
+  // ---- phase B, pass by pass: the owner table, then kNfB candidates per lane in flight, folded into their evals' bests
+  uint4* own4 = reinterpret_cast<uint4*>(ws.own);
+  const int o0 = lane * kNfU;  // ordinal of this lane's list u = 0
   for (int lo = 0; lo < W; lo += kNfSlots)
   {
     const int hi = min(W, lo + kNfSlots);
+    // owner table (device_funcs.cuh: nnf_owner_mark): clear the pass's bytes, mark each list's first slot in the pass
+    // with its ordinal, and max-scan the marks in rounds of 512 bytes, lane L taking bytes 16 L .. 16 L + 15 of a round
+    for (int i = lane; i * 16 < hi - lo; i += 32) own4[i] = make_uint4(0u, 0u, 0u, 0u);
+    __syncwarp();
 #pragma unroll
-    for (int u = 0; u < kNfU; ++u) nnf_fill_owner(ws.own, lo, hi, b[u], max(c[u], 0), u * 32 + lane);
+    for (int u = 0; u < kNfU; ++u)
+    {
+      const int m = nnf_owner_mark(lo, hi, b[u], c[u]);
+      if (m >= 0)
+        ws.own[m] = static_cast<uint8_t>(o0 + u);
+    }
+    __syncwarp();
+    uint32_t carry = 0;  // the largest mark of the rounds before
+    for (int r0 = 0; r0 * 16 < hi - lo; r0 += 32)
+    {
+      const int i = r0 + lane;
+      const bool in = i * 16 < hi - lo;
+      uint4 r = in ? own4[i] : make_uint4(0u, 0u, 0u, 0u);
+      uint32_t incl = max(nnf_owner_run_max(r), carry);
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) incl = max(incl, __shfl_up_sync(0xffffffffu, incl, o));
+      uint32_t run = __shfl_up_sync(0xffffffffu, incl, 1);
+      if (lane == 0)
+        run = carry;
+      carry = __shfl_sync(0xffffffffu, incl, 31);
+      run *= 0x00010001u;
+      r.x = nnf_owner_evals(nnf_owner_scan_word(r.x, run), kNfUShift);
+      r.y = nnf_owner_evals(nnf_owner_scan_word(r.y, run), kNfUShift);
+      r.z = nnf_owner_evals(nnf_owner_scan_word(r.z, run), kNfUShift);
+      r.w = nnf_owner_evals(nnf_owner_scan_word(r.w, run), kNfUShift);
+      if (in)
+        own4[i] = r;
+    }
     __syncwarp();
     if (CUT == 4)
     {

@@ -131,8 +131,9 @@ def table(res, names):
 
 def counts():
     """Per warp trip of lik_kernel_nf_pm over the 32 c2 stations (32 consecutive particles x UNIT consecutive points):
-    W (flattened slots), the longest list per u, the owner-fill iterations (sum over u of the longest list) and the
-    phase-B rounds (ceil(W / (32 * LOADS)))."""
+    W (flattened slots), the longest list per u, the iterations the serial owner fill took (sum over u of the longest
+    list), the owner table's marks, words and scan rounds, the phase-B rounds (ceil(W / (32 * LOADS))) and the share of
+    evals without candidates."""
     tmp = tempfile.mkdtemp()
     so = os.path.join(tmp, "liblikpmcounts.so")
     r = subprocess.run(["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-fPIC", "-shared", "-o", so,
@@ -146,7 +147,7 @@ def counts():
     stations = bench.build_stations("c2", 0, 1, s, 32)
     lik = engine.LikParams(dist_weight=bench.DIST_WEIGHT)
     mp = np.ascontiguousarray(s["map"], dtype=synth.POINT)
-    W, longest, fill, rounds, ovf = [], [], [], [], 0
+    W, longest, fill, rounds, marks, ovf, zero, evals = [], [], [], [], [], 0, 0, 0
     for st in stations:
         poses = np.ascontiguousarray(st["particles"], dtype=synth.POSE)
         pts = np.ascontiguousarray(st["lik"], dtype=synth.POINT)
@@ -156,6 +157,8 @@ def counts():
                              n, cnt.ctypes.data)
         assert rc == 0
         ovf += int((cnt < 0).sum())
+        zero += int((cnt == 0).sum())
+        evals += cnt.size
         c = np.maximum(cnt, 0)
         n_pad = -(-n // UNIT) * UNIT
         c = np.pad(c, ((0, 0), (0, n_pad - n)))
@@ -166,14 +169,19 @@ def counts():
         longest.append(mx.reshape(-1, UNIT))
         fill.append(mx.sum(axis=2).ravel())
         rounds.append(-(-w // (32 * LOADS)))
-    W, longest, fill, rounds = (np.concatenate(x) for x in (W, longest, fill, rounds))
+        marks.append((trips > 0).sum(axis=(1, 3)).ravel())
+    W, longest, fill, rounds, marks = (np.concatenate(x) for x in (W, longest, fill, rounds, marks))
 
     def stat(x):
         return {"mean": round(float(x.mean()), 2), "p50": float(np.median(x)), "p90": float(np.quantile(x, 0.9)),
                 "max": int(x.max())}
+    # the owner table (kernels.cuh: nf_warp_scan) of a trip's one pass: the marks (lists with candidates), the 32-bit
+    # words that hold it, and its scan rounds of 32 lanes x 16 bytes
     return {"warp_trips": int(len(W)), "W_slots": stat(W), "longest_list_per_u": stat(longest),
-            "owner_fill_iterations": stat(fill), "phase_b_rounds": stat(rounds),
-            "trips_over_1024_slots": int((W > 1024).sum()), "overflow_evals": ovf}
+            "owner_fill_iterations": stat(fill), "owner_table_marks": stat(marks),
+            "owner_table_words": stat(-(-W // 4)), "owner_scan_rounds": stat(-(-W // 512)),
+            "phase_b_rounds": stat(rounds), "trips_over_1024_slots": int((W > 1024).sum()),
+            "evals_without_candidates": round(zero / max(evals, 1), 4), "overflow_evals": ovf}
 
 
 def main():
