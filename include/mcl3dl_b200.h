@@ -145,6 +145,29 @@ void mcl3dl_destroy(mcl3dl_engine*);
 int mcl3dl_set_map(mcl3dl_engine*, const mcl3dl_point* pts, size_t n, uint64_t stamp,
                    const mcl3dl_lik_params* lik, const mcl3dl_beam_params* beam);
 
+typedef struct
+{
+  uint64_t n_before, n_appended, n_after;
+  int32_t incremental;       /* 1: lattices unchanged, only reached NN-field cells re-selected; 0: full device rebuild */
+  uint64_t cells_reselected; /* NN-field directory cells re-selected (all of them on the full path) */
+  double build_ms;           /* device time of this append (max over devices) */
+} mcl3dl_map_append_info;
+
+/* The node's map update (cbMapUpdateTimer, src/mcl_3dl.cpp:1350-1378): pc_map2_ = pc_map_ + pc_update_ into the cloud
+ * the index already holds, so every update appends to the staged map and nothing is removed or reordered.  After the
+ * call the staged map is the previous map followed by pts[0..n) and `stamp` is its stamp; every later call gives the
+ * records of a fresh engine that ran mcl3dl_set_map on the concatenated array.  The staged points stay on every device,
+ * so only the n new points are uploaded.  When they lie inside the staged map's raw and rescaled bounding boxes every
+ * lattice is unchanged: the grids are re-sorted on the device and the NN field re-selects only the directory cells the
+ * new points can reach (incremental == 1; their new lists go after the live ones, the old ones become dead space).
+ * Otherwise, or when the NN field's storage or MCL3DL_NNF_MAX_MB leaves no room, the map is rebuilt on the device from
+ * the resident points (incremental == 0), which also compacts the field.
+ * The resident particle set, the prepared scans, the exchange buffers and the scalar params are untouched; in field mode
+ * the volume is restaged.  n == 0 only sets the stamp (incremental == 1, no cell re-selected).
+ * NO_MAP before set_map; INVALID_ARG for a NULL engine or pts == NULL with n > 0; TOO_LARGE when the map would reach
+ * 2^31 points (all checked before pts is read).  info may be NULL. */
+int mcl3dl_map_append(mcl3dl_engine*, const mcl3dl_point* pts, size_t n, uint64_t stamp, mcl3dl_map_append_info* info);
+
 /* Scalar parameters may change between updates without restaging the map
  * (refreshParameters(), lidar_measurement_model_likelihood.cpp:56-61 / _beam.cpp:58-80), as long as
  * match_dist_min, dist_weight and dda_grid_size are unchanged; otherwise returns INVALID_ARG. */
@@ -388,7 +411,8 @@ int mcl3dl_near_field_info(const mcl3dl_engine*, int32_t k_out[2], uint64_t byte
 
 /* The NN field staged by the last set_map (exact per-voxel candidate lists, the default likelihood search structure;
  * no reference counterpart — ChunkedKdtree::radiusSearch, chunked_kdtree.h:218-251, descends a kd-tree per query):
- * out[0] = bytes per device (0: not staged, the CSR-window kernels serve the searches), out[1] = candidates stored,
+ * out[0] = bytes per device (0: not staged, the CSR-window kernels serve the searches; after mcl3dl_map_append the
+ * allocation, dead lists included), out[1] = candidates stored (live ones: those a fresh build stores),
  * out[2] = directory cells that overflowed (a voxel with more than 40 candidates: queries there fall back to the CSR
  * window search), out[3] = fine voxel edge in micrometres of the rescaled space, out[4] = wide cells (a voxel with 15..40
  * candidates: counts in a side table, one more dependent load).  A voxel-filtered map has neither kind.

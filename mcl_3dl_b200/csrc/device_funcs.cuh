@@ -868,6 +868,21 @@ __device__ __forceinline__ bool nnf_dominates(const NnfPt& a, const NnfPt& p, do
   return fmin_ > 1e-5 * nnf_max2(p, h) + 1e-12;
 }
 
+// One axis of fine voxel v's selection window: the CSR cells [lo, hi] that nnf_select reads (fo: the field's origin on the
+// axis; go / inv_cell / n: the grid's).  lo and hi are non-decreasing in v.
+__device__ __forceinline__ void nnf_window_axis(const NnFieldDev& f, float fo, int v, float go, float inv_cell, int n, int& lo,
+                                                int& hi)
+{
+  const double e = static_cast<double>(f.e);
+  const double c = static_cast<double>(fo) + (static_cast<double>(v) + 0.5) * e;
+  const double h = 0.5 * e + static_cast<double>(f.pad);
+  const double reach = static_cast<double>(f.radius) * 1.00001 + 1e-7;
+  const float w = static_cast<float>(h + reach) * 1.001f + 1e-5f;
+  const float fc = static_cast<float>(c);
+  lo = max(__float2int_rd(fmul(fsub(fsub(fc, w), go), inv_cell)), 0);
+  hi = min(__float2int_rd(fmul(fsub(fadd(fc, w), go), inv_cell)), n - 1);
+}
+
 __device__ __forceinline__ int nnf_select(const NnGridDev& g, const NnFieldDev& f, int vx, int vy, int vz, uint32_t* out)
 {
   // voxel centre and padded half edge; search reach = radius (already padded by the caller's 1.0001 factor) + pad
@@ -879,14 +894,10 @@ __device__ __forceinline__ int nnf_select(const NnGridDev& g, const NnFieldDev& 
   const double reach = static_cast<double>(f.radius) * 1.00001 + 1e-7;
   const double r2 = reach * reach;
   // CSR cells that can hold such points: the same (monotone) float cell function as the build, on widened float bounds
-  const float w = static_cast<float>(h + reach) * 1.001f + 1e-5f;
-  const float fx = static_cast<float>(cx), fy = static_cast<float>(cy), fz = static_cast<float>(cz);
-  const int lx = max(__float2int_rd(fmul(fsub(fsub(fx, w), g.ox), g.inv_cell)), 0);
-  const int ly = max(__float2int_rd(fmul(fsub(fsub(fy, w), g.oy), g.inv_cell)), 0);
-  const int lz = max(__float2int_rd(fmul(fsub(fsub(fz, w), g.oz), g.inv_cell)), 0);
-  const int hx = min(__float2int_rd(fmul(fsub(fadd(fx, w), g.ox), g.inv_cell)), g.nx - 1);
-  const int hy = min(__float2int_rd(fmul(fsub(fadd(fy, w), g.oy), g.inv_cell)), g.ny - 1);
-  const int hz = min(__float2int_rd(fmul(fsub(fadd(fz, w), g.oz), g.inv_cell)), g.nz - 1);
+  int lx, ly, lz, hx, hy, hz;
+  nnf_window_axis(f, f.ox, vx, g.ox, g.inv_cell, g.nx, lx, hx);
+  nnf_window_axis(f, f.oy, vy, g.oy, g.inv_cell, g.ny, ly, hy);
+  nnf_window_axis(f, f.oz, vz, g.oz, g.inv_cell, g.nz, lz, hz);
   if (lx > hx || ly > hy || lz > hz)
     return 0;
   // pass 1: the anchor = the in-reach point whose farthest corner is nearest (it bounds the NN distance of every query)
@@ -968,6 +979,51 @@ __device__ __forceinline__ int nnf_select(const NnGridDev& g, const NnFieldDev& 
     out[n_out++] = surv_s[i];
   }
   return n_out;
+}
+
+// NN field after an append (engine.cu: update_nn_field).  The directory cells whose selection can change because of one
+// appended map point p (raw coordinates): every cell with a fine voxel whose nnf_select window holds p's CSR cell.  A
+// voxel's selection reads only the points of the CSR cells in its window, in CSR order, so a cell that no appended point
+// marks selects exactly what it selected before.  Per axis the voxels whose window holds the cell form an interval (the
+// window bounds are non-decreasing in the voxel index); it is found by evaluating nnf_window_axis itself over a slightly
+// wider range.  Calls mark(directory cell) once per marked cell.
+template <class Mark>
+__device__ __forceinline__ void nnf_mark_append(const NnGridDev& g, const NnFieldDev& f, float px, float py, float pz, Mark&& mark)
+{
+  const float s[3] = {fmul(px, g.wx), fmul(py, g.wy), fmul(pz, g.wz)};
+  const float go[3] = {g.ox, g.oy, g.oz}, fo[3] = {f.ox, f.oy, f.oz};
+  const int gn[3] = {g.nx, g.ny, g.nz}, fn[3] = {f.nx, f.ny, f.nz};
+  const double cell = 1.0 / static_cast<double>(g.inv_cell);
+  const double w = static_cast<double>(static_cast<float>(0.5 * f.e + f.pad + f.radius * 1.00001 + 1e-7) * 1.001f + 1e-5f);
+  int c0[3], c1[3];
+  for (int a = 0; a < 3; ++a)
+  {
+    // nn_key_kernel's cell of the point
+    const int c = min(max(__float2int_rd(fmul(fsub(s[a], go[a]), g.inv_cell)), 0), gn[a] - 1);
+    const double lo_edge = static_cast<double>(go[a]) + c * cell, hi_edge = lo_edge + cell;
+    const int v_from = max(static_cast<int>(floor((lo_edge - w - fo[a]) / f.e)) - 3, 0);
+    const int v_to = min(static_cast<int>(floor((hi_edge + w - fo[a]) / f.e)) + 3, fn[a] - 1);
+    int first = -1, last = -2;
+    for (int v = v_from; v <= v_to; ++v)
+    {
+      int lo, hi;
+      nnf_window_axis(f, fo[a], v, go[a], g.inv_cell, gn[a], lo, hi);
+      if (lo <= c && c <= hi)
+      {
+        if (first < 0)
+          first = v;
+        last = v;
+      }
+    }
+    if (first < 0)
+      return;
+    c0[a] = first >> 1;
+    c1[a] = last >> 1;
+  }
+  for (int cz = c0[2]; cz <= c1[2]; ++cz)
+    for (int cy = c0[1]; cy <= c1[1]; ++cy)
+      for (int cx = c0[0]; cx <= c1[0]; ++cx)
+        mark((static_cast<size_t>(cz) * f.cny + cy) * f.cnx + cx);
 }
 
 // One ray with RaycastUsingKDTree (raycasts/raycast_using_kdtree.h:57-110) + getBeamStatus (beam.cpp:157-192), cut into

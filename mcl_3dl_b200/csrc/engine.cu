@@ -156,13 +156,16 @@ __global__ void near_mark_kernel(const mcl3dl_point* __restrict__ pts, uint32_t 
 // lanes.  Pass 1 counts the candidates (nibbles + per-cell totals); after an exclusive scan of the totals pass 2 repeats
 // the selection and stores the candidates.  `bits` is the field's own k = 2 near field: a clear bit proves that no map
 // point is within the radius of any query that maps to the voxel, so the (costly) selection only runs near surfaces.
-__device__ __forceinline__ bool nnf_voxel_of_thread(const NnFieldDev& f, size_t n_cells, size_t t, size_t& cell, int& sub, int& vx,
-                                                    int& vy, int& vz)
+// With `list` (after an append, update_nn_field) the threads cover the listed directory cells only: item i is cell
+// list[i], and the per-item arrays (totals, base) are indexed by i; without it, item i is cell i.
+__device__ __forceinline__ bool nnf_voxel_of_thread(const NnFieldDev& f, const uint32_t* list, size_t n_items, size_t t,
+                                                    size_t& item, size_t& cell, int& sub, int& vx, int& vy, int& vz)
 {
-  cell = t >> 3;
+  item = t >> 3;
   sub = static_cast<int>(t & 7);
-  if (cell >= n_cells)
+  if (item >= n_items)
     return false;
+  cell = list ? list[item] : item;
   const int cx = static_cast<int>(cell % f.cnx);
   const size_t r = cell / f.cnx;
   const int cy = static_cast<int>(r % f.cny), cz = static_cast<int>(r / f.cny);
@@ -174,13 +177,15 @@ __device__ __forceinline__ bool nnf_voxel_of_thread(const NnFieldDev& f, size_t 
 
 __global__ void __launch_bounds__(256)
     nnf_count_kernel(NnGridDev g, NnFieldDev f, const uint32_t* __restrict__ bits, int pitch, uint2* __restrict__ dir,
-                     uint32_t* __restrict__ totals, size_t n_cells, uint4* __restrict__ wide, uint32_t wide_cap,
-                     uint32_t* __restrict__ counters /* [0] wide cells used, [1] overflow cells */)
+                     uint32_t* __restrict__ totals, const uint32_t* __restrict__ list, size_t n_items, uint4* __restrict__ wide,
+                     uint32_t wide_cap,
+                     uint32_t* __restrict__ counters /* [0] wide cells used, [1] overflow cells; with a list also the
+                                                         listed cells' old [2] candidates, [3] overflow and [4] wide cells */)
 {
   const size_t t = blockIdx.x * static_cast<size_t>(256) + threadIdx.x;
-  size_t cell;
+  size_t item, cell = 0;
   int sub, vx, vy, vz, cnt = 0;
-  if (nnf_voxel_of_thread(f, n_cells, t, cell, sub, vx, vy, vz) &&
+  if (nnf_voxel_of_thread(f, list, n_items, t, item, cell, sub, vx, vy, vz) &&
       ((__ldg(bits + (static_cast<size_t>(vz) * f.ny + vy) * pitch + (vx >> 5)) >> (vx & 31)) & 1u))
   {
     uint32_t tmp[kNnfMaxSurv];
@@ -200,8 +205,23 @@ __global__ void __launch_bounds__(256)
     ovf |= __shfl_xor_sync(0xffffffffu, ovf, o);
     big |= __shfl_xor_sync(0xffffffffu, big, o);
   }
-  if (sub != 0 || cell >= n_cells)
+  if (sub != 0 || item >= n_items)
     return;
+  if (list)
+  {
+    // what the cell held before its re-selection (its old list becomes dead space)
+    const uint2 d = dir[cell];
+    if (d.x == 0xffffffffu)
+      atomicAdd(counters + 3, 1u);
+    else
+    {
+      uint32_t old = 0, start;
+      for (int k = 0; k < 8; ++k) old += static_cast<uint32_t>(max(nnf_slot(f, d, k, start), 0));
+      atomicAdd(counters + 2, old);
+      if (d.x & 0x80000000u)
+        atomicAdd(counters + 4, 1u);
+    }
+  }
   // dir[cell].y: nibbles | 0xfffffffe = wide cell (dir[cell].x already holds 0x80000000 | index) | 0xffffffff = overflow
   if (!ovf && big)
   {
@@ -210,7 +230,7 @@ __global__ void __launch_bounds__(256)
     {
       wide[idx] = make_uint4(0u, lo, hi, 0u);  // x = first candidate, filled in by nnf_base_kernel
       dir[cell] = make_uint2(0x80000000u | idx, 0xfffffffeu);
-      totals[cell] = tot;
+      totals[item] = tot;
       return;
     }
     ovf = 1u;  // side table full: treat as an overflow cell
@@ -218,7 +238,7 @@ __global__ void __launch_bounds__(256)
   if (ovf)
   {
     dir[cell].y = 0xffffffffu;
-    totals[cell] = 0u;
+    totals[item] = 0u;
     atomicAdd(counters + 1, 1u);
     return;
   }
@@ -226,7 +246,7 @@ __global__ void __launch_bounds__(256)
 #pragma unroll
   for (int k = 0; k < 4; ++k) nib |= (((lo >> (8 * k)) & 15u) << (4 * k)) | (((hi >> (8 * k)) & 15u) << (4 * (k + 4)));
   dir[cell].y = nib;
-  totals[cell] = tot;
+  totals[item] = tot;
 }
 
 struct WidenU32
@@ -234,28 +254,32 @@ struct WidenU32
   __host__ __device__ unsigned long long operator()(uint32_t v) const { return v; }
 };
 
-__global__ void nnf_base_kernel(uint2* __restrict__ dir, const uint32_t* __restrict__ base, size_t n_cells, uint4* __restrict__ wide)
+// First candidate of every (listed) cell: the exclusive scan of the totals, plus `offset` (after an append: the end of
+// the candidates already placed).
+__global__ void nnf_base_kernel(uint2* __restrict__ dir, const uint32_t* __restrict__ base, uint32_t offset,
+                                const uint32_t* __restrict__ list, size_t n_items, uint4* __restrict__ wide)
 {
-  const size_t c = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
-  if (c >= n_cells)
+  const size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;
+  if (i >= n_items)
     return;
+  const size_t c = list ? list[i] : i;
   const uint32_t y = dir[c].y;
   if (y == 0xffffffffu)
     dir[c].x = 0xffffffffu;
   else if (y == 0xfffffffeu)
-    wide[dir[c].x & 0x7fffffffu].x = base[c];
+    wide[dir[c].x & 0x7fffffffu].x = base[i] + offset;
   else
-    dir[c].x = base[c];
+    dir[c].x = base[i] + offset;
 }
 
 __global__ void __launch_bounds__(256)
     nnf_fill_kernel(NnGridDev g, NnFieldDev f, const uint32_t* __restrict__ bits, int pitch, const uint2* __restrict__ dir,
-                    float4* __restrict__ cand, size_t n_cells)
+                    float4* __restrict__ cand, const uint32_t* __restrict__ list, size_t n_items)
 {
   const size_t t = blockIdx.x * static_cast<size_t>(256) + threadIdx.x;
-  size_t cell;
+  size_t item, cell;
   int sub, vx, vy, vz;
-  if (!nnf_voxel_of_thread(f, n_cells, t, cell, sub, vx, vy, vz))
+  if (!nnf_voxel_of_thread(f, list, n_items, t, item, cell, sub, vx, vy, vz))
     return;
   uint32_t start = 0;
   const int want = nnf_slot(f, dir[cell], sub, start);
@@ -264,6 +288,25 @@ __global__ void __launch_bounds__(256)
   uint32_t pos[kNnfMaxSurv];
   const int cnt = nnf_select(g, f, vx, vy, vz, pos);
   for (int i = 0; i < cnt && i < want; ++i) cand[start + i] = g.pts[pos[i]];
+}
+
+// After an append: the directory cells the appended points pts[0..n) reach (device_funcs.cuh: nnf_mark_append), each
+// listed once; count > cap tells the host that the list did not fit.
+__global__ void nnf_mark_kernel(const mcl3dl_point* __restrict__ pts, uint32_t n, NnGridDev g, NnFieldDev f,
+                                uint32_t* __restrict__ marks, uint32_t* __restrict__ list, uint32_t cap, uint32_t* __restrict__ count)
+{
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n)
+    return;
+  const float4 p = __ldg(reinterpret_cast<const float4*>(pts) + i);
+  nnf_mark_append(g, f, p.x, p.y, p.z, [&](size_t cell) {
+    const uint32_t bit = 1u << (cell & 31);
+    if (atomicOr(marks + (cell >> 5), bit) & bit)
+      return;
+    const uint32_t k = atomicAdd(count, 1u);
+    if (k < cap)
+      list[k] = static_cast<uint32_t>(cell);
+  });
 }
 
 // Field mode (device_funcs.cuh: FieldDev).  Node volume: exact distance (clamped) from every lattice node to the
@@ -424,6 +467,10 @@ struct DeviceCtx
   DevBuf raw_pts;  // map points in original order (with a likelihood grid: KD-tree raycaster, matched / unmatched output)
   DevBuf near_lik, near_kd;  // near-field bits (MCL3DL_NEAR_BITS builds)
   DevBuf nnf_dir, nnf_cand, nnf_wide;  // NN field: directory, candidate lists, side table of the wide cells
+  // NN field storage: candidates / wide entries placed so far (after appends: live and dead ones), wide-table capacity
+  size_t nnf_cand_used = 0;
+  uint32_t nnf_wide_used = 0, nnf_wide_cap = 0;
+  uint32_t map_box[12] = {};  // bounding boxes of the staged map (bbox_kernel's encoding)
   DevBuf fld_cells;          // field mode: 8 corner distances per lattice cell
   DevBuf fld_mem;              // field mode: node volume (cudaMalloc3D), the owner of fld_nodes.ptr
   cudaPitchedPtr fld_nodes{};
@@ -966,8 +1013,10 @@ void fill_kd_scalars(const mcl3dl_beam_params& b, KdRayDev& k)
 #if MCL3DL_NEAR_BITS
 // Near field for search radius r over the rescaled map points (device_funcs.cuh: NearBitsDev).  k == 0, or a box that
 // cannot be laid out within the byte cap, leaves `out.bits` null (the searches then run unscreened).
-int build_near_field(mcl3dl_engine* eng, DeviceCtx& c, cudaStream_t st, const mcl3dl_point* pts, uint32_t n, float wx,
-                     float wy, float wz, float r, int k, const float sc_min[3], const float sc_max[3], DevBuf& buf,
+// first > 0: the bits of points [0, first) are already in `buf`, laid out for the same box (an append): only the rest are
+// added (a bit is an OR over points).
+int build_near_field(mcl3dl_engine* eng, DeviceCtx& c, cudaStream_t st, const mcl3dl_point* pts, uint32_t n, uint32_t first,
+                     float wx, float wy, float wz, float r, int k, const float sc_min[3], const float sc_max[3], DevBuf& buf,
                      NearBitsDev& out, int slot)
 {
   out = NearBitsDev{};
@@ -980,8 +1029,9 @@ int build_near_field(mcl3dl_engine* eng, DeviceCtx& c, cudaStream_t st, const mc
   int rc = reserve(eng, buf, bytes);
   if (rc != MCL3DL_OK)
     return rc;
-  CK(cudaMemsetAsync(buf.p, 0, bytes, st));
-  near_mark_kernel<<<(n + 255) / 256, 256, 0, st>>>(pts, n, wx, wy, wz, f, static_cast<uint32_t*>(buf.p), k);
+  if (first == 0)
+    CK(cudaMemsetAsync(buf.p, 0, bytes, st));
+  near_mark_kernel<<<(n - first + 255) / 256, 256, 0, st>>>(pts + first, n - first, wx, wy, wz, f, static_cast<uint32_t*>(buf.p), k);
   CK(cudaGetLastError());
   eng->launches++;
   f.bits = static_cast<const uint32_t*>(buf.p);
@@ -1037,7 +1087,7 @@ int build_nn_field(mcl3dl_engine* eng, DeviceCtx& c, cudaStream_t st, const mcl3
   uint32_t* tot = static_cast<uint32_t*>(d_tot.p);
   CK(cudaMemsetAsync(tot + n_cells, 0, 16, st));  // [n_cells]: scan tail, [n_cells + 2] wide cells, [n_cells + 3] overflow cells
   f.wide = static_cast<const uint4*>(c.nnf_wide.p);
-  nnf_count_kernel<<<blocks, 256, 0, st>>>(g, f, static_cast<const uint32_t*>(d_bits.p), lay.pitch, dir, tot, n_cells,
+  nnf_count_kernel<<<blocks, 256, 0, st>>>(g, f, static_cast<const uint32_t*>(d_bits.p), lay.pitch, dir, tot, nullptr, n_cells,
                                            static_cast<uint4*>(c.nnf_wide.p), wide_cap, tot + n_cells + 2);
   CK(cudaGetLastError());
   // exclusive scan of the per-cell totals (in place); the grand total sizes the candidate array.  A candidate index
@@ -1077,9 +1127,10 @@ int build_nn_field(mcl3dl_engine* eng, DeviceCtx& c, cudaStream_t st, const mcl3
   }
   if ((rc = reserve(eng, c.nnf_cand, std::max<size_t>(cand_bytes, 16))))
     return rc;
-  nnf_base_kernel<<<static_cast<unsigned>((n_cells + 255) / 256), 256, 0, st>>>(dir, tot, n_cells, static_cast<uint4*>(c.nnf_wide.p));
+  nnf_base_kernel<<<static_cast<unsigned>((n_cells + 255) / 256), 256, 0, st>>>(dir, tot, 0u, nullptr, n_cells,
+                                                                                 static_cast<uint4*>(c.nnf_wide.p));
   nnf_fill_kernel<<<blocks, 256, 0, st>>>(g, f, static_cast<const uint32_t*>(d_bits.p), lay.pitch, dir,
-                                          static_cast<float4*>(c.nnf_cand.p), n_cells);
+                                          static_cast<float4*>(c.nnf_cand.p), nullptr, n_cells);
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(st));
   eng->launches += 4;
@@ -1088,26 +1139,152 @@ int build_nn_field(mcl3dl_engine* eng, DeviceCtx& c, cudaStream_t st, const mcl3
   g.field = f;
   eng->nnf_bytes = n_cells * 8 + cand_bytes + static_cast<size_t>(wide_cap) * sizeof(uint4);
   eng->nnf_cands = total;
+  c.nnf_cand_used = total;
+  c.nnf_wide_used = std::min<uint32_t>(tail[2], wide_cap);
+  c.nnf_wide_cap = wide_cap;
   c.map_bytes += eng->nnf_bytes;
   return MCL3DL_OK;
 }
 
-// Build both grids on one device from the uploaded points.
-int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_point* h_pts, size_t n)
+// NN field after an append that left every lattice as it was (same boxes, same parameters), over the re-sorted CSR grid
+// g: only the directory cells an appended point pts[n_before..n) can reach are re-selected (nnf_mark_append), with the
+// count / base / fill kernels of the build over that list; their new lists go after the candidates already placed, their
+// new wide entries after the used ones.  The old lists become dead space.  The first append that needs room grows the
+// candidate array; done = false when the lists or the wide entries do not fit, or the cap (MCL3DL_NNF_MAX_MB) would be
+// exceeded: the caller then rebuilds the field, which compacts.
+int update_nn_field(mcl3dl_engine* eng, DeviceCtx& c, cudaStream_t st, const mcl3dl_point* pts, uint32_t n_before, uint32_t n,
+                    NnGridDev& g, const float sc_min[3], const float sc_max[3], bool& done, uint64_t& reselected)
+{
+  done = false;
+  NnFieldDev f = c.nn.field;  // lattice, pad and radius are those of the staged map
+  NearBitsDev lay{};
+  if (!f.dir || !near_layout(lay, f.radius, 2, sc_min, sc_max, size_t(1) << 40))
+    return MCL3DL_OK;
+  const size_t n_cells = static_cast<size_t>(f.cnx) * f.cny * f.cnz;
+  const uint32_t n_new = n - n_before;
+  // list capacity: the directory cells one point can mark, per axis (nnf_mark_append's voxel interval, halved, + 2)
+  const double w = static_cast<double>(static_cast<float>(0.5 * f.e + f.pad + f.radius * 1.00001 + 1e-7) * 1.001f + 1e-5f);
+  const size_t per_axis = static_cast<size_t>((1.0 / g.inv_cell + 2.0 * w) / f.e + 7.0) / 2 + 2;
+  const size_t list_cap = std::min(n_cells, static_cast<size_t>(n_new) * per_axis * per_axis * per_axis);
+  const size_t bits_bytes = static_cast<size_t>(lay.pitch) * lay.ny * lay.nz * 4;
+  const size_t mark_words = (n_cells + 31) / 32;
+  DevBuf d_bits, d_mark, d_list, d_tot, d_cnt, d_tmp;
+  int rc = MCL3DL_OK;
+  if ((rc = reserve(eng, d_bits, bits_bytes)) || (rc = reserve(eng, d_mark, mark_words * 4)) ||
+      (rc = reserve(eng, d_list, list_cap * 4)) || (rc = reserve(eng, d_tot, (list_cap + 1) * 4)) ||
+      (rc = reserve(eng, d_cnt, 8 * 4)))
+    return rc;
+  uint32_t* cnt = static_cast<uint32_t*>(d_cnt.p);  // [0..4] nnf_count_kernel's counters, [5] marked cells
+  uint32_t* list = static_cast<uint32_t*>(d_list.p);
+  uint32_t* tot = static_cast<uint32_t*>(d_tot.p);
+  // the field's k = 2 near field of the whole map, as the build makes it
+  CK(cudaMemsetAsync(d_bits.p, 0, bits_bytes, st));
+  near_mark_kernel<<<(n + 255) / 256, 256, 0, st>>>(pts, n, g.wx, g.wy, g.wz, lay, static_cast<uint32_t*>(d_bits.p), 2);
+  CK(cudaMemsetAsync(d_mark.p, 0, mark_words * 4, st));
+  const uint32_t init[8] = {c.nnf_wide_used, 0, 0, 0, 0, 0, 0, 0};
+  CK(cudaMemcpyAsync(cnt, init, sizeof(init), cudaMemcpyHostToDevice, st));
+  nnf_mark_kernel<<<(n_new + 255) / 256, 256, 0, st>>>(pts + n_before, n_new, g, f, static_cast<uint32_t*>(d_mark.p), list,
+                                                        static_cast<uint32_t>(list_cap), cnt + 5);
+  CK(cudaGetLastError());
+  uint32_t n_list = 0;
+  CK(cudaMemcpyAsync(&n_list, cnt + 5, 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  eng->launches += 2;
+  if (n_list > list_cap)
+    return MCL3DL_OK;
+  reselected = n_list;
+  if (n_list == 0)
+  {
+    g.field = f;
+    c.map_bytes += eng->nnf_bytes;
+    done = true;
+    return MCL3DL_OK;
+  }
+  uint2* dir = const_cast<uint2*>(f.dir);
+  CK(cudaMemsetAsync(tot + n_list, 0, 4, st));
+  const unsigned blocks = static_cast<unsigned>((static_cast<size_t>(n_list) * 8 + 255) / 256);
+  nnf_count_kernel<<<blocks, 256, 0, st>>>(g, f, static_cast<const uint32_t*>(d_bits.p), lay.pitch, dir, tot, list, n_list,
+                                           static_cast<uint4*>(c.nnf_wide.p), c.nnf_wide_cap, cnt);
+  CK(cudaGetLastError());
+  // at most 8 x 41 candidates per listed cell, fewer than 2^31 listed: the sum is taken in 64 bits
+  cub::TransformInputIterator<unsigned long long, WidenU32, const uint32_t*> wide_in(tot, WidenU32());
+  DevBuf d_sum;
+  if ((rc = reserve(eng, d_sum, 8)))
+    return rc;
+  unsigned long long* sum = static_cast<unsigned long long*>(d_sum.p);
+  size_t tmp_scan = 0, tmp_sum = 0;
+  CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp_scan, tot, tot, static_cast<int>(n_list + 1), st));
+  CK(cub::DeviceReduce::Sum(nullptr, tmp_sum, wide_in, sum, static_cast<int>(n_list), st));
+  if ((rc = reserve(eng, d_tmp, std::max(tmp_scan, tmp_sum))))
+    return rc;
+  tmp_sum = d_tmp.cap;
+  CK(cub::DeviceReduce::Sum(d_tmp.p, tmp_sum, wide_in, sum, static_cast<int>(n_list), st));
+  uint32_t h_cnt[5];
+  unsigned long long added = 0;
+  CK(cudaMemcpyAsync(h_cnt, cnt, sizeof(h_cnt), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(&added, sum, 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  const size_t need = c.nnf_cand_used + added;  // candidates placed once the new lists are in
+  const size_t live = eng->nnf_cands - h_cnt[2] + added;
+  if (h_cnt[0] > c.nnf_wide_cap || need >= (size_t(1) << 31))
+    return MCL3DL_OK;  // (the directory entries the count pass rewrote are rebuilt with the rest)
+  const size_t wide_bytes = static_cast<size_t>(c.nnf_wide_cap) * sizeof(uint4);
+  if (need * sizeof(float4) > c.nnf_cand.cap)
+  {
+    // grow once, with room for more appends; not while dead lists would outweigh the live ones (rebuild then)
+    const size_t cap = need + live / 4;
+    if (need - live > live || n_cells * 8 + cap * sizeof(float4) + wide_bytes > eng->nnf_max_bytes)
+      return MCL3DL_OK;
+    DevBuf grown;
+    if ((rc = reserve(eng, grown, cap * sizeof(float4))))
+      return rc;
+    CK(cudaMemcpyAsync(grown.p, c.nnf_cand.p, c.nnf_cand_used * sizeof(float4), cudaMemcpyDeviceToDevice, st));
+    c.nnf_cand = std::move(grown);
+    eng->nnf_bytes = n_cells * 8 + cap * sizeof(float4) + wide_bytes;
+  }
+  size_t tsz = d_tmp.cap;
+  CK(cub::DeviceScan::ExclusiveSum(d_tmp.p, tsz, tot, tot, static_cast<int>(n_list + 1), st));
+  f.cand = static_cast<const float4*>(c.nnf_cand.p);
+  nnf_base_kernel<<<(n_list + 255) / 256, 256, 0, st>>>(dir, tot, static_cast<uint32_t>(c.nnf_cand_used), list, n_list,
+                                                        static_cast<uint4*>(c.nnf_wide.p));
+  nnf_fill_kernel<<<blocks, 256, 0, st>>>(g, f, static_cast<const uint32_t*>(d_bits.p), lay.pitch, dir,
+                                          static_cast<float4*>(c.nnf_cand.p), list, n_list);
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(st));
+  eng->launches += 4;
+  eng->nnf_cands = live;
+  eng->nnf_overflow_cells = eng->nnf_overflow_cells - h_cnt[3] + h_cnt[1];
+  eng->nnf_wide_cells = eng->nnf_wide_cells - h_cnt[4] + (h_cnt[0] - c.nnf_wide_used);
+  c.nnf_cand_used = need;
+  c.nnf_wide_used = h_cnt[0];
+  g.field = f;
+  c.map_bytes += eng->nnf_bytes;
+  done = true;
+  return MCL3DL_OK;
+}
+
+// Build both grids on one device from the map points in d_pts (device memory, map order, n points, written on c.stream).
+// On success the points become the context's raw_pts: the map stays on the device, so that mcl3dl_map_append uploads only
+// the appended points.
+//
+// n_before > 0: d_pts is the staged map followed by appended points.  When the appended points leave both bounding boxes
+// as they were, every lattice is unchanged: the grids are re-sorted, the near fields get the new points' bits and the NN
+// field re-selects only the cells the new points reach (update_nn_field); `reselected` counts its re-selected cells
+// (all of them on a full build) and `incremental` says which path ran.
+int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, DevBuf& d_pts, size_t n, size_t n_before, uint64_t& reselected,
+                        bool& incremental)
 {
   CK(cudaSetDevice(c.dev));
   cudaStream_t st = c.stream;
   cudaEvent_t e0 = c.ev[0], e1 = c.ev[1];  // build time: the per-update timing events, unused between calls
-  DevBuf d_pts, d_bbox, d_keys[2], d_vals[2], d_tmp;  // keys / values: [0] per point, [1] sorted by cell
+  DevBuf d_bbox, d_keys[2], d_vals[2], d_tmp;  // keys / values: [0] per point, [1] sorted by cell
   int rc = MCL3DL_OK;
   const uint32_t n32 = static_cast<uint32_t>(n);
   const int tb = 256;
   const int nb = static_cast<int>((n + tb - 1) / tb);
-  if ((rc = reserve(eng, d_pts, n * sizeof(mcl3dl_point))) || (rc = reserve(eng, d_bbox, 12 * sizeof(uint32_t))) ||
-      (rc = reserve(eng, d_keys[0], n * 4)) || (rc = reserve(eng, d_vals[0], n * 4)) || (rc = reserve(eng, d_keys[1], n * 4)) ||
-      (rc = reserve(eng, d_vals[1], n * 4)))
+  if ((rc = reserve(eng, d_bbox, 12 * sizeof(uint32_t))) || (rc = reserve(eng, d_keys[0], n * 4)) ||
+      (rc = reserve(eng, d_vals[0], n * 4)) || (rc = reserve(eng, d_keys[1], n * 4)) || (rc = reserve(eng, d_vals[1], n * 4)))
     return rc;
-  CK(cudaMemcpyAsync(d_pts.p, h_pts, n * sizeof(mcl3dl_point), cudaMemcpyHostToDevice, st));
   CK(cudaEventRecord(e0, st));
   const mcl3dl_point* pts = static_cast<const mcl3dl_point*>(d_pts.p);
   uint32_t* keys[2] = {static_cast<uint32_t*>(d_keys[0].p), static_cast<uint32_t*>(d_keys[1].p)};
@@ -1156,6 +1333,10 @@ int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_point* h_
     sc_min[k] = ord2f(h_bbox[6 + k]);
     sc_max[k] = ord2f(h_bbox[9 + k]);
   }
+  incremental = n_before > 0 && std::memcmp(h_bbox, c.map_box, sizeof(h_bbox)) == 0;
+  std::memcpy(c.map_box, h_bbox, sizeof(h_bbox));
+  const uint32_t first = incremental ? static_cast<uint32_t>(n_before) : 0u;  // near fields: bits of points [first, n)
+  reselected = 0;
   c.map_bytes = 0;
 
   // ---- likelihood search grid
@@ -1204,7 +1385,8 @@ int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_point* h_
     g.cell_start = cell_start;
     g.pts = static_cast<const float4*>(c.nn_pts.p);
 #if MCL3DL_NEAR_BITS
-    if ((rc = build_near_field(eng, c, st, pts, n32, wx, wy, wz, eng->likdev.rpad, eng->near_k, sc_min, sc_max, c.near_lik, g.near, 0)))
+    if ((rc = build_near_field(eng, c, st, pts, n32, first, wx, wy, wz, eng->likdev.rpad, eng->near_k, sc_min, sc_max, c.near_lik,
+                               g.near, 0)))
       return rc;
 #endif
     // NN field: exact for the likelihood radius and, with the KD-tree raycaster, for its marching radius as well
@@ -1219,8 +1401,21 @@ int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_point* h_
         radius = std::max(radius, eng->nnf_kd_r2 ? tmp.r2_pad : tmp.r1_pad);
       }
       g.field = NnFieldDev{};
-      if (eng->nnf && (rc = build_nn_field(eng, c, st, pts, n32, g, radius, sc_min, sc_max)))
+      bool done = false;
+      // (the field's radius follows the beam params, which set_params may have changed since the field was built)
+      if (incremental && eng->nnf && radius == c.nn.field.radius &&
+          (rc = update_nn_field(eng, c, st, pts, static_cast<uint32_t>(n_before), n32, g, sc_min, sc_max, done, reselected)))
         return rc;
+      if (!done)
+      {
+        incremental = false;
+        if (n_before > 0)
+          c.nnf_cand = DevBuf();  // the rebuild compacts: no dead lists, no room kept from earlier appends
+        if (eng->nnf && (rc = build_nn_field(eng, c, st, pts, n32, g, radius, sc_min, sc_max)))
+          return rc;
+        if (g.field.dir)
+          reselected = static_cast<uint64_t>(g.field.cnx) * g.field.cny * g.field.cnz;
+      }
     }
     // window table of the CSR-window kernel (lik_kernel_wi): only when the field is not staged
     size_t row3_total = 0;
@@ -1251,14 +1446,11 @@ int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_point* h_
     eng->info.nn_origin[2] = g.oz;
   }
   // ---- the raw points by original index (the KD-tree raycaster's colliding point; the chunk rule of
-  // mcl3dl_match_output): keep the upload wherever there is a likelihood grid
+  // mcl3dl_match_output; the base of mcl3dl_map_append).  device_bytes counts them where the models read them: with a
+  // likelihood grid.
+  c.raw_pts = std::move(d_pts);
   if (eng->has_lik)
-  {
-    c.raw_pts = std::move(d_pts);
     c.map_bytes += n * 16;
-  }
-  else
-    c.raw_pts = DevBuf();
 
   // ---- KD-tree raycaster: marches over the likelihood grid; needs the raw points by original index
   if (eng->has_beam && !eng->beam.use_raycast_using_dda)
@@ -1268,7 +1460,9 @@ int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_point* h_
     fill_dda_scalars(eng->beam, c.dda);
     fill_kd_scalars(eng->beam, c.kd);
 #if MCL3DL_NEAR_BITS
-    if ((rc = build_near_field(eng, c, st, pts, n32, wx, wy, wz, c.kd.r1_pad, eng->near_kd_k, sc_min, sc_max, c.near_kd, c.kd.near, 1)))
+    // (set_params may have widened the marching radius since the field was built: then it is built anew)
+    if ((rc = build_near_field(eng, c, st, pts, n32, c.near_kd_r == c.kd.r1_pad ? first : 0u, wx, wy, wz, c.kd.r1_pad,
+                               eng->near_kd_k, sc_min, sc_max, c.near_kd, c.kd.near, 1)))
       return rc;
     c.near_kd_r = c.kd.r1_pad;
 #endif
@@ -1335,6 +1529,15 @@ int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_point* h_
   eng->info.build_ms = std::max(eng->info.build_ms, static_cast<double>(ms));
   eng->info.device_bytes = c.map_bytes;
   return MCL3DL_OK;
+}
+
+// After a build: a field-mode volume of the previous map is stale; in field mode the new one is staged.
+int restage_field(mcl3dl_engine* eng, DeviceCtx& c)
+{
+  c.fld_nodes_valid = false;
+  c.fld_mem = DevBuf();
+  c.fld_nodes = cudaPitchedPtr{};
+  return eng->field_mode && eng->has_lik ? stage_field(eng, c, nullptr) : MCL3DL_OK;
 }
 }  // namespace
 
@@ -1531,18 +1734,75 @@ int mcl3dl_set_map(mcl3dl_engine* eng, const mcl3dl_point* pts, size_t n, uint64
   eng->info.n_points = n;
   for (DeviceCtx& c : eng->devs)
   {
-    int rc = build_map_on_device(eng, c, pts, n);
-    if (rc != MCL3DL_OK)
+    DevBuf d_pts;
+    int rc = MCL3DL_OK;
+    CK(cudaSetDevice(c.dev));
+    if ((rc = reserve(eng, d_pts, n * sizeof(mcl3dl_point))))
       return rc;
-    c.fld_nodes_valid = false;  // a volume of the previous map is stale
-    c.fld_mem = DevBuf();
-    c.fld_nodes = cudaPitchedPtr{};
-    if (eng->field_mode && eng->has_lik && (rc = stage_field(eng, c, nullptr)) != MCL3DL_OK)
+    CK(cudaMemcpyAsync(d_pts.p, pts, n * sizeof(mcl3dl_point), cudaMemcpyHostToDevice, c.stream));
+    uint64_t reselected = 0;
+    bool incremental = false;
+    if ((rc = build_map_on_device(eng, c, d_pts, n, 0, reselected, incremental)) || (rc = restage_field(eng, c)))
       return rc;
   }
   eng->has_map = true;
   eng->stamp = stamp;
   eng->n_points = n;
+  return MCL3DL_OK;
+}
+
+int mcl3dl_map_append(mcl3dl_engine* eng, const mcl3dl_point* pts, size_t n, uint64_t stamp, mcl3dl_map_append_info* info)
+{
+  if (!eng)
+    return MCL3DL_ERR_INVALID_ARG;
+  if (!eng->has_map)
+    return MCL3DL_ERR_NO_MAP;
+  if (!pts && n > 0)
+    return MCL3DL_ERR_INVALID_ARG;
+  const size_t n_before = eng->n_points;
+  if (n >= (size_t(1) << 31) || n_before + n >= (size_t(1) << 31))
+    return MCL3DL_ERR_TOO_LARGE;
+  mcl3dl_map_append_info r{};
+  r.n_before = n_before;
+  r.n_appended = n;
+  r.n_after = n_before + n;
+  r.incremental = 1;  // n == 0: only the stamp changes
+  if (n > 0)
+  {
+    r.incremental = 0;
+    eng->has_map = false;
+    std::memset(&eng->info, 0, sizeof(eng->info));
+    eng->info.n_points = r.n_after;
+    for (DeviceCtx& c : eng->devs)
+    {
+      // the staged points followed by the new ones, joined on the device: the base map does not cross the bus again
+      DevBuf d_pts;
+      int rc = MCL3DL_OK;
+      CK(cudaSetDevice(c.dev));
+      if ((rc = reserve(eng, d_pts, r.n_after * sizeof(mcl3dl_point))))
+        return rc;
+      CK(cudaEventRecord(c.ev[2], c.stream));
+      CK(cudaMemcpyAsync(d_pts.p, c.raw_pts.p, n_before * sizeof(mcl3dl_point), cudaMemcpyDeviceToDevice, c.stream));
+      CK(cudaMemcpyAsync(static_cast<mcl3dl_point*>(d_pts.p) + n_before, pts, n * sizeof(mcl3dl_point),
+                         cudaMemcpyHostToDevice, c.stream));
+      uint64_t reselected = 0;
+      bool incremental = false;
+      if ((rc = build_map_on_device(eng, c, d_pts, r.n_after, n_before, reselected, incremental)))
+        return rc;
+      r.incremental = &c == &eng->devs[0] ? incremental : r.incremental && incremental;
+      r.cells_reselected = std::max(r.cells_reselected, reselected);
+      float ms = 0;
+      CK(cudaEventElapsedTime(&ms, c.ev[2], c.ev[1]));  // (ev[1]: the end of the build, synchronised)
+      r.build_ms = std::max(r.build_ms, static_cast<double>(ms));
+      if ((rc = restage_field(eng, c)))
+        return rc;
+    }
+    eng->has_map = true;
+    eng->n_points = r.n_after;
+  }
+  eng->stamp = stamp;
+  if (info)
+    *info = r;
   return MCL3DL_OK;
 }
 

@@ -55,6 +55,14 @@ class MapInfo(C.Structure):
                 ("dda_max", C.c_float * 3), ("device_bytes", C.c_uint64), ("build_ms", C.c_double)]
 
 
+class MapAppendInfo(C.Structure):
+    _fields_ = [("n_before", C.c_uint64), ("n_appended", C.c_uint64), ("n_after", C.c_uint64), ("incremental", C.c_int32),
+                ("cells_reselected", C.c_uint64), ("build_ms", C.c_double)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
 class UpdateSummary(C.Structure):
     _fields_ = [("weight_sum", C.c_float), ("entropy", C.c_float), ("match_ratio_min", C.c_float),
                 ("match_ratio_max", C.c_float), ("kept", C.c_int32), ("max_index", C.c_uint32)]
@@ -107,7 +115,7 @@ class WorkStats(C.Structure):
         return {k: int(getattr(self, k)) for k, _ in self._fields_}
 
 
-EXPORTED_SYMBOLS = ["mcl3dl_measure_update", "mcl3dl_collect_stats", "mcl3dl_read_stats", "mcl3dl_abi_version", "mcl3dl_create", "mcl3dl_destroy", "mcl3dl_set_map", "mcl3dl_set_params",
+EXPORTED_SYMBOLS = ["mcl3dl_measure_update", "mcl3dl_collect_stats", "mcl3dl_read_stats", "mcl3dl_abi_version", "mcl3dl_create", "mcl3dl_destroy", "mcl3dl_set_map", "mcl3dl_map_append", "mcl3dl_set_params",
                     "mcl3dl_measure", "mcl3dl_measure_device", "mcl3dl_beam_status",
                     "mcl3dl_beam_params_from_reference", "mcl3dl_get_map_info", "mcl3dl_last_timing",
                     "mcl3dl_kernel_launches", "mcl3dl_strerror", "mcl3dl_last_error_detail", "mcl3dl_near_field_info", "mcl3dl_nn_field_info", "mcl3dl_host_alloc", "mcl3dl_host_free", "mcl3dl_field_mode", "mcl3dl_field_nodes", "mcl3dl_field_upload", "mcl3dl_collect_timing",
@@ -138,6 +146,7 @@ def load_library(path=None):
     L.mcl3dl_destroy.argtypes = [vp]
     L.mcl3dl_destroy.restype = None
     L.mcl3dl_set_map.argtypes = [vp, vp, sz, C.c_uint64, vp, vp]
+    L.mcl3dl_map_append.argtypes = [vp, vp, sz, C.c_uint64, vp]
     L.mcl3dl_set_params.argtypes = [vp, vp, vp]
     L.mcl3dl_measure.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp, sz, vp]
     L.mcl3dl_measure_update.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp, sz, vp, vp, vp, vp, vp]
@@ -240,6 +249,17 @@ class Engine:
         self._check(self.L.mcl3dl_set_map(self.h, _ptr(map_pts), len(map_pts), stamp,
                                           C.byref(lik) if lik is not None else None,
                                           C.byref(beam) if beam is not None else None))
+
+    def map_append(self, pts, stamp=None):
+        """Append pts to the staged map (the node's map update; include/mcl3dl_b200.h: mcl3dl_map_append).  stamp as in
+        set_map.  Returns {"n_before", "n_appended", "n_after", "incremental", "cells_reselected", "build_ms"}."""
+        pts = np.ascontiguousarray(pts, dtype=POINT)
+        if stamp is None:
+            self._stamp = getattr(self, "_stamp", 0) + 1
+            stamp = (1 << 40) + self._stamp
+        info = MapAppendInfo()
+        self._check(self.L.mcl3dl_map_append(self.h, _ptr(pts), len(pts), stamp, C.byref(info)))
+        return info.as_dict()
 
     def set_params(self, lik=None, beam=None):
         self._check(self.L.mcl3dl_set_params(self.h, C.byref(lik) if lik is not None else None,

@@ -265,6 +265,9 @@ public:
   }
   void checked(int rc, const char* what) const { check(rc, what); }
   size_t likPoints() const { return lik_cloud_ ? lik_cloud_->size() : 0; }
+  // How each new map reached the engine: appended (mcl3dl_map_append) or staged whole (mcl3dl_set_map).
+  size_t mapAppends() const { return map_appends_; }
+  size_t mapRestages() const { return map_restages_; }
   mcl3dl_engine* engine() { return engine_; }
 
 private:
@@ -320,13 +323,52 @@ private:
       refreshScalars();
       return;
     }
-    std::vector<mcl3dl_point> pts;
-    pack(map, pts);
+    // The node's map update (cbMapUpdateTimer, src/mcl_3dl.cpp:1350-1378) appends to the cloud the index already holds:
+    // the same object, grown, with a new stamp and the staged points unchanged in front.  Only the tail goes to the
+    // engine then.
+    if (map.get() == staged_map_ && map->header.stamp != staged_stamp_ && map->size() > staged_size_ && extendsStaged(*map))
+    {
+      refreshScalars();
+      if (staged_map_)  // (null: a grid-shaping parameter changed, restage below)
+      {
+        std::vector<mcl3dl_point> tail;
+        tail.reserve(map->size() - staged_size_);
+        for (size_t i = staged_size_; i < map->size(); ++i)
+        {
+          const auto& p = map->points[i];
+          tail.push_back(mcl3dl_point{p.x, p.y, p.z, p.label});
+        }
+        staged_map_ = nullptr;  // until the engine holds the grown map (a failed append restages on the next call)
+        check(mcl3dl_map_append(engine_, tail.data(), tail.size(), ++stamp_counter_, nullptr), "mcl3dl_map_append");
+        staged_map_ = map.get();
+        staged_pts_.insert(staged_pts_.end(), tail.begin(), tail.end());
+        staged_stamp_ = map->header.stamp;
+        staged_size_ = map->size();
+        ++map_appends_;
+        return;
+      }
+    }
+    staged_map_ = nullptr;  // until the engine holds the new map
+    pack(map, staged_pts_);
     deriveParams();
-    check(mcl3dl_set_map(engine_, pts.data(), pts.size(), ++stamp_counter_, &lik_c_, &beam_c_), "mcl3dl_set_map");
+    check(mcl3dl_set_map(engine_, staged_pts_.data(), staged_pts_.size(), ++stamp_counter_, &lik_c_, &beam_c_),
+          "mcl3dl_set_map");
     staged_map_ = map.get();
     staged_stamp_ = map->header.stamp;
     staged_size_ = map->size();
+    ++map_restages_;
+  }
+  // The first staged_size_ points of `map` pack to the staged points.
+  bool extendsStaged(const Cloud& map) const
+  {
+    for (size_t i = 0; i < staged_size_; ++i)
+    {
+      const auto& p = map.points[i];
+      const mcl3dl_point q{p.x, p.y, p.z, p.label};
+      if (std::memcmp(&q, &staged_pts_[i], sizeof(q)) != 0)
+        return false;
+    }
+    return true;
   }
   void deriveParams()
   {
@@ -402,7 +444,9 @@ private:
   const Cloud* staged_map_ = nullptr;
   decltype(pcl::PCLHeader().stamp) staged_stamp_ = 0;
   size_t staged_size_ = 0;
+  std::vector<mcl3dl_point> staged_pts_;  // the staged map as packed: recognises an append to it
   uint64_t stamp_counter_ = 0;
+  size_t map_appends_ = 0, map_restages_ = 0;
   Cloud::ConstPtr lik_cloud_, beam_cloud_;
   std::vector<mcl3dl_point> lik_pts_, beam_pts_;
   PinnedArray<mcl3dl_pose> poses_;
