@@ -268,8 +268,8 @@ typedef struct
   float odom_err_integ_ang[3];
 } mcl3dl_state; /* 68 bytes */
 
-/* pf_->init()/resizeParticle() happen on the host; set() uploads the result (states + probability_), get() reads the
- * set back (either pointer may be NULL) — e.g. for pf_->expectationBiased()/covariance(), which stay host code. */
+/* pf_->init() happens on the host (resizeParticle and the global localisation seed have device versions below); set()
+ * uploads the result (states + probability_), get() reads the set back (either pointer may be NULL). */
 int mcl3dl_particles_set(mcl3dl_engine*, const mcl3dl_state* states, const float* prob, size_t n_particles);
 int mcl3dl_particles_get(mcl3dl_engine*, mcl3dl_state* states, float* prob, size_t n_particles);
 /* pf_->predict(motion_prediction_model) for MotionPredictionModelDifferentialDrive: setOdoms(odom_prev, odom_current,
@@ -294,6 +294,53 @@ int mcl3dl_particles_measure_update(mcl3dl_engine*, const mcl3dl_point* lik_pts,
  * sinf / cosf (a few ulp of the noise). */
 int mcl3dl_particles_resample(mcl3dl_engine*, const float sigma_pos[3], const float sigma_rpy[3], float initial_frac,
                               uint64_t seed);
+
+/* pf_->resizeParticle(num) (pf.h:399-436) on the resident set, as the node calls it after every update while the set is
+ * larger than num_particles (src/mcl_3dl.cpp:875-888): sequential float prefix sum accum, pstep = accum_total / num in
+ * float, the sequential float chain pscan += pstep (from 0, added before each pick), output i = the whole state of the
+ * first particle with accum >= pscan_i; outputs whose pscan passes the total copy the last earlier output that found a
+ * particle (particle 0 when none did); probability float(1.0 / num).  Shrink and growth.  Deterministic and exact;
+ * the one departure is the one of resample: particles that tie in accum are taken by lowest index.  INVALID_ARG for
+ * num == 0, num >= 2^31, no resident set or a multi-device engine.  Synchronous. */
+int mcl3dl_particles_resize(mcl3dl_engine*, size_t num);
+
+/* Global localisation (the node's global_localization service, src/mcl_3dl.cpp:1039-1099) on the device; the result
+ * replaces the resident set.
+ *   1. pcl::VoxelGrid of the cloud with leaf float(grid) on all three axes: the restatement of mcl3dl_scan_prepare
+ *      (finite points only, PCL's INT32_MAX overflow rule leaves the cloud unfiltered, output in ascending voxel index,
+ *      centroid float sums in input order; the label vote runs as there, the labels are unused).
+ *   2. Free-space filter: a downsampled point p is dropped when some downsampled point lies within grid of
+ *      q = (p.x, p.y, float(double(p.z) + (0.01 + grid))) — flann::L2_Simple d2 < float(grid * grid) in the space
+ *      rescaled by dist_weight (KdTreeFLANN with the node's point representation; exact, the node's tree has no eps).
+ *      The survivors (the seeds) keep their order.
+ *   3. n_particles = n_seeds * div_yaw: particle i = State6DOF(seed[i / div_yaw], yaw[i % div_yaw]) with
+ *      yaw[c] = (Quat(Vec3(0, 0, 2 pi c / div_yaw)) * imu_quat).normalized() (computed on the host in the reference's
+ *      operation order), noise and odometry-error fields 0, and probability float(1.0 / float(n_seeds)) for every particle.
+ *      That is the reference's own quirk, kept: the set sums to div_yaw, not 1.
+ * pts == NULL: the staged map (set_map, appends included; n is ignored); nothing is uploaded.  Otherwise the host cloud
+ * pts[0..n).
+ * Only the resident set changes (count = n_particles, the resample call count is kept, as for particles_set); the
+ * staged map and its structures, the prepared scans, the matched / unmatched buffers and the exchange buffers are
+ * untouched.  n_seeds == 0 (e.g. an empty cloud): OK with zero counts and the resident set unchanged — a documented
+ * departure, the reference would resize to 0.  Errors, all before the set is touched: INVALID_ARG for a null engine or
+ * params, a multi-device engine, grid <= 0 or not finite, div_yaw < 1, a dist_weight component <= 0 or not finite,
+ * or a host cloud of 2^31 points or more; NO_MAP for pts == NULL before set_map; TOO_LARGE
+ * when n_seeds * div_yaw >= 2^31 or the free-space filter's grid would have 2^31 cells or more.  Synchronous. */
+typedef struct
+{
+  double grid;          /* Parameters::global_localization_grid_ (node default 0.3) */
+  int32_t div_yaw;      /* Parameters::global_localization_div_yaw_ = lround(2 pi / grid_ang) */
+  float imu_quat[4];    /* the node's imu_quat_ (x y z w) */
+  float dist_weight[3]; /* the node's point representation rescale (Parameters::dist_weight_) */
+} mcl3dl_global_localization_params;
+typedef struct
+{
+  uint64_t n_input, n_downsampled, n_seeds, n_particles;
+  float probability; /* what every particle got (0 when n_seeds == 0) */
+  double build_ms;   /* device time of the call (CUDA events on the engine's stream) */
+} mcl3dl_global_localization_info;
+int mcl3dl_global_localization(mcl3dl_engine*, const mcl3dl_point* pts, size_t n, const mcl3dl_global_localization_params*,
+                               mcl3dl_global_localization_info* info);
 
 /* The pose estimate the node takes from the filter after every measurement, on the resident set
  * (src/mcl_3dl.cpp:428-452,704-724): pf_->bias(bias_func) + pf_->expectationBiased() (pf.h:246-251,294-303;

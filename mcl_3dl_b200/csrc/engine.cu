@@ -8,6 +8,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <initializer_list>
 #include <limits>
 #include <string>
 #include <type_traits>
@@ -19,6 +20,7 @@
 #include <cub/device/device_scan.cuh>
 #include <cub/iterator/transform_input_iterator.cuh>
 
+#include "gl_kernels.cuh"
 #include "kernels.cuh"
 #include "match_funcs.cuh"
 #include "pf_kernels.cuh"
@@ -1271,6 +1273,71 @@ int update_nn_field(mcl3dl_engine* eng, DeviceCtx& c, cudaStream_t st, const mcl
 // as they were, every lattice is unchanged: the grids are re-sorted, the near fields get the new points' bits and the NN
 // field re-selects only the cells the new points reach (update_nn_field); `reselected` counts its re-selected cells
 // (all of them on a full build) and `incremental` says which path ran.
+// CSR order of a grid, once its key kernel has written the (cell, point) pairs to keys[0] / vals[0] and the per-cell
+// counts to cell_start[1 .. cells]: the pairs sorted by cell into keys[1] / vals[1] (stable: input order inside a cell),
+// then the inclusive scan that turns the counts into each cell's first index.  tmp: cub scratch.
+int sort_csr(mcl3dl_engine* eng, cudaStream_t st, uint32_t n, size_t cells, uint32_t* cell_start, uint32_t* const keys[2],
+             uint32_t* const vals[2], DevBuf& tmp)
+{
+  int end_bit = 1;
+  while ((size_t(1) << end_bit) < cells && end_bit < 32) ++end_bit;
+  size_t tmp_sort = 0, tmp_scan = 0;
+  CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, keys[0], keys[1], vals[0], vals[1], n, 0, end_bit, st));
+  CK(cub::DeviceScan::InclusiveSum(nullptr, tmp_scan, cell_start, cell_start, static_cast<int>(cells + 1), st));
+  if (int r = reserve(eng, tmp, std::max(tmp_sort, tmp_scan)))
+    return r;
+  size_t tsz = tmp.cap;
+  CK(cub::DeviceRadixSort::SortPairs(tmp.p, tsz, keys[0], keys[1], vals[0], vals[1], n, 0, end_bit, st));
+  tsz = tmp.cap;
+  CK(cub::DeviceScan::InclusiveSum(tmp.p, tsz, cell_start, cell_start, static_cast<int>(cells + 1), st));
+  return MCL3DL_OK;
+}
+
+// Lattice of a likelihood-style search grid with edge `cell` over the rescaled bounding box [sc_min, sc_max]: origin half
+// a cell below the minimum, one spare cell above.  false: 2^31 cells or more.
+bool nn_lattice(float cell, const float sc_min[3], const float sc_max[3], NnGridDev& g, size_t& cells)
+{
+  g.inv_cell = 1.0f / cell;
+  int64_t total = 1;
+  int dims[3];
+  float org[3];
+  for (int k = 0; k < 3; ++k)
+  {
+    org[k] = sc_min[k] - 0.5f * cell;
+    dims[k] = static_cast<int>(std::floor((static_cast<double>(sc_max[k]) - org[k]) / cell)) + 2;
+    total *= dims[k];
+  }
+  if (total >= (int64_t(1) << 31))
+    return false;
+  g.nx = dims[0];
+  g.ny = dims[1];
+  g.nz = dims[2];
+  g.ox = org[0];
+  g.oy = org[1];
+  g.oz = org[2];
+  cells = static_cast<size_t>(total);
+  return true;
+}
+
+// The CSR of a likelihood-style grid g (lattice and dist_weight set) over pts[0..n): cell_start (cells + 1 entries) and
+// the rescaled points in cell order, w = the point's index (nn_key_kernel / sort_csr / nn_gather_kernel).  keys / vals:
+// two arrays of n each; tmp: cub scratch.
+int build_nn_csr(mcl3dl_engine* eng, cudaStream_t st, const mcl3dl_point* pts, uint32_t n, const NnGridDev& g, size_t cells,
+                 uint32_t* const keys[2], uint32_t* const vals[2], DevBuf& tmp, uint32_t* cell_start, float4* out)
+{
+  const int nb = static_cast<int>((static_cast<size_t>(n) + 255) / 256);
+  CK(cudaMemsetAsync(cell_start, 0, (cells + 1) * 4, st));
+  nn_key_kernel<<<nb, 256, 0, st>>>(pts, n, g, keys[0], vals[0], cell_start);
+  CK(cudaGetLastError());
+  eng->launches++;
+  if (int rc = sort_csr(eng, st, n, cells, cell_start, keys, vals, tmp))
+    return rc;
+  nn_gather_kernel<<<nb, 256, 0, st>>>(pts, n, vals[1], g.wx, g.wy, g.wz, out);
+  CK(cudaGetLastError());
+  eng->launches += 3;
+  return MCL3DL_OK;
+}
+
 int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, DevBuf& d_pts, size_t n, size_t n_before, uint64_t& reselected,
                         bool& incremental)
 {
@@ -1287,25 +1354,8 @@ int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, DevBuf& d_pts, size_t 
     return rc;
   CK(cudaEventRecord(e0, st));
   const mcl3dl_point* pts = static_cast<const mcl3dl_point*>(d_pts.p);
-  uint32_t* keys[2] = {static_cast<uint32_t*>(d_keys[0].p), static_cast<uint32_t*>(d_keys[1].p)};
-  uint32_t* vals[2] = {static_cast<uint32_t*>(d_vals[0].p), static_cast<uint32_t*>(d_vals[1].p)};
-  // CSR order of a grid, once its key kernel has written the (cell, point) pairs to keys[0] / vals[0] and the per-cell
-  // counts to cell_start[1 .. cells]: the pairs sorted by cell into keys[1] / vals[1] (stable: map order inside a cell),
-  // then the inclusive scan that turns the counts into each cell's first index
-  auto sort_csr = [&](size_t cells, uint32_t* cell_start) -> int {
-    int end_bit = 1;
-    while ((size_t(1) << end_bit) < cells && end_bit < 32) ++end_bit;
-    size_t tmp_sort = 0, tmp_scan = 0;
-    CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, keys[0], keys[1], vals[0], vals[1], n32, 0, end_bit, st));
-    CK(cub::DeviceScan::InclusiveSum(nullptr, tmp_scan, cell_start, cell_start, static_cast<int>(cells + 1), st));
-    if (int r = reserve(eng, d_tmp, std::max(tmp_sort, tmp_scan)))
-      return r;
-    size_t tsz = d_tmp.cap;
-    CK(cub::DeviceRadixSort::SortPairs(d_tmp.p, tsz, keys[0], keys[1], vals[0], vals[1], n32, 0, end_bit, st));
-    tsz = d_tmp.cap;
-    CK(cub::DeviceScan::InclusiveSum(d_tmp.p, tsz, cell_start, cell_start, static_cast<int>(cells + 1), st));
-    return MCL3DL_OK;
-  };
+  uint32_t* const keys[2] = {static_cast<uint32_t*>(d_keys[0].p), static_cast<uint32_t*>(d_keys[1].p)};
+  uint32_t* const vals[2] = {static_cast<uint32_t*>(d_vals[0].p), static_cast<uint32_t*>(d_vals[1].p)};
 
   // ---- bounding boxes (raw: pcl::getMinMax3D, raycast_using_dda.h:175; rescaled: likelihood grid)
   uint32_t h_bbox[12];
@@ -1348,40 +1398,17 @@ int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, DevBuf& d_pts, size_t 
     const float cell = std::max(eng->lik.match_dist_min * eng->nn_cell_factor, eng->likdev.rpad * 1.01f);
     if (!(cell > 0.0f))
       return MCL3DL_ERR_INVALID_ARG;
-    g.inv_cell = 1.0f / cell;
     g.wx = wx;
     g.wy = wy;
     g.wz = wz;
-    int64_t total = 1;
-    int dims[3];
-    float org[3];
-    for (int k = 0; k < 3; ++k)
-    {
-      org[k] = sc_min[k] - 0.5f * cell;
-      dims[k] = static_cast<int>(std::floor((static_cast<double>(sc_max[k]) - org[k]) / cell)) + 2;
-      total *= dims[k];
-    }
-    if (total >= (int64_t(1) << 31))
+    size_t cells = 0;
+    if (!nn_lattice(cell, sc_min, sc_max, g, cells))
       return MCL3DL_ERR_TOO_LARGE;
-    g.nx = dims[0];
-    g.ny = dims[1];
-    g.nz = dims[2];
-    g.ox = org[0];
-    g.oy = org[1];
-    g.oz = org[2];
-    const size_t cells = static_cast<size_t>(total);
     if ((rc = reserve(eng, c.nn_cell_start, (cells + 1) * 4)) || (rc = reserve(eng, c.nn_pts, n * 16)))
       return rc;
     uint32_t* cell_start = static_cast<uint32_t*>(c.nn_cell_start.p);
-    CK(cudaMemsetAsync(cell_start, 0, (cells + 1) * 4, st));
-    nn_key_kernel<<<nb, tb, 0, st>>>(pts, n32, g, keys[0], vals[0], cell_start);
-    CK(cudaGetLastError());
-    eng->launches++;
-    if ((rc = sort_csr(cells, cell_start)))
+    if ((rc = build_nn_csr(eng, st, pts, n32, g, cells, keys, vals, d_tmp, cell_start, static_cast<float4*>(c.nn_pts.p))))
       return rc;
-    nn_gather_kernel<<<nb, tb, 0, st>>>(pts, n32, vals[1], wx, wy, wz, static_cast<float4*>(c.nn_pts.p));
-    CK(cudaGetLastError());
-    eng->launches += 3;
     g.cell_start = cell_start;
     g.pts = static_cast<const float4*>(c.nn_pts.p);
 #if MCL3DL_NEAR_BITS
@@ -1505,7 +1532,7 @@ int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, DevBuf& d_pts, size_t 
     CK(cudaMemsetAsync(c.dda_occ.p, 0, occ_words * 4, st));
     dda_key_kernel<<<nb, tb, 0, st>>>(pts, n32, g, keys[0], vals[0], cell_start, static_cast<uint32_t*>(c.dda_occ.p));
     CK(cudaGetLastError());
-    if ((rc = sort_csr(cells, cell_start)))
+    if ((rc = sort_csr(eng, st, n32, cells, cell_start, keys, vals, d_tmp)))
       return rc;
     dda_gather_kernel<<<nb, tb, 0, st>>>(pts, n32, vals[1], static_cast<float4*>(c.dda_pts.p));
     CK(cudaGetLastError());
@@ -1538,6 +1565,78 @@ int restage_field(mcl3dl_engine* eng, DeviceCtx& c)
   c.fld_mem = DevBuf();
   c.fld_nodes = cudaPitchedPtr{};
   return eng->field_mode && eng->has_lik ? stage_field(eng, c, nullptr) : MCL3DL_OK;
+}
+
+// The buffers of one VoxelGrid pass: sort keys / values (x2, at least n each, reserved by the caller), the (voxel, label)
+// keys of the vote (x2), voxel-head flags and their scan positions (at least n each, reserved by the caller), cub scratch
+struct VoxelBufs
+{
+  DevBuf* keys[2];
+  DevBuf* vals[2];
+  DevBuf* key_label[2];
+  DevBuf* flags;
+  DevBuf* pos;
+  DevBuf* tmp;
+};
+
+// pcl::VoxelGrid with leaf `leaf` over the device cloud in[0..n) (scan_kernels.cuh: the finite points' bounding box,
+// the lattice and PCL's overflow rule of scan_voxel_lattice, stable sort by voxel key, sort of the (voxel, label) keys,
+// one centroid per voxel in ascending voxel index).  done: the pass wrote the downsampled cloud to out and its size to
+// *d_count; false when the cloud passes unfiltered (out and *d_count untouched).  With no finite point, done is true and
+// nothing is written: the caller's zeroed count stands.  cap: the capacity the vote's keys are reserved for (>= n).
+int voxel_grid(mcl3dl_engine* eng, DeviceCtx& c, cudaStream_t st, const mcl3dl_point* in, uint32_t n, size_t cap, const float leaf[3],
+               const VoxelBufs& b, mcl3dl_point* out, uint32_t* d_count, bool& done)
+{
+  done = false;
+  int rc;
+  const int nb = static_cast<int>((n + 255) / 256);
+  // bounding box of the finite points -> VoxelGrid lattice and PCL's overflow rule (scan_voxel_lattice)
+  uint32_t h_bbox[6] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u};
+  if ((rc = reserve(eng, *b.tmp, 4096)))
+    return rc;
+  uint32_t* bb = static_cast<uint32_t*>(b.tmp->p);
+  CK(cudaMemcpyAsync(bb, h_bbox, sizeof(h_bbox), cudaMemcpyHostToDevice, st));
+  scan_bbox_kernel<<<std::min(nb, c.sm_count * 8), 256, 0, st>>>(in, n, bb);
+  CK(cudaGetLastError());
+  eng->launches++;
+  CK(cudaMemcpyAsync(h_bbox, bb, sizeof(h_bbox), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  const float mn[3] = {ord2f(h_bbox[0]), ord2f(h_bbox[1]), ord2f(h_bbox[2])};
+  const float mx[3] = {ord2f(h_bbox[3]), ord2f(h_bbox[4]), ord2f(h_bbox[5])};
+  VoxelGridDev g{};
+  int end_bit = 0;
+  if (!(mn[0] <= mx[0]))
+  {
+    done = true;  // no finite point: the voxel pass skips every point, the downsampled cloud is empty
+    return MCL3DL_OK;
+  }
+  if (!scan_voxel_lattice(leaf, mn, mx, g, end_bit))
+    return MCL3DL_OK;
+  if ((rc = reserve(eng, *b.key_label[0], cap * 8)) || (rc = reserve(eng, *b.key_label[1], cap * 8)))
+    return rc;
+  uint32_t *k0 = static_cast<uint32_t*>(b.keys[0]->p), *k1 = static_cast<uint32_t*>(b.keys[1]->p);
+  uint32_t *v0 = static_cast<uint32_t*>(b.vals[0]->p), *v1 = static_cast<uint32_t*>(b.vals[1]->p);
+  uint64_t *kl0 = static_cast<uint64_t*>(b.key_label[0]->p), *kl1 = static_cast<uint64_t*>(b.key_label[1]->p);
+  uint32_t *fl = static_cast<uint32_t*>(b.flags->p), *ps = static_cast<uint32_t*>(b.pos->p);
+  scan_key_kernel<<<nb, 256, 0, st>>>(in, n, g, k0, v0, kl0);
+  size_t t_sort = 0, t_sort_kl = 0, t_scan = 0;
+  CK(cub::DeviceRadixSort::SortPairs(nullptr, t_sort, k0, k1, v0, v1, n, 0, end_bit, st));
+  CK(cub::DeviceRadixSort::SortKeys(nullptr, t_sort_kl, kl0, kl1, n, 0, 32 + end_bit, st));
+  CK(cub::DeviceScan::ExclusiveSum(nullptr, t_scan, fl, ps, n, st));
+  if ((rc = reserve(eng, *b.tmp, std::max(std::max(t_sort, t_sort_kl), t_scan) + 256)))
+    return rc;
+  size_t tsz = b.tmp->cap;
+  CK(cub::DeviceRadixSort::SortPairs(b.tmp->p, tsz, k0, k1, v0, v1, n, 0, end_bit, st));  // stable: input order inside a voxel
+  tsz = b.tmp->cap;
+  CK(cub::DeviceRadixSort::SortKeys(b.tmp->p, tsz, kl0, kl1, n, 0, 32 + end_bit, st));  // labels ascending inside a voxel
+  scan_heads_kernel<<<nb, 256, 0, st>>>(k1, n, fl);
+  tsz = b.tmp->cap;
+  CK(cub::DeviceScan::ExclusiveSum(b.tmp->p, tsz, fl, ps, n, st));
+  scan_centroid_kernel<<<nb, 256, 0, st>>>(in, k1, v1, kl1, fl, ps, n, g.cells, out, d_count);
+  CK(cudaGetLastError());
+  eng->launches += 6;
+  done = true;
+  return MCL3DL_OK;
 }
 }  // namespace
 
@@ -2172,6 +2271,32 @@ int mcl3dl_measure_device(mcl3dl_engine* eng, const mcl3dl_pose* d_poses, size_t
 
 // ---- resident particle set (scope row f3; see include/mcl3dl_b200.h; tests/test_gpu_pf_exact.py holds it to its host
 // restatement)
+// Every per-particle buffer of the resident set with room for n particles: both state buffers, the probabilities, the
+// prefix sum + pstep (n + 1), the packed poses and r_extra (the odometry-error factors of an update, the pscan chain of
+// a resize).  reserve() drops a buffer's contents when it grows, so the buffers a kernel still has to read are named in
+// `live` and left as they are (the caller reserves them again once that kernel has run); before anything grows, the
+// stream's pending work is waited for.
+static int reserve_resident(mcl3dl_engine* eng, DeviceCtx& c, size_t n, std::initializer_list<const DevBuf*> live = {})
+{
+  const std::pair<DevBuf*, size_t> want[] = {{&c.r_states[0], n * sizeof(mcl3dl_state)}, {&c.r_states[1], n * sizeof(mcl3dl_state)},
+                                             {&c.r_prob, n * 4},  {&c.r_accum, (n + 1) * 4},
+                                             {&c.r_poses, n * sizeof(mcl3dl_pose)}, {&c.r_extra, n * 4}};
+  bool synced = false;
+  for (const auto& w : want)
+  {
+    if (std::find(live.begin(), live.end(), w.first) != live.end() || (w.first->p && w.second <= w.first->cap))
+      continue;
+    if (!synced)
+    {
+      CK(cudaStreamSynchronize(c.stream));
+      synced = true;
+    }
+    if (int rc = reserve(eng, *w.first, w.second))
+      return rc;
+  }
+  return MCL3DL_OK;
+}
+
 int mcl3dl_particles_set(mcl3dl_engine* eng, const mcl3dl_state* states, const float* prob, size_t n)
 {
   if (!eng || eng->devs.size() != 1 || !states || !prob || n == 0 || n >= (size_t(1) << 31))
@@ -2179,9 +2304,7 @@ int mcl3dl_particles_set(mcl3dl_engine* eng, const mcl3dl_state* states, const f
   DeviceCtx& c = eng->devs[0];
   CK(cudaSetDevice(c.dev));
   int rc;
-  if ((rc = reserve(eng, c.r_states[0], n * sizeof(mcl3dl_state))) || (rc = reserve(eng, c.r_states[1], n * sizeof(mcl3dl_state))) ||
-      (rc = reserve(eng, c.r_prob, n * 4)) || (rc = reserve(eng, c.r_accum, (n + 1) * 4)) ||
-      (rc = reserve(eng, c.r_poses, n * sizeof(mcl3dl_pose))) || (rc = reserve(eng, c.r_extra, n * 4)))
+  if ((rc = reserve_resident(eng, c, n)))
     return rc;
   CK(cudaMemcpyAsync(c.r_states[0].p, states, n * sizeof(mcl3dl_state), cudaMemcpyHostToDevice, c.stream));
   CK(cudaMemcpyAsync(c.r_prob.p, prob, n * 4, cudaMemcpyHostToDevice, c.stream));
@@ -2252,6 +2375,203 @@ int mcl3dl_particles_resample(mcl3dl_engine* eng, const float sigma_pos[3], cons
   CK(cudaGetLastError());
   eng->launches += 2;
   c.r_cur = 1 - c.r_cur;
+  return MCL3DL_OK;
+}
+
+// ---- resize and global localisation of the resident set (gl_kernels.cuh)
+int mcl3dl_particles_resize(mcl3dl_engine* eng, size_t num)
+{
+  if (!eng || eng->devs.size() != 1 || num == 0 || num >= (size_t(1) << 31))
+    return MCL3DL_ERR_INVALID_ARG;
+  DeviceCtx& c = eng->devs[0];
+  if (c.r_n == 0)
+    return MCL3DL_ERR_INVALID_ARG;
+  CK(cudaSetDevice(c.dev));
+  const uint32_t n = static_cast<uint32_t>(c.r_n), num32 = static_cast<uint32_t>(num);
+  float* accum = static_cast<float*>(c.r_accum.p);
+  pf_accum_kernel<<<1, 32, 0, c.stream>>>(static_cast<const float*>(c.r_prob.p), n, accum, accum + n);
+  CK(cudaGetLastError());
+  // the pick reads the current states and accum: they keep their storage until it has run
+  int rc = reserve_resident(eng, c, num, {&c.r_states[c.r_cur], &c.r_accum});
+  if (rc != MCL3DL_OK)
+    return rc;
+  float* pscan = static_cast<float*>(c.r_extra.p);
+  gl_pscan_kernel<<<1, 32, 0, c.stream>>>(accum, n, num32, pscan);
+  gl_resize_kernel<<<(num32 + 255) / 256, 256, 0, c.stream>>>(static_cast<const PfState*>(c.r_states[c.r_cur].p), accum, n, pscan, num32,
+                                                            static_cast<PfState*>(c.r_states[1 - c.r_cur].p),
+                                                            static_cast<float*>(c.r_prob.p));
+  CK(cudaGetLastError());
+  eng->launches += 3;
+  c.r_cur = 1 - c.r_cur;
+  c.r_n = num;
+  if ((rc = reserve_resident(eng, c, num)))  // now the other state buffer and accum as well
+    return rc;
+  CK(cudaStreamSynchronize(c.stream));
+  return MCL3DL_OK;
+}
+
+int mcl3dl_global_localization(mcl3dl_engine* eng, const mcl3dl_point* pts, size_t n, const mcl3dl_global_localization_params* gp,
+                               mcl3dl_global_localization_info* info)
+{
+  if (!eng || eng->devs.size() != 1 || !gp || !(gp->grid > 0.0) || !std::isfinite(gp->grid) || gp->div_yaw < 1 ||
+      (pts && n >= (size_t(1) << 31)))
+    return MCL3DL_ERR_INVALID_ARG;
+  for (int k = 0; k < 3; ++k)
+    if (!(gp->dist_weight[k] > 0.0f) || !std::isfinite(gp->dist_weight[k]))
+      return MCL3DL_ERR_INVALID_ARG;
+  if (!pts && !eng->has_map)
+    return MCL3DL_ERR_NO_MAP;
+  DeviceCtx& c = eng->devs[0];
+  const size_t cnt = pts ? n : eng->n_points;
+  mcl3dl_global_localization_info out{};
+  out.n_input = cnt;
+  if (info)
+    *info = out;
+  if (cnt == 0)
+    return MCL3DL_OK;
+  CK(cudaSetDevice(c.dev));
+  cudaStream_t st = c.stream;
+  cudaEvent_t e0 = c.ev[0], e1 = c.ev[1];  // the per-update timing events, unused between calls
+  // stage buffers of this call only: the uploaded cloud, the VoxelGrid's sort and scan buffers, the downsampled cloud,
+  // the filter's CSR grid, the seeds, the yaw table, [0] downsampled / [1] seed counts
+  DevBuf d_in, d_keys[2], d_vals[2], d_kl[2], d_flags, d_pos, d_tmp, d_ds, d_cell_start, d_grid, d_seeds, d_yaw, d_count, d_bbox;
+  const uint32_t n32 = static_cast<uint32_t>(cnt);
+  int rc;
+  if ((rc = reserve(eng, d_keys[0], cnt * 4)) || (rc = reserve(eng, d_keys[1], cnt * 4)) || (rc = reserve(eng, d_vals[0], cnt * 4)) ||
+      (rc = reserve(eng, d_vals[1], cnt * 4)) || (rc = reserve(eng, d_flags, cnt * 4)) || (rc = reserve(eng, d_pos, cnt * 4)) ||
+      (rc = reserve(eng, d_ds, cnt * 16)) || (rc = reserve(eng, d_count, 64)) || (rc = reserve(eng, d_bbox, 12 * 4)) ||
+      (pts && (rc = reserve(eng, d_in, cnt * 16))))
+    return rc;
+  CK(cudaEventRecord(e0, st));
+  const mcl3dl_point* src = static_cast<const mcl3dl_point*>(c.raw_pts.p);
+  if (pts)
+  {
+    CK(cudaMemcpyAsync(d_in.p, pts, cnt * 16, cudaMemcpyHostToDevice, st));
+    src = static_cast<const mcl3dl_point*>(d_in.p);
+  }
+  uint32_t* count = static_cast<uint32_t*>(d_count.p);
+  CK(cudaMemsetAsync(count, 0, 64, st));
+  // 1. VoxelGrid at float(grid)
+  const float g32 = static_cast<float>(gp->grid);
+  const float leaf[3] = {g32, g32, g32};
+  const VoxelBufs vb{{&d_keys[0], &d_keys[1]}, {&d_vals[0], &d_vals[1]}, {&d_kl[0], &d_kl[1]}, &d_flags, &d_pos, &d_tmp};
+  bool filtered = false;
+  if ((rc = voxel_grid(eng, c, st, src, n32, cnt, leaf, vb, static_cast<mcl3dl_point*>(d_ds.p), count, filtered)))
+    return rc;
+  const mcl3dl_point* ds = src;  // unfiltered (PCL's overflow rule): the cloud itself
+  uint32_t n_ds = n32;
+  if (filtered)
+  {
+    CK(cudaMemcpyAsync(&n_ds, count, 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    ds = static_cast<const mcl3dl_point*>(d_ds.p);
+  }
+  out.n_downsampled = n_ds;
+  if (n_ds == 0)
+  {
+    if (info)
+      *info = out;
+    return MCL3DL_OK;
+  }
+  // 2. free-space filter over a likelihood-style CSR grid of the downsampled cloud in the rescaled space
+  const float wx = gp->dist_weight[0], wy = gp->dist_weight[1], wz = gp->dist_weight[2];
+  const int nb = static_cast<int>((n_ds + 255) / 256);
+  uint32_t h_bbox[12];
+  for (int k = 0; k < 3; ++k)
+  {
+    h_bbox[k] = 0xffffffffu;
+    h_bbox[3 + k] = 0u;
+    h_bbox[6 + k] = 0xffffffffu;
+    h_bbox[9 + k] = 0u;
+  }
+  CK(cudaMemcpyAsync(d_bbox.p, h_bbox, sizeof(h_bbox), cudaMemcpyHostToDevice, st));
+  bbox_kernel<<<std::min(nb, c.sm_count * 8), 256, 0, st>>>(ds, n_ds, wx, wy, wz, static_cast<uint32_t*>(d_bbox.p));
+  CK(cudaGetLastError());
+  eng->launches++;
+  CK(cudaMemcpyAsync(h_bbox, d_bbox.p, sizeof(h_bbox), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  float sc_min[3], sc_max[3];
+  for (int k = 0; k < 3; ++k)
+  {
+    sc_min[k] = ord2f(h_bbox[6 + k]);
+    sc_max[k] = ord2f(h_bbox[9 + k]);
+    if (!std::isfinite(sc_min[k]) || !std::isfinite(sc_max[k]))
+      return MCL3DL_ERR_TOO_LARGE;  // an infinite coordinate (only an unfiltered cloud keeps one): no finite lattice
+  }
+  GlDev m{};
+  m.z_off = 0.01 + gp->grid;
+  m.r2 = static_cast<float>(gp->grid * gp->grid);
+  m.rpad = g32 * 1.0001f + 1e-6f;
+  NnGridDev g{};
+  g.wx = wx;
+  g.wy = wy;
+  g.wz = wz;
+  size_t cells = 0;
+  // the window (q -/+ rpad) spans at most 3 cells per axis: cell edge strictly above rpad (1 % margin, as for the map)
+  if (!nn_lattice(m.rpad * 1.01f, sc_min, sc_max, g, cells))
+    return MCL3DL_ERR_TOO_LARGE;
+  if ((rc = reserve(eng, d_cell_start, (cells + 1) * 4)) || (rc = reserve(eng, d_grid, static_cast<size_t>(n_ds) * 16)) ||
+      (rc = reserve(eng, d_seeds, static_cast<size_t>(n_ds) * 16)))
+    return rc;
+  uint32_t* const keys[2] = {static_cast<uint32_t*>(d_keys[0].p), static_cast<uint32_t*>(d_keys[1].p)};
+  uint32_t* const vals[2] = {static_cast<uint32_t*>(d_vals[0].p), static_cast<uint32_t*>(d_vals[1].p)};
+  if ((rc = build_nn_csr(eng, st, ds, n_ds, g, cells, keys, vals, d_tmp, static_cast<uint32_t*>(d_cell_start.p),
+                         static_cast<float4*>(d_grid.p))))
+    return rc;
+  g.cell_start = static_cast<const uint32_t*>(d_cell_start.p);
+  g.pts = static_cast<const float4*>(d_grid.p);
+  uint32_t* flags = static_cast<uint32_t*>(d_flags.p);
+  uint32_t* pos = static_cast<uint32_t*>(d_pos.p);
+  gl_flag_kernel<<<nb, 256, 0, st>>>(ds, n_ds, g, m, flags);
+  CK(cudaGetLastError());
+  size_t t_scan = 0;
+  CK(cub::DeviceScan::ExclusiveSum(nullptr, t_scan, flags, pos, n_ds, st));
+  if ((rc = reserve(eng, d_tmp, t_scan + 256)))
+    return rc;
+  size_t tsz = d_tmp.cap;
+  CK(cub::DeviceScan::ExclusiveSum(d_tmp.p, tsz, flags, pos, n_ds, st));
+  scan_compact_kernel<<<nb, 256, 0, st>>>(ds, flags, pos, n_ds, static_cast<mcl3dl_point*>(d_seeds.p), count + 1);
+  CK(cudaGetLastError());
+  eng->launches += 3;
+  uint32_t n_seeds = 0;
+  CK(cudaMemcpyAsync(&n_seeds, count + 1, 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  out.n_seeds = n_seeds;
+  if (n_seeds == 0)
+  {
+    if (info)
+      *info = out;
+    return MCL3DL_OK;  // documented departure: the set stays as it was
+  }
+  const uint64_t n_particles = static_cast<uint64_t>(n_seeds) * static_cast<uint64_t>(gp->div_yaw);
+  if (n_particles >= (uint64_t(1) << 31))
+    return MCL3DL_ERR_TOO_LARGE;
+  // 3. the particles: yaw table from the host, one thread per particle
+  std::vector<Q4> yaw(static_cast<size_t>(gp->div_yaw));
+  gl_yaw_quats(gp->div_yaw, gp->imu_quat, yaw.data());
+  if ((rc = reserve(eng, d_yaw, yaw.size() * sizeof(Q4))))
+    return rc;
+  CK(cudaMemcpyAsync(d_yaw.p, yaw.data(), yaw.size() * sizeof(Q4), cudaMemcpyHostToDevice, st));
+  if ((rc = reserve_resident(eng, c, n_particles)))
+    return rc;
+  const float prob = gl_probability(n_seeds);
+  const uint32_t np32 = static_cast<uint32_t>(n_particles);
+  gl_fill_kernel<<<(np32 + 255) / 256, 256, 0, st>>>(static_cast<const mcl3dl_point*>(d_seeds.p), static_cast<const Q4*>(d_yaw.p),
+                                                     static_cast<uint32_t>(gp->div_yaw), np32, prob,
+                                                     static_cast<PfState*>(c.r_states[0].p), static_cast<float*>(c.r_prob.p));
+  CK(cudaGetLastError());
+  eng->launches++;
+  CK(cudaEventRecord(e1, st));
+  CK(cudaStreamSynchronize(st));
+  c.r_n = n_particles;
+  c.r_cur = 0;
+  float ms = 0;
+  CK(cudaEventElapsedTime(&ms, e0, e1));
+  out.n_particles = n_particles;
+  out.probability = prob;
+  out.build_ms = ms;
+  if (info)
+    *info = out;
   return MCL3DL_OK;
 }
 
@@ -2387,52 +2707,10 @@ int mcl3dl_scan_prepare(mcl3dl_engine* eng, const mcl3dl_point* raw, size_t n_ra
   bool ds_done = false;
   if (downsample)
   {
-    // bounding box of the finite points -> VoxelGrid lattice and PCL's overflow rule (scan_voxel_lattice)
-    uint32_t h_bbox[6] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0u, 0u, 0u};
-    if ((rc = reserve(eng, c.s_tmp, 4096)))
+    const VoxelBufs vb{{&c.s_keys[0], &c.s_keys[1]}, {&c.s_vals[0], &c.s_vals[1]}, {&c.s_key_label[0], &c.s_key_label[1]},
+                       &c.s_flags[0], &c.s_pos[0], &c.s_tmp};
+    if ((rc = voxel_grid(eng, c, st, d_raw, n, cap, sp->downsample, vb, static_cast<mcl3dl_point*>(c.s_ds.p), counts + 0, ds_done)))
       return rc;
-    uint32_t* bb = static_cast<uint32_t*>(c.s_tmp.p);
-    CK(cudaMemcpyAsync(bb, h_bbox, sizeof(h_bbox), cudaMemcpyHostToDevice, st));
-    scan_bbox_kernel<<<std::min(nb, c.sm_count * 8), 256, 0, st>>>(d_raw, n, bb);
-    CK(cudaGetLastError());
-    eng->launches++;
-    CK(cudaMemcpyAsync(h_bbox, bb, sizeof(h_bbox), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    const float mn[3] = {ord2f(h_bbox[0]), ord2f(h_bbox[1]), ord2f(h_bbox[2])};
-    const float mx[3] = {ord2f(h_bbox[3]), ord2f(h_bbox[4]), ord2f(h_bbox[5])};
-    VoxelGridDev g{};
-    int end_bit = 0;
-    if (!(mn[0] <= mx[0]))
-    {
-      ds_done = true;  // no finite point: the voxel pass skips every point, the downsampled cloud is empty (counts[0] == 0)
-    }
-    else if (scan_voxel_lattice(sp->downsample, mn, mx, g, end_bit))
-    {
-      if ((rc = reserve(eng, c.s_key_label[0], cap * 8)) || (rc = reserve(eng, c.s_key_label[1], cap * 8)))
-        return rc;
-      uint32_t *k0 = static_cast<uint32_t*>(c.s_keys[0].p), *k1 = static_cast<uint32_t*>(c.s_keys[1].p);
-      uint32_t *v0 = static_cast<uint32_t*>(c.s_vals[0].p), *v1 = static_cast<uint32_t*>(c.s_vals[1].p);
-      uint64_t *kl0 = static_cast<uint64_t*>(c.s_key_label[0].p), *kl1 = static_cast<uint64_t*>(c.s_key_label[1].p);
-      uint32_t *fl = static_cast<uint32_t*>(c.s_flags[0].p), *ps = static_cast<uint32_t*>(c.s_pos[0].p);
-      scan_key_kernel<<<nb, 256, 0, st>>>(d_raw, n, g, k0, v0, kl0);
-      size_t t_sort = 0, t_sort_kl = 0, t_scan = 0;
-      CK(cub::DeviceRadixSort::SortPairs(nullptr, t_sort, k0, k1, v0, v1, n, 0, end_bit, st));
-      CK(cub::DeviceRadixSort::SortKeys(nullptr, t_sort_kl, kl0, kl1, n, 0, 32 + end_bit, st));
-      CK(cub::DeviceScan::ExclusiveSum(nullptr, t_scan, fl, ps, n, st));
-      if ((rc = reserve(eng, c.s_tmp, std::max(std::max(t_sort, t_sort_kl), t_scan) + 256)))
-        return rc;
-      size_t tsz = c.s_tmp.cap;
-      CK(cub::DeviceRadixSort::SortPairs(c.s_tmp.p, tsz, k0, k1, v0, v1, n, 0, end_bit, st));  // stable: input order inside a voxel
-      tsz = c.s_tmp.cap;
-      CK(cub::DeviceRadixSort::SortKeys(c.s_tmp.p, tsz, kl0, kl1, n, 0, 32 + end_bit, st));  // labels ascending inside a voxel
-      scan_heads_kernel<<<nb, 256, 0, st>>>(k1, n, fl);
-      tsz = c.s_tmp.cap;
-      CK(cub::DeviceScan::ExclusiveSum(c.s_tmp.p, tsz, fl, ps, n, st));
-      scan_centroid_kernel<<<nb, 256, 0, st>>>(d_raw, k1, v1, kl1, fl, ps, n, g.cells, static_cast<mcl3dl_point*>(c.s_ds.p), counts + 0);
-      CK(cudaGetLastError());
-      eng->launches += 6;
-      ds_done = true;
-    }
     d_ds = static_cast<const mcl3dl_point*>(c.s_ds.p);
   }
   if (!ds_done)

@@ -100,6 +100,19 @@ class MatchParams(C.Structure):
                 ("max_search_radius", C.c_float)]
 
 
+class GlobalLocalizationParams(C.Structure):
+    """mcl3dl_global_localization_params (Engine.global_localization fills it; its defaults are the node's)."""
+    _fields_ = [("grid", C.c_double), ("div_yaw", C.c_int32), ("imu_quat", C.c_float * 4), ("dist_weight", C.c_float * 3)]
+
+
+class GlobalLocalizationInfo(C.Structure):
+    _fields_ = [("n_input", C.c_uint64), ("n_downsampled", C.c_uint64), ("n_seeds", C.c_uint64), ("n_particles", C.c_uint64),
+                ("probability", C.c_float), ("build_ms", C.c_double)]
+
+    def as_dict(self):
+        return {k: (float if k in ("probability", "build_ms") else int)(getattr(self, k)) for k, _ in self._fields_}
+
+
 class Estimate(C.Structure):
     """mcl3dl_estimate"""
     _fields_ = [("mean_biased", C.c_float * 8), ("max_state", C.c_float * 8), ("max_index", C.c_uint32),
@@ -122,7 +135,8 @@ EXPORTED_SYMBOLS = ["mcl3dl_measure_update", "mcl3dl_collect_stats", "mcl3dl_rea
                     "mcl3dl_exchange_create", "mcl3dl_exchange_open", "mcl3dl_measure_exchange_device", "mcl3dl_exchange_current",
                     "mcl3dl_particles_set", "mcl3dl_particles_get", "mcl3dl_particles_predict",
                     "mcl3dl_particles_measure_update", "mcl3dl_particles_resample", "mcl3dl_particles_estimate", "mcl3dl_scan_prepare", "mcl3dl_scan_get",
-                    "mcl3dl_particles_measure_update_prepared", "mcl3dl_match_output"]
+                    "mcl3dl_particles_measure_update_prepared", "mcl3dl_match_output",
+                    "mcl3dl_particles_resize", "mcl3dl_global_localization"]
 
 _LIBS = {}
 
@@ -172,6 +186,8 @@ def load_library(path=None):
     L.mcl3dl_particles_measure_update.argtypes = [vp, vp, sz, vp, sz, vp, sz, C.c_float, vp]
     L.mcl3dl_particles_resample.argtypes = [vp, vp, vp, C.c_float, C.c_uint64]
     L.mcl3dl_particles_estimate.argtypes = [vp, vp, C.c_float, C.c_float, vp]
+    L.mcl3dl_particles_resize.argtypes = [vp, sz]
+    L.mcl3dl_global_localization.argtypes = [vp, vp, sz, vp, vp]
     L.mcl3dl_scan_prepare.argtypes = [vp, vp, sz, vp, vp]
     L.mcl3dl_scan_get.argtypes = [vp, C.c_int, vp, sz, C.POINTER(sz)]
     L.mcl3dl_particles_measure_update_prepared.argtypes = [vp, vp, sz, C.c_float, vp]
@@ -435,6 +451,28 @@ class Engine:
         sp = np.ascontiguousarray(sigma_pos, dtype=np.float32)
         sr = np.ascontiguousarray(sigma_rpy, dtype=np.float32)
         self._check(self.L.mcl3dl_particles_resample(self.h, _ptr(sp), _ptr(sr), initial_frac, seed))
+
+    def particles_resize(self, num):
+        """pf_->resizeParticle(num) on the resident set (include/mcl3dl_b200.h: mcl3dl_particles_resize)."""
+        self._check(self.L.mcl3dl_particles_resize(self.h, num))
+        self._n_resident = int(num)
+
+    def global_localization(self, pts=None, grid=0.3, div_yaw=12, imu_quat=(0.0, 0.0, 0.0, 1.0), dist_weight=(1.0, 1.0, 1.0)):
+        """The node's global_localization service on the device (include/mcl3dl_b200.h: mcl3dl_global_localization): seeds
+        the resident set from pts (POINT array) or, pts=None, from the staged map.  Returns the info as a dict; with no
+        seed the resident set is left as it was."""
+        gp = GlobalLocalizationParams(grid, div_yaw, (C.c_float * 4)(*imu_quat), (C.c_float * 3)(*dist_weight))
+        info = GlobalLocalizationInfo()
+        src, n = None, 0
+        if pts is not None:  # a host cloud, possibly empty: never NULL, which would mean the staged map
+            pts = np.ascontiguousarray(pts, dtype=POINT)
+            n = len(pts)
+            buf = pts if n else np.zeros(1, POINT)
+            src = buf.ctypes.data_as(C.c_void_p)
+        self._check(self.L.mcl3dl_global_localization(self.h, src, n, C.byref(gp), C.byref(info)))
+        if info.n_particles:
+            self._n_resident = int(info.n_particles)
+        return info.as_dict()
 
     # ---- scan preprocessing on the device (scope row f4; include/mcl3dl_b200.h)
     def scan_prepare(self, raw_pts, params):

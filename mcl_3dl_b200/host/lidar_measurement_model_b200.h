@@ -210,6 +210,13 @@ public:
           "mcl3dl_measure_update");
   }
   // Scope row f3: the same update on the engine's RESIDENT particle set (nothing per particle crosses the bus).
+  // the global_localization service on the device over the index's cloud, staged first if it is not (or is stale)
+  void globalLocalization(ChunkedKdtree<PointType>::Ptr& kdtree, const mcl3dl_global_localization_params& params,
+                          mcl3dl_global_localization_info* info)
+  {
+    stageMap(kdtree);
+    check(mcl3dl_global_localization(engine_, nullptr, 0, &params, info), "mcl3dl_global_localization");
+  }
   void measureResident(ChunkedKdtree<PointType>::Ptr& kdtree, const Cloud::ConstPtr& pc_lik, const Cloud::ConstPtr& pc_beam,
                        const std::vector<Vec3>& origins, float odom_err_integ_lin_sigma, mcl3dl_update_summary* summary)
   {
@@ -561,9 +568,9 @@ public:
   // ---- Scope row f3: the particle set kept RESIDENT on the device between updates.  The node's cycle
   //   pf_->predict(model) / pf_->measure(lambda) / pf_->bias + expectationBiased + max + covariance / pf_->resample(sigma)
   // (src/mcl_3dl.cpp:227-232,402-452,704-724,809-815) becomes predictResident / measureResident / estimateResident /
-  // resampleResident; only scans, odometry and summaries cross the bus.  uploadResident() after init() / resizeParticle() /
-  // any host-side edit of particles_, downloadResident() whenever host code needs the particles (markers, expansion
-  // resetting).  Documented departures (include/mcl3dl_b200.h): counter-based noise instead of the std engine's stream,
+  // resampleResident; only scans, odometry and summaries cross the bus.  uploadResident() after init() / any host-side
+  // edit of particles_ (globalLocalizationResident / resizeResident replace the service body and resizeParticle),
+  // downloadResident() whenever host code needs the particles (markers, expansion resetting).  Documented departures (include/mcl3dl_b200.h): counter-based noise instead of the std engine's stream,
   // ties of the accumulated probability go to the lowest index, sums in double.
   static mcl3dl_state toState(const State6DOF& s)
   {
@@ -664,6 +671,26 @@ public:
       frac = 0.0f;
     const float sp[3] = {sigma_pos.x_, sigma_pos.y_, sigma_pos.z_}, sr[3] = {sigma_rpy.x_, sigma_rpy.y_, sigma_rpy.z_};
     batcher.checked(mcl3dl_particles_resample(batcher.engine(), sp, sr, frac, seed), "mcl3dl_particles_resample");
+  }
+  // The global_localization service body (src/mcl_3dl.cpp:1039-1099) on the device over the map index's cloud (pc_map_,
+  // staged here if it is not yet): VoxelGrid, free-space filter and the div_yaw particles per seed replace the resident
+  // set.  particles_ is resized to the new count, its contents stale until downloadResident(), so getParticleSize() and
+  // setGlobalLocalizationStatus() keep working.  With no seed nothing changes (the reference would resize to 0).
+  mcl3dl_global_localization_info globalLocalizationResident(MeasurementBatcher& batcher, ChunkedKdtree<PointType>::Ptr& kdtree,
+                                                             const mcl3dl_global_localization_params& params)
+  {
+    mcl3dl_global_localization_info info;
+    batcher.globalLocalization(kdtree, params, &info);
+    if (info.n_particles)
+      particles_.resize(info.n_particles);
+    return info;
+  }
+  // pf_->resizeParticle(num) (pf.h:399-436) on the resident set, e.g. the node's shrink after an update while the set is
+  // larger than num_particles (src/mcl_3dl.cpp:875-888); particles_ is resized as in globalLocalizationResident
+  void resizeResident(MeasurementBatcher& batcher, size_t num)
+  {
+    batcher.checked(mcl3dl_particles_resize(batcher.engine(), num), "mcl3dl_particles_resize");
+    particles_.resize(num);
   }
 };
 
