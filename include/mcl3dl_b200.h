@@ -295,6 +295,42 @@ int mcl3dl_particles_measure_update(mcl3dl_engine*, const mcl3dl_point* lik_pts,
 int mcl3dl_particles_resample(mcl3dl_engine*, const float sigma_pos[3], const float sigma_rpy[3], float initial_frac,
                               uint64_t seed);
 
+/* The node's other per-particle events on the resident set.  Single-device engines; synchronous; INVALID_ARG for a null
+ * engine or pointer, no resident set or a multi-device engine.
+ *
+ * Random numbers: the documented departure of resample, Philox-4x32-10 keyed by seed (key words = its low and high 32
+ * bits), one block per counter (particle index, call count, block, event).  The event word keeps the streams apart:
+ * 0 resample (blocks 0 and 1), 1 the odometry-noise redraw (block 0), 2 the expansion noise (blocks 0 and 1).  A block's
+ * four output words w0..w3 give uniforms u(w) = float((w >> 8) + 1) * 2^-24 in (0, 1], and Box-Muller on a pair (u, v)
+ * gives z = sqrtf(-2 logf(u)) * cosf(2 pi v) and z' = ... * sinf(2 pi v) (float, in that order).  Resample and the
+ * expansion noise take the pairs (w0, w1), (w2, w3) of block 0 and (w0, w1) of block 1 for x, y, z, roll, pitch, yaw,
+ * each times its sigma (0 where the sigma is 0).  Every entry point keeps its own call count: 1 on the first call of an
+ * engine, never reset by particles_set.
+ *
+ * redraw_odom_noise: the node's update_noise_func through pf_->predict (src/mcl_3dl.cpp:817-825).  Block 0's two pairs give
+ * z0..z3 and, in the node's draw order, noise_ll = float(double(z0) * lin_lin), noise_la = float(double(z1) * lin_ang),
+ * noise_aa = float(double(z2) * ang_ang), noise_al = float(double(z3) * ang_lin).  Nothing else changes, the
+ * probabilities included.  INVALID_ARG for a negative or non-finite sigma. */
+int mcl3dl_particles_redraw_odom_noise(mcl3dl_engine*, double lin_lin, double lin_ang, double ang_lin, double ang_ang,
+                                       uint64_t seed);
+/* noise: pf_->noise(State6DOF(sigma_pos, sigma_rpy)) (pf.h:226-237), expansion resetting (src/mcl_3dl.cpp:853-864): every
+ * particle becomes state + generateNoise, as resample treats a duplicate, with two differences the reference makes and
+ * that are kept: the rotation is NOT normalised afterwards (rot = nrot * rot as it comes), and operator+ builds a fresh
+ * State6DOF, so noise_ll/la/al/aa become 0 (the node calls this right after the redraw, whose values are discarded).  The
+ * probabilities are unchanged.  INVALID_ARG for a negative or non-finite sigma. */
+int mcl3dl_particles_noise(mcl3dl_engine*, const float sigma_pos[3], const float sigma_rpy[3], uint64_t seed);
+/* imu_update: ImuMeasurementModelGravity::setAccMeasure(acc_measure) + pf_->measure(imu measure) (cbImu,
+ * src/mcl_3dl.cpp:941-1018; imu_measurement_model_gravity.h:45-55; pf.h:252-279).  On the host, once: |acc_measure| as
+ * Vec3::norm and NormalLikelihood<float>(float(acc_var)) (a = float(1.0 / sqrt(2 pi s s)), sq2 = float(float(s s) * 2.0)).
+ * Per particle: acc_estim = rot.inv() * (0, 0, 1) with the RAW rot, diff = acosf(dot / (|acc_measure| |acc_estim|)),
+ * likelihood = a * expf(-diff * diff / sq2), w = prior * likelihood; then the fold of mcl3dl_particles_measure_update
+ * (double sums with a fixed tree, the posterior replaces the probabilities, kept = 0 keeps the prior).  The summary's
+ * match_ratio_min and match_ratio_max are both 0: no likelihood model ran.  An acosf argument that rounds above 1 makes
+ * that particle's likelihood NaN; as in the reference (sum > 0 is false), the whole update is then discarded: kept = 0,
+ * weight_sum NaN, probabilities untouched.  Documented departure: INVALID_ARG when float(acc_var) is not finite and
+ * positive (the reference would compute with it). */
+int mcl3dl_particles_imu_update(mcl3dl_engine*, const float acc_measure[3], double acc_var, mcl3dl_update_summary* summary);
+
 /* pf_->resizeParticle(num) (pf.h:399-436) on the resident set, as the node calls it after every update while the set is
  * larger than num_particles (src/mcl_3dl.cpp:875-888): sequential float prefix sum accum, pstep = accum_total / num in
  * float, the sequential float chain pscan += pstep (from 0, added before each pick), output i = the whole state of the

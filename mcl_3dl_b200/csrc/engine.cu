@@ -509,6 +509,7 @@ struct DeviceCtx
   size_t r_n = 0;
   int r_cur = 0;
   uint32_t r_calls = 0;
+  uint32_t r_redraw_calls = 0, r_noise_calls = 0;  // the Philox call words of the odometry-noise redraw and the expansion noise
   // record exchange over peer memory (one process per GPU, mcl3dl_exchange_*): [world * n_local records | world flags]
   DevBuf xchg, x_ticket;  // x_ticket: [0] completed-step counter, [1] error word (device memory, local)
   PeerTable xt{};
@@ -2375,6 +2376,93 @@ int mcl3dl_particles_resample(mcl3dl_engine* eng, const float sigma_pos[3], cons
   CK(cudaGetLastError());
   eng->launches += 2;
   c.r_cur = 1 - c.r_cur;
+  return MCL3DL_OK;
+}
+
+// ---- the node's other particle events on the resident set: the odometry-noise redraw, expansion resetting and the
+// IMU gravity update (pf_kernels.cuh)
+static bool finite_nonneg(double v) { return v >= 0.0 && std::isfinite(v); }
+
+int mcl3dl_particles_redraw_odom_noise(mcl3dl_engine* eng, double lin_lin, double lin_ang, double ang_lin, double ang_ang, uint64_t seed)
+{
+  if (!eng || eng->devs.size() != 1 || !finite_nonneg(lin_lin) || !finite_nonneg(lin_ang) || !finite_nonneg(ang_lin) ||
+      !finite_nonneg(ang_ang))
+    return MCL3DL_ERR_INVALID_ARG;
+  DeviceCtx& c = eng->devs[0];
+  if (c.r_n == 0)
+    return MCL3DL_ERR_INVALID_ARG;
+  CK(cudaSetDevice(c.dev));
+  const uint32_t n = static_cast<uint32_t>(c.r_n);
+  OdomNoiseSigma sg;
+  sg.ll = lin_lin;
+  sg.la = lin_ang;
+  sg.aa = ang_ang;
+  sg.al = ang_lin;
+  ++c.r_redraw_calls;
+  pf_redraw_kernel<<<(n + 255) / 256, 256, 0, c.stream>>>(static_cast<PfState*>(c.r_states[c.r_cur].p), n, seed, c.r_redraw_calls, sg);
+  CK(cudaGetLastError());
+  eng->launches++;
+  CK(cudaStreamSynchronize(c.stream));
+  return MCL3DL_OK;
+}
+
+int mcl3dl_particles_noise(mcl3dl_engine* eng, const float sigma_pos[3], const float sigma_rpy[3], uint64_t seed)
+{
+  if (!eng || eng->devs.size() != 1 || !sigma_pos || !sigma_rpy)
+    return MCL3DL_ERR_INVALID_ARG;
+  Sigma6 sg;
+  for (int k = 0; k < 3; ++k)
+  {
+    sg.v[k] = sigma_pos[k];
+    sg.v[k + 3] = sigma_rpy[k];
+  }
+  for (float v : sg.v)
+    if (!finite_nonneg(v))
+      return MCL3DL_ERR_INVALID_ARG;
+  DeviceCtx& c = eng->devs[0];
+  if (c.r_n == 0)
+    return MCL3DL_ERR_INVALID_ARG;
+  CK(cudaSetDevice(c.dev));
+  const uint32_t n = static_cast<uint32_t>(c.r_n);
+  ++c.r_noise_calls;
+  pf_noise_kernel<<<(n + 255) / 256, 256, 0, c.stream>>>(static_cast<PfState*>(c.r_states[c.r_cur].p), n, seed, c.r_noise_calls, sg);
+  CK(cudaGetLastError());
+  eng->launches++;
+  CK(cudaStreamSynchronize(c.stream));
+  return MCL3DL_OK;
+}
+
+int mcl3dl_particles_imu_update(mcl3dl_engine* eng, const float acc_measure[3], double acc_var, mcl3dl_update_summary* summary)
+{
+  if (!eng || eng->devs.size() != 1 || !acc_measure || !summary)
+    return MCL3DL_ERR_INVALID_ARG;
+  const float sigma = static_cast<float>(acc_var);  // ImuMeasurementModelGravity(const float acc_var)
+  if (!(sigma > 0.0f) || !std::isfinite(sigma))
+    return MCL3DL_ERR_INVALID_ARG;
+  DeviceCtx& c = eng->devs[0];
+  const size_t P = c.r_n;
+  if (P == 0)
+    return MCL3DL_ERR_INVALID_ARG;
+  CK(cudaSetDevice(c.dev));
+  const Share s = share_of(P, 1, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0);  // only the two WeightPartials come back
+  int rc;
+  if ((rc = reserve(eng, c.h_pinned, s.total)) || (rc = reserve(eng, c.d_out, P * sizeof(mcl3dl_result))))
+    return rc;
+  const ImuDev m = pf_imu_setup(acc_measure, sigma);
+  const uint32_t n32 = static_cast<uint32_t>(P);
+  mcl3dl_result* d_rec = static_cast<mcl3dl_result*>(c.d_out.p);
+  float* lik = static_cast<float*>(c.r_extra.p);
+  pf_imu_kernel<<<(n32 + 255) / 256, 256, 0, c.stream>>>(static_cast<const PfState*>(c.r_states[c.r_cur].p), n32, m, d_rec, lik);
+  CK(cudaGetLastError());
+  eng->launches++;
+  // unit records and the likelihood as the extra factor: w = prior * (((1 * 1) * 1) * lik) = prior * lik; n_lik = 0 makes
+  // every particle's match ratio 0
+  float* prob = static_cast<float*>(c.r_prob.p);
+  WeightPartial* h_part = reinterpret_cast<WeightPartial*>(static_cast<char*>(c.h_pinned.p) + s.o_part);
+  if ((rc = fold_weights(eng, c, d_rec, prob, lik, prob, P, 0, 0, h_part, nullptr)))
+    return rc;
+  CK(cudaStreamSynchronize(c.stream));
+  make_summary(h_part[0], h_part[1], summary);
   return MCL3DL_OK;
 }
 

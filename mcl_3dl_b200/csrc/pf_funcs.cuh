@@ -205,10 +205,11 @@ __device__ __forceinline__ uint32_t pf_pick(const float* __restrict__ accum, uin
   return lo == 0 ? 0u : pf_lower_bound(accum, n, pf_pscan(pstep, initial_p, lo - 1));
 }
 
-// state + generateNoise(org[0..6)) followed by normalize(): State6DOF::generateNoise / operator+ / normalize
-// (state_6dof.h:226-261,154-157), Quat::setRPY (quat.h:196-209).  org = the six draws (x y z roll pitch yaw); the noise
-// mean is zero (DiagonalNoiseGenerator(State6DOF(), sigma)).  The result is a fresh State6DOF: noise_* = 0.
-__device__ __forceinline__ PfState pf_add_noise(const PfState& s, const float org[6])
+// state + generateNoise(org[0..6)): State6DOF::generateNoise / operator+ (state_6dof.h:226-261), Quat::setRPY
+// (quat.h:196-209).  org = the six draws (x y z roll pitch yaw); the noise mean is zero (DiagonalNoiseGenerator(State6DOF(),
+// sigma)).  The result is a fresh State6DOF: noise_* = 0, and rot = nrot * rot as it comes, not normalised — what
+// pf::ParticleFilter::addNoiseUsingNoiseGenerator leaves (pf.h:226-237).
+__device__ __forceinline__ PfState pf_add_noise_raw(const PfState& s, const float org[6])
 {
   const float t2 = cosf(fdiv(org[3], 2.0f)), t3 = sinf(fdiv(org[3], 2.0f));
   const float t4 = cosf(fdiv(org[4], 2.0f)), t5 = sinf(fdiv(org[4], 2.0f));
@@ -231,7 +232,24 @@ __device__ __forceinline__ PfState pf_add_noise(const PfState& s, const float or
   rot.y = s.rot[1];
   rot.z = s.rot[2];
   rot.w = s.rot[3];
-  rot = qnormalize4(qmul(nrot, rot));  // ret.rot_ = a.rot_ * rot_ with a = the noise (:259), then normalize()
+  rot = qmul(nrot, rot);  // ret.rot_ = a.rot_ * rot_ with a = the noise (:259)
+  r.rot[0] = rot.x;
+  r.rot[1] = rot.y;
+  r.rot[2] = rot.z;
+  r.rot[3] = rot.w;
+  return r;
+}
+
+// state + noise followed by normalize() (state_6dof.h:154-157), as resampling treats a duplicate (pf.h:216-217)
+__device__ __forceinline__ PfState pf_add_noise(const PfState& s, const float org[6])
+{
+  PfState r = pf_add_noise_raw(s, org);
+  Q4 rot;
+  rot.x = r.rot[0];
+  rot.y = r.rot[1];
+  rot.z = r.rot[2];
+  rot.w = r.rot[3];
+  rot = qnormalize4(rot);
   r.rot[0] = rot.x;
   r.rot[1] = rot.y;
   r.rot[2] = rot.z;
@@ -267,10 +285,18 @@ __device__ __forceinline__ void philox4x32_10(uint32_t c[4], uint32_t k0, uint32
 // uniform in (0, 1]: never 0, so the logarithm below is finite
 __device__ __forceinline__ float u01(uint32_t x) { return fmul(fadd(static_cast<float>(x >> 8), 1.0f), 5.9604644775390625e-08f); }
 
-// six N(0, sigma_k) draws for output particle `index` of resampling call `call` (Box-Muller on three pairs)
-__device__ __forceinline__ void pf_noise6(uint64_t seed, uint32_t index, uint32_t call, const float sigma[6], float org[6])
+// The counter's fourth word names the event, so that the events of one seed draw from disjoint streams:
+//   (index, call, block, kPfEventResample): resampling's duplicate noise, blocks 0 and 1 (pf_noise6);
+//   (index, call, 0, kPfEventRedraw):       the odometry-noise redraw, one block = two Box-Muller pairs;
+//   (index, call, block, kPfEventNoise):    expansion resetting's noise, blocks 0 and 1, laid out as pf_noise6.
+// `call` is the entry point's own call count (1 on the first call of an engine).
+constexpr uint32_t kPfEventResample = 0, kPfEventRedraw = 1, kPfEventNoise = 2;
+
+// six N(0, sigma_k) draws for particle `index` of call `call` of `event` (Box-Muller on three pairs)
+__device__ __forceinline__ void pf_noise6_event(uint64_t seed, uint32_t index, uint32_t call, uint32_t event, const float sigma[6],
+                                                float org[6])
 {
-  uint32_t a[4] = {index, call, 0u, 0u}, b[4] = {index, call, 1u, 0u};
+  uint32_t a[4] = {index, call, 0u, event}, b[4] = {index, call, 1u, event};
   const uint32_t k0 = static_cast<uint32_t>(seed), k1 = static_cast<uint32_t>(seed >> 32);
   philox4x32_10(a, k0, k1);
   philox4x32_10(b, k0, k1);
@@ -282,6 +308,92 @@ __device__ __forceinline__ void pf_noise6(uint64_t seed, uint32_t index, uint32_
     org[2 * pair] = sigma[2 * pair] == 0.0f ? 0.0f : fmul(fmul(rad, cosf(phi)), sigma[2 * pair]);
     org[2 * pair + 1] = sigma[2 * pair + 1] == 0.0f ? 0.0f : fmul(fmul(rad, sinf(phi)), sigma[2 * pair + 1]);
   }
+}
+
+// resampling's draws for output particle `index` of resampling call `call`
+__device__ __forceinline__ void pf_noise6(uint64_t seed, uint32_t index, uint32_t call, const float sigma[6], float org[6])
+{
+  pf_noise6_event(seed, index, call, kPfEventResample, sigma, org);
+}
+
+// The node's update_noise_func (src/mcl_3dl.cpp:817-825) for particle `index` of redraw call `call`: four standard
+// normals z0..z3 (Box-Muller on the two pairs of one Philox block), noise_x = float(double(z_k) * sigma_x) in the node's
+// draw order ll, la, aa, al (the reference multiplies its float draw by the double parameter).  Nothing else changes.
+struct OdomNoiseSigma
+{
+  double ll, la, aa, al;  // Parameters::odom_err_lin_lin_, _lin_ang_, _ang_ang_, _ang_lin_
+};
+
+__device__ __forceinline__ void pf_redraw_odom_noise(PfState& s, uint64_t seed, uint32_t index, uint32_t call, const OdomNoiseSigma& sg)
+{
+  uint32_t c[4] = {index, call, 0u, kPfEventRedraw};
+  philox4x32_10(c, static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32));
+  float z[4];
+  for (int pair = 0; pair < 2; ++pair)
+  {
+    const float rad = __fsqrt_rn(fmul(-2.0f, logf(u01(c[2 * pair]))));
+    const float phi = fmul(6.283185307179586f, u01(c[2 * pair + 1]));
+    z[2 * pair] = fmul(rad, cosf(phi));
+    z[2 * pair + 1] = fmul(rad, sinf(phi));
+  }
+  s.noise_ll = __double2float_rn(dmul(static_cast<double>(z[0]), sg.ll));
+  s.noise_la = __double2float_rn(dmul(static_cast<double>(z[1]), sg.la));
+  s.noise_aa = __double2float_rn(dmul(static_cast<double>(z[2]), sg.aa));
+  s.noise_al = __double2float_rn(dmul(static_cast<double>(z[3]), sg.al));
+}
+
+// pf_->noise(State6DOF(sigma_pos, sigma_rpy)) for particle `index` of call `call` (pf.h:226-237): state + noise, the
+// rotation NOT normalised and noise_* = 0, as the reference leaves them
+__device__ __forceinline__ PfState pf_expansion_noise(const PfState& s, uint64_t seed, uint32_t index, uint32_t call, const float sigma[6])
+{
+  float org[6];
+  pf_noise6_event(seed, index, call, kPfEventNoise, sigma, org);
+  return pf_add_noise_raw(s, org);
+}
+
+// ---- IMU gravity update: ImuMeasurementModelGravity::setAccMeasure + measure (imu_measurement_model_gravity.h:45-55)
+struct ImuDev
+{
+  F3 acc;          // acc_measure_
+  float acc_norm;  // acc_measure_norm_ = Vec3::norm (vec3.h:153-156)
+  float nd_a;      // NormalLikelihood<float>(float(acc_var)): a_ = float(1.0 / sqrt(2 pi s s)) (nd.h:45-49)
+  float nd_sq2;    //   sq2_ = float(float(s * s) * 2.0)
+};
+
+// Host side, once per call, in the reference's operation order (plain host arithmetic, as pf_set_odoms)
+inline ImuDev pf_imu_setup(const float acc[3], float sigma)
+{
+  ImuDev m;
+  m.acc = F3{acc[0], acc[1], acc[2]};
+  m.acc_norm = sqrtf(acc[0] * acc[0] + acc[1] * acc[1] + acc[2] * acc[2]);
+  m.nd_a = static_cast<float>(1.0 / sqrt(2.0 * M_PI * sigma * sigma));
+  m.nd_sq2 = static_cast<float>(sigma * sigma * 2.0);
+  return m;
+}
+
+// The likelihood of one particle: acc_estim = rot.inv() * (0, 0, 1) with the RAW rot (Quat::inv = conj * float(1.0 / dot),
+// quat.h:187-190, and the two-Hamilton-product rotation), diff = acosf(dot / (|acc_measure| * |acc_estim|)),
+// nd(diff) = a * expf(-diff * diff / sq2).  An acosf argument that rounds above 1 gives NaN, as in the reference.
+__device__ __forceinline__ float pf_imu_likelihood(const PfState& s, const ImuDev& m)
+{
+  Q4 r;
+  r.x = s.rot[0];
+  r.y = s.rot[1];
+  r.z = s.rot[2];
+  r.w = s.rot[3];
+  Q4 cj;
+  cj.x = -r.x;
+  cj.y = -r.y;
+  cj.z = -r.z;
+  cj.w = r.w;
+  const Q4 inv = qdiv(cj, qdot4(r, r));
+  F3 ez;
+  ez.x = 0.0f;
+  ez.y = 0.0f;
+  ez.z = 1.0f;
+  const F3 e = qrot(inv, ez);
+  const float diff = acosf(fdiv(dot3(e, m.acc), fmul(m.acc_norm, __fsqrt_rn(dot3(e, e)))));
+  return fmul(m.nd_a, expf(fdiv(fmul(-diff, diff), m.nd_sq2)));
 }
 
 // ---- pose estimate (src/mcl_3dl.cpp:428-452,704-724): per-particle terms

@@ -128,6 +128,39 @@ __global__ void pf_resample_kernel(const PfState* __restrict__ in, const float* 
   out_probs[i] = __double2float_rn(ddiv(1.0, static_cast<double>(n)));
 }
 
+// the node's update_noise_func through pf_->predict (src/mcl_3dl.cpp:817-825): the four noise_* fields, in place
+__global__ void pf_redraw_kernel(PfState* __restrict__ states, uint32_t n, uint64_t seed, uint32_t call, OdomNoiseSigma sigma)
+{
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n)
+    pf_redraw_odom_noise(states[i], seed, i, call, sigma);
+}
+
+// pf_->noise(State6DOF(sigma)) (pf.h:226-237, expansion resetting at src/mcl_3dl.cpp:853-864): every particle, in place
+__global__ void pf_noise_kernel(PfState* __restrict__ states, uint32_t n, uint64_t seed, uint32_t call, Sigma6 sigma)
+{
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n)
+    states[i] = pf_expansion_noise(states[i], seed, i, call, sigma.v);
+}
+
+// The IMU gravity likelihood per particle into lik, and a unit record (score_beam = score_like = 1, match_cnt = 0) per
+// particle, so that pass 1 of the weight fold computes prior * lik with the extra factor
+__global__ void pf_imu_kernel(const PfState* __restrict__ states, uint32_t n, ImuDev m, mcl3dl_result* __restrict__ rec,
+                              float* __restrict__ lik)
+{
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n)
+    return;
+  lik[i] = pf_imu_likelihood(states[i], m);
+  mcl3dl_result r;
+  r.score_like = 1.0f;
+  r.match_cnt = 0;
+  r.score_beam = 1.0f;
+  r.n_short = r.n_hit = r.n_long = 0;
+  rec[i] = r;
+}
+
 // ---- pose estimate on the resident set (mcl3dl_particles_estimate): pf_->bias + expectationBiased + max + covariance
 // (src/mcl_3dl.cpp:428-452,704-724; pf.h:246-251,281-374).  Two passes of double sums with a fixed tree (lanes by
 // shuffles, warps and CTAs in order), so the result is deterministic; the reference sums sequentially in float, hence

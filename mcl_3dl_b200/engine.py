@@ -136,7 +136,8 @@ EXPORTED_SYMBOLS = ["mcl3dl_measure_update", "mcl3dl_collect_stats", "mcl3dl_rea
                     "mcl3dl_particles_set", "mcl3dl_particles_get", "mcl3dl_particles_predict",
                     "mcl3dl_particles_measure_update", "mcl3dl_particles_resample", "mcl3dl_particles_estimate", "mcl3dl_scan_prepare", "mcl3dl_scan_get",
                     "mcl3dl_particles_measure_update_prepared", "mcl3dl_match_output",
-                    "mcl3dl_particles_resize", "mcl3dl_global_localization"]
+                    "mcl3dl_particles_resize", "mcl3dl_global_localization",
+                    "mcl3dl_particles_redraw_odom_noise", "mcl3dl_particles_noise", "mcl3dl_particles_imu_update"]
 
 _LIBS = {}
 
@@ -188,6 +189,9 @@ def load_library(path=None):
     L.mcl3dl_particles_estimate.argtypes = [vp, vp, C.c_float, C.c_float, vp]
     L.mcl3dl_particles_resize.argtypes = [vp, sz]
     L.mcl3dl_global_localization.argtypes = [vp, vp, sz, vp, vp]
+    L.mcl3dl_particles_redraw_odom_noise.argtypes = [vp, C.c_double, C.c_double, C.c_double, C.c_double, C.c_uint64]
+    L.mcl3dl_particles_noise.argtypes = [vp, vp, vp, C.c_uint64]
+    L.mcl3dl_particles_imu_update.argtypes = [vp, vp, C.c_double, vp]
     L.mcl3dl_scan_prepare.argtypes = [vp, vp, sz, vp, vp]
     L.mcl3dl_scan_get.argtypes = [vp, C.c_int, vp, sz, C.POINTER(sz)]
     L.mcl3dl_particles_measure_update_prepared.argtypes = [vp, vp, sz, C.c_float, vp]
@@ -451,6 +455,27 @@ class Engine:
         sp = np.ascontiguousarray(sigma_pos, dtype=np.float32)
         sr = np.ascontiguousarray(sigma_rpy, dtype=np.float32)
         self._check(self.L.mcl3dl_particles_resample(self.h, _ptr(sp), _ptr(sr), initial_frac, seed))
+
+    def particles_redraw_odom_noise(self, lin_lin, lin_ang, ang_lin, ang_ang, seed):
+        """The node's odometry-noise redraw on the resident set (include/mcl3dl_b200.h: mcl3dl_particles_redraw_odom_noise)."""
+        self._check(self.L.mcl3dl_particles_redraw_odom_noise(self.h, lin_lin, lin_ang, ang_lin, ang_ang, seed))
+
+    def particles_noise(self, sigma_pos, sigma_rpy, seed):
+        """pf_->noise(State6DOF(sigma_pos, sigma_rpy)), expansion resetting, on the resident set
+        (include/mcl3dl_b200.h: mcl3dl_particles_noise)."""
+        sp = np.ascontiguousarray(sigma_pos, dtype=np.float32)
+        sr = np.ascontiguousarray(sigma_rpy, dtype=np.float32)
+        assert sp.size == 3 and sr.size == 3
+        self._check(self.L.mcl3dl_particles_noise(self.h, _ptr(sp), _ptr(sr), seed))
+
+    def particles_imu_update(self, acc_measure, acc_var):
+        """The IMU gravity update on the resident set (include/mcl3dl_b200.h: mcl3dl_particles_imu_update); returns the
+        update summary as a dict."""
+        acc = np.ascontiguousarray(acc_measure, dtype=np.float32)
+        assert acc.size == 3
+        summ = UpdateSummary()
+        self._check(self.L.mcl3dl_particles_imu_update(self.h, _ptr(acc), acc_var, C.byref(summ)))
+        return summ.as_dict()
 
     def particles_resize(self, num):
         """pf_->resizeParticle(num) on the resident set (include/mcl3dl_b200.h: mcl3dl_particles_resize)."""

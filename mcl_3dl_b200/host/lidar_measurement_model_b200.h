@@ -568,9 +568,11 @@ public:
   // ---- Scope row f3: the particle set kept RESIDENT on the device between updates.  The node's cycle
   //   pf_->predict(model) / pf_->measure(lambda) / pf_->bias + expectationBiased + max + covariance / pf_->resample(sigma)
   // (src/mcl_3dl.cpp:227-232,402-452,704-724,809-815) becomes predictResident / measureResident / estimateResident /
-  // resampleResident; only scans, odometry and summaries cross the bus.  uploadResident() after init() / any host-side
-  // edit of particles_ (globalLocalizationResident / resizeResident replace the service body and resizeParticle),
-  // downloadResident() whenever host code needs the particles (markers, expansion resetting).  Documented departures (include/mcl3dl_b200.h): counter-based noise instead of the std engine's stream,
+  // resampleResident; only scans, odometry and summaries cross the bus.  redrawOdomNoiseResident, noiseResident and
+  // imuMeasureResident replace the odometry-noise redraw, expansion resetting and cbImu's gravity update.  uploadResident()
+  // after init() / any host-side edit of particles_ (globalLocalizationResident / resizeResident replace the service body
+  // and resizeParticle), downloadResident() whenever host code needs the particles (publishParticles' markers).
+  // Documented departures (include/mcl3dl_b200.h): counter-based noise instead of the std engine's stream,
   // ties of the accumulated probability go to the lowest index, sums in double.
   static mcl3dl_state toState(const State6DOF& s)
   {
@@ -671,6 +673,31 @@ public:
       frac = 0.0f;
     const float sp[3] = {sigma_pos.x_, sigma_pos.y_, sigma_pos.z_}, sr[3] = {sigma_rpy.x_, sigma_rpy.y_, sigma_rpy.z_};
     batcher.checked(mcl3dl_particles_resample(batcher.engine(), sp, sr, frac, seed), "mcl3dl_particles_resample");
+  }
+  // The odometry-noise redraw after resampling, pf_->predict(update_noise_func) (src/mcl_3dl.cpp:817-825), with the node's
+  // params_.odom_err_lin_lin_, _lin_ang_, _ang_lin_, _ang_ang_
+  void redrawOdomNoiseResident(MeasurementBatcher& batcher, double lin_lin, double lin_ang, double ang_lin, double ang_ang, uint64_t seed)
+  {
+    batcher.checked(mcl3dl_particles_redraw_odom_noise(batcher.engine(), lin_lin, lin_ang, ang_lin, ang_ang, seed),
+                    "mcl3dl_particles_redraw_odom_noise");
+  }
+  // Expansion resetting, pf_->noise(State6DOF(sigma_pos, sigma_rpy)) (src/mcl_3dl.cpp:853-864): rotations are left
+  // un-normalised and noise_* zeroed, as the reference leaves them
+  void noiseResident(MeasurementBatcher& batcher, const Vec3& sigma_pos, const Vec3& sigma_rpy, uint64_t seed)
+  {
+    const float sp[3] = {sigma_pos.x_, sigma_pos.y_, sigma_pos.z_}, sr[3] = {sigma_rpy.x_, sigma_rpy.y_, sigma_rpy.z_};
+    batcher.checked(mcl3dl_particles_noise(batcher.engine(), sp, sr, seed), "mcl3dl_particles_noise");
+  }
+  // cbImu's imu_measurement_model_->setAccMeasure(acc_measure) + pf_->measure(imu_measure_func) (src/mcl_3dl.cpp:1003-1008)
+  // for ImuMeasurementModelGravity(acc_var)
+  UpdateResult imuMeasureResident(MeasurementBatcher& batcher, const Vec3& acc_measure, float acc_var)
+  {
+    mcl3dl_update_summary s;
+    const float acc[3] = {acc_measure.x_, acc_measure.y_, acc_measure.z_};
+    batcher.checked(mcl3dl_particles_imu_update(batcher.engine(), acc, acc_var, &s), "mcl3dl_particles_imu_update");
+    if (s.kept)
+      entropy_ = s.entropy;
+    return UpdateResult{s.match_ratio_min, s.match_ratio_max, s.kept != 0};
   }
   // The global_localization service body (src/mcl_3dl.cpp:1039-1099) on the device over the map index's cloud (pc_map_,
   // staged here if it is not yet): VoxelGrid, free-space filter and the div_yaw particles per seed replace the resident
