@@ -812,8 +812,15 @@ int stage_field(mcl3dl_engine* eng, DeviceCtx& c, const float* host_nodes)
     LikDev lp = eng->likdev;
     lp.rpad = f.radius;
     lp.r2 = static_cast<float>(static_cast<double>(clamp) * static_cast<double>(clamp));
+    NnGridDev g = c.nn;
+#if MCL3DL_NEAR_BITS
+    // The likelihood screen is built for likdev.rpad, and the field's radius can be larger (the KD-tree raycaster's
+    // search radius): in an overflow cell the window search must then run unscreened, or a node whose nearest point
+    // lies between the two radii would read `clamp`.
+    g.near.bits = nullptr;
+#endif
     const size_t total = static_cast<size_t>(nnx) * nny * nnz;
-    field_nodes_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(c.nn, lp, c.fld_nodes, nnx, nny, nnz, clamp);
+    field_nodes_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(g, lp, c.fld_nodes, nnx, nny, nnz, clamp);
     CK(cudaGetLastError());
     eng->launches++;
   }
