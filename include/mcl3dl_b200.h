@@ -331,6 +331,37 @@ int mcl3dl_particles_noise(mcl3dl_engine*, const float sigma_pos[3], const float
  * positive (the reference would compute with it). */
 int mcl3dl_particles_imu_update(mcl3dl_engine*, const float acc_measure[3], double acc_var, mcl3dl_update_summary* summary);
 
+/* landmark_update: cbLandmark's pf_->measure (src/mcl_3dl.cpp:899-931; nd.h:61-83; pf.h:252-279).  The host builds the
+ * reference's own NormalLikelihoodNd<float, 6> from the message's covariance, as cbLandmark does
+ * (Eigen::Matrix<double, 6, 6>(covariance.data()).cast<float>(); Eigen maps that array column-major, so a non-symmetric
+ * covariance enters transposed), and passes its a_ and sigma_inv_: Eigen's determinant and inverse stay on the host.
+ * measured is the message's pose as received (RAW rotation; _pad ignored).  Per particle: diff = s - measured
+ * (state_6dof.h:262-274: the position per axis in float, rot = measured.rot.inv() * rot with both rotations RAW,
+ * Quat::inv = conj * float(1.0 / double(dot))), x = (diff.pos, diff.rot.getRPY()), likelihood = a * expf(q) with
+ * q = -0.5 x^T S x evaluated in float in this fixed order (a documented departure: Eigen's order depends on its
+ * vectorisation): h_k = -0.5 x_k, r_j = sum over k = 0..5 of h_k S(k, j), q = sum over j = 0..5 of r_j x_j, each sum
+ * accumulated left to right from its first product.  Then the fold of mcl3dl_particles_imu_update: w = prior *
+ * likelihood, double sums with a fixed tree, the posterior replaces the probabilities; match_ratio_min and _max are 0.
+ * A NaN likelihood (e.g. a NaN rotation) or weights that all underflow to 0 (a landmark far from every particle)
+ * discard the whole update, as the reference's sum > 0 test does: kept = 0, probabilities untouched.  The states never
+ * change.  Documented departure: INVALID_ARG when nd_a, any sigma_inv entry or any of the measured pose's seven values
+ * is not finite (the reference would compute with them). */
+typedef struct
+{
+  mcl3dl_pose measured;  /* the message's pose: position + orientation as received (RAW) */
+  float nd_a;            /* NormalLikelihoodNd<float, 6>::a_ */
+  float sigma_inv[36];   /* NormalLikelihoodNd<float, 6>::sigma_inv_, row-major: [r * 6 + c] = sigma_inv_(r, c) */
+} mcl3dl_landmark_params;
+int mcl3dl_particles_landmark_update(mcl3dl_engine*, const mcl3dl_landmark_params* params, mcl3dl_update_summary* summary);
+/* reset_odom_err_integ: the node's integ_reset_func through pf_->predict (the pose-jump branch of measure(),
+ * src/mcl_3dl.cpp:653-658, and cbPosition, :190-195): odom_err_integ_lin and odom_err_integ_ang become +0.0f.  Nothing
+ * else changes, the probabilities included. */
+int mcl3dl_particles_reset_odom_err_integ(mcl3dl_engine*);
+/* get_poses: what publishParticles (src/mcl_3dl.cpp:1101-1125) publishes, 32 bytes per particle instead of the 72 of
+ * particles_get: out[i] = the position and rot.normalized() (quat.h:175-177: rot * float(1.0 / double(sqrtf(dot)))),
+ * _pad = 0.  The resident set is not modified (the reference normalises a copy).  n must equal the resident count. */
+int mcl3dl_particles_get_poses(mcl3dl_engine*, mcl3dl_pose* out, size_t n);
+
 /* pf_->resizeParticle(num) (pf.h:399-436) on the resident set, as the node calls it after every update while the set is
  * larger than num_particles (src/mcl_3dl.cpp:875-888): sequential float prefix sum accum, pstep = accum_total / num in
  * float, the sequential float chain pscan += pstep (from 0, added before each pick), output i = the whole state of the

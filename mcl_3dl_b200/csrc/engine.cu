@@ -2439,6 +2439,35 @@ int mcl3dl_particles_noise(mcl3dl_engine* eng, const float sigma_pos[3], const f
   return MCL3DL_OK;
 }
 
+// An update of the resident set whose likelihood one thread-per-particle kernel computes (pf_imu_kernel,
+// pf_landmark_kernel): launch(d_rec, lik) writes a unit record and the likelihood of every particle, and the weight fold
+// takes the likelihood as the extra factor: w = prior * (((1 * 1) * 1) * lik) = prior * lik; n_lik = 0 makes every
+// particle's match ratio 0.  The posterior replaces the resident probabilities unless the update is discarded.
+extern "C++" {
+template <typename Launch>
+static int resident_likelihood_update(mcl3dl_engine* eng, DeviceCtx& c, mcl3dl_update_summary* summary, Launch launch)
+{
+  const size_t P = c.r_n;
+  CK(cudaSetDevice(c.dev));
+  const Share s = share_of(P, 1, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0);  // only the two WeightPartials come back
+  int rc;
+  if ((rc = reserve(eng, c.h_pinned, s.total)) || (rc = reserve(eng, c.d_out, P * sizeof(mcl3dl_result))))
+    return rc;
+  mcl3dl_result* d_rec = static_cast<mcl3dl_result*>(c.d_out.p);
+  float* lik = static_cast<float*>(c.r_extra.p);
+  launch(d_rec, lik);
+  CK(cudaGetLastError());
+  eng->launches++;
+  float* prob = static_cast<float*>(c.r_prob.p);
+  WeightPartial* h_part = reinterpret_cast<WeightPartial*>(static_cast<char*>(c.h_pinned.p) + s.o_part);
+  if ((rc = fold_weights(eng, c, d_rec, prob, lik, prob, P, 0, 0, h_part, nullptr)))
+    return rc;
+  CK(cudaStreamSynchronize(c.stream));
+  make_summary(h_part[0], h_part[1], summary);
+  return MCL3DL_OK;
+}
+}  // extern "C++"
+
 int mcl3dl_particles_imu_update(mcl3dl_engine* eng, const float acc_measure[3], double acc_var, mcl3dl_update_summary* summary)
 {
   if (!eng || eng->devs.size() != 1 || !acc_measure || !summary)
@@ -2447,29 +2476,78 @@ int mcl3dl_particles_imu_update(mcl3dl_engine* eng, const float acc_measure[3], 
   if (!(sigma > 0.0f) || !std::isfinite(sigma))
     return MCL3DL_ERR_INVALID_ARG;
   DeviceCtx& c = eng->devs[0];
-  const size_t P = c.r_n;
-  if (P == 0)
+  if (c.r_n == 0)
+    return MCL3DL_ERR_INVALID_ARG;
+  const ImuDev m = pf_imu_setup(acc_measure, sigma);
+  const uint32_t n32 = static_cast<uint32_t>(c.r_n);
+  return resident_likelihood_update(eng, c, summary, [&](mcl3dl_result* d_rec, float* lik) {
+    pf_imu_kernel<<<(n32 + 255) / 256, 256, 0, c.stream>>>(static_cast<const PfState*>(c.r_states[c.r_cur].p), n32, m, d_rec, lik);
+  });
+}
+
+// ---- the landmark update, the odometry-error reset and the published poses on the resident set (pf_kernels.cuh)
+int mcl3dl_particles_landmark_update(mcl3dl_engine* eng, const mcl3dl_landmark_params* params, mcl3dl_update_summary* summary)
+{
+  if (!eng || eng->devs.size() != 1 || !params || !summary)
+    return MCL3DL_ERR_INVALID_ARG;
+  const mcl3dl_pose& q = params->measured;
+  const float pose[7] = {q.px, q.py, q.pz, q.qx, q.qy, q.qz, q.qw};
+  for (float v : pose)
+    if (!std::isfinite(v))
+      return MCL3DL_ERR_INVALID_ARG;
+  if (!std::isfinite(params->nd_a))
+    return MCL3DL_ERR_INVALID_ARG;
+  for (float v : params->sigma_inv)
+    if (!std::isfinite(v))
+      return MCL3DL_ERR_INVALID_ARG;
+  DeviceCtx& c = eng->devs[0];
+  if (c.r_n == 0)
+    return MCL3DL_ERR_INVALID_ARG;
+  LandmarkDev m;
+  m.pos[0] = q.px;
+  m.pos[1] = q.py;
+  m.pos[2] = q.pz;
+  m.rot = Q4{q.qx, q.qy, q.qz, q.qw};
+  m.nd_a = params->nd_a;
+  std::memcpy(m.sigma_inv, params->sigma_inv, sizeof(m.sigma_inv));
+  const uint32_t n32 = static_cast<uint32_t>(c.r_n);
+  return resident_likelihood_update(eng, c, summary, [&](mcl3dl_result* d_rec, float* lik) {
+    pf_landmark_kernel<<<(n32 + 255) / 256, 256, 0, c.stream>>>(static_cast<const PfState*>(c.r_states[c.r_cur].p), n32, m, d_rec, lik);
+  });
+}
+
+int mcl3dl_particles_reset_odom_err_integ(mcl3dl_engine* eng)
+{
+  if (!eng || eng->devs.size() != 1)
+    return MCL3DL_ERR_INVALID_ARG;
+  DeviceCtx& c = eng->devs[0];
+  if (c.r_n == 0)
     return MCL3DL_ERR_INVALID_ARG;
   CK(cudaSetDevice(c.dev));
-  const Share s = share_of(P, 1, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0);  // only the two WeightPartials come back
-  int rc;
-  if ((rc = reserve(eng, c.h_pinned, s.total)) || (rc = reserve(eng, c.d_out, P * sizeof(mcl3dl_result))))
-    return rc;
-  const ImuDev m = pf_imu_setup(acc_measure, sigma);
-  const uint32_t n32 = static_cast<uint32_t>(P);
-  mcl3dl_result* d_rec = static_cast<mcl3dl_result*>(c.d_out.p);
-  float* lik = static_cast<float*>(c.r_extra.p);
-  pf_imu_kernel<<<(n32 + 255) / 256, 256, 0, c.stream>>>(static_cast<const PfState*>(c.r_states[c.r_cur].p), n32, m, d_rec, lik);
+  const uint32_t n = static_cast<uint32_t>(c.r_n);
+  pf_reset_odom_err_kernel<<<(n + 255) / 256, 256, 0, c.stream>>>(static_cast<PfState*>(c.r_states[c.r_cur].p), n);
   CK(cudaGetLastError());
   eng->launches++;
-  // unit records and the likelihood as the extra factor: w = prior * (((1 * 1) * 1) * lik) = prior * lik; n_lik = 0 makes
-  // every particle's match ratio 0
-  float* prob = static_cast<float*>(c.r_prob.p);
-  WeightPartial* h_part = reinterpret_cast<WeightPartial*>(static_cast<char*>(c.h_pinned.p) + s.o_part);
-  if ((rc = fold_weights(eng, c, d_rec, prob, lik, prob, P, 0, 0, h_part, nullptr)))
-    return rc;
   CK(cudaStreamSynchronize(c.stream));
-  make_summary(h_part[0], h_part[1], summary);
+  return MCL3DL_OK;
+}
+
+int mcl3dl_particles_get_poses(mcl3dl_engine* eng, mcl3dl_pose* out, size_t n)
+{
+  if (!eng || eng->devs.size() != 1 || !out)
+    return MCL3DL_ERR_INVALID_ARG;
+  DeviceCtx& c = eng->devs[0];
+  if (c.r_n == 0 || n != c.r_n)
+    return MCL3DL_ERR_INVALID_ARG;
+  CK(cudaSetDevice(c.dev));
+  const uint32_t n32 = static_cast<uint32_t>(n);
+  // r_poses (room for n poses since the set was sized) is the staging buffer; an update repacks it before it reads it
+  pf_poses_kernel<<<(n32 + 255) / 256, 256, 0, c.stream>>>(static_cast<const PfState*>(c.r_states[c.r_cur].p), n32,
+                                                            static_cast<mcl3dl_pose*>(c.r_poses.p));
+  CK(cudaGetLastError());
+  eng->launches++;
+  CK(cudaMemcpyAsync(out, c.r_poses.p, n * sizeof(mcl3dl_pose), cudaMemcpyDeviceToHost, c.stream));
+  CK(cudaStreamSynchronize(c.stream));
   return MCL3DL_OK;
 }
 

@@ -451,6 +451,96 @@ __device__ __forceinline__ void pf_rpy(const float rot[4], float rpy[3])
   rpy[2] = atan2f(t1, t0);
 }
 
+// ---- the landmark update of cbLandmark (src/mcl_3dl.cpp:899-940): NormalLikelihoodNd<float, 6> (nd.h:61-83) of the
+// pose difference.  nd_a and sigma_inv are the reference's a_ and sigma_inv_, computed once per message on the host.
+struct LandmarkDev
+{
+  float pos[3];          // measured.pos_
+  Q4 rot;                // measured.rot_, RAW (as the message carries it)
+  float nd_a;            // a_
+  float sigma_inv[36];   // sigma_inv_, row-major: [r * 6 + c] = sigma_inv_(r, c)
+};
+
+// -0.5 x^T S x in the order include/mcl3dl_b200.h fixes, all in float: h_k = -0.5 x_k, r_j = sum over k ascending of
+// h_k S(k, j), q = sum over j ascending of r_j x_j (each sum starts from its first product)
+__device__ __forceinline__ float pf_nd6_exponent(const float x[6], const float S[36])
+{
+  float h[6];
+#pragma unroll
+  for (int k = 0; k < 6; ++k) h[k] = fmul(-0.5f, x[k]);
+  float q = 0.0f;
+#pragma unroll
+  for (int j = 0; j < 6; ++j)
+  {
+    float r = fmul(h[0], S[j]);
+#pragma unroll
+    for (int k = 1; k < 6; ++k) r = fadd(r, fmul(h[k], S[k * 6 + j]));
+    q = j == 0 ? fmul(r, x[0]) : fadd(q, fmul(r, x[j]));
+  }
+  return q;
+}
+
+// x of one particle (cbLandmark's measure_func, src/mcl_3dl.cpp:913-926): diff = s - measured (State6DOF::operator-,
+// state_6dof.h:262-274: pos_ - measured.pos_ per axis, rot_ = measured.rot_.inv() * rot_ with both rotations RAW and
+// Quat::inv = conj * float(1.0 / dot)), x = (diff.pos_, diff.rot_.getRPY())
+__device__ __forceinline__ void pf_landmark_x(const PfState& s, const LandmarkDev& m, float x[6])
+{
+  Q4 cj;
+  cj.x = -m.rot.x;
+  cj.y = -m.rot.y;
+  cj.z = -m.rot.z;
+  cj.w = m.rot.w;
+  Q4 r;
+  r.x = s.rot[0];
+  r.y = s.rot[1];
+  r.z = s.rot[2];
+  r.w = s.rot[3];
+  const Q4 d = qmul(qdiv(cj, qdot4(m.rot, m.rot)), r);
+  const float drot[4] = {d.x, d.y, d.z, d.w};
+  for (int k = 0; k < 3; ++k) x[k] = fsub(s.pos[k], m.pos[k]);
+  pf_rpy(drot, x + 3);
+}
+
+// The likelihood of one particle: a * expf(-0.5 x^T S x) (nd.h:76-79)
+__device__ __forceinline__ float pf_landmark_likelihood(const PfState& s, const LandmarkDev& m)
+{
+  float x[6];
+  pf_landmark_x(s, m, x);
+  return fmul(m.nd_a, expf(pf_nd6_exponent(x, m.sigma_inv)));
+}
+
+// The node's integ_reset_func through pf_->predict (src/mcl_3dl.cpp:190-195,653-658): odom_err_integ_lin_ = Vec3(),
+// odom_err_integ_ang_ = Vec3()
+__device__ __forceinline__ void pf_reset_odom_err_integ(PfState& s)
+{
+#pragma unroll
+  for (int k = 0; k < 3; ++k)
+  {
+    s.lin[k] = 0.0f;
+    s.ang[k] = 0.0f;
+  }
+}
+
+// What publishParticles (src/mcl_3dl.cpp:1101-1125) publishes for one particle: the position and rot_.normalized()
+// (quat.h:175-177, q * float(1.0 / double(sqrtf(dot)))); _pad = 0
+__device__ __forceinline__ void pf_published_pose(const PfState& s, float out[8])
+{
+  Q4 r;
+  r.x = s.rot[0];
+  r.y = s.rot[1];
+  r.z = s.rot[2];
+  r.w = s.rot[3];
+  r = qnormalize4(r);
+  out[0] = s.pos[0];
+  out[1] = s.pos[1];
+  out[2] = s.pos[2];
+  out[3] = 0.0f;
+  out[4] = r.x;
+  out[5] = r.y;
+  out[6] = r.z;
+  out[7] = r.w;
+}
+
 // the terms ParticleWeightedMeanQuat::add accumulates (state_6dof.h:327-341): pos, rot * (1,0,0), rot * (0,0,1) (RAW rot)
 __device__ __forceinline__ void pf_mean_terms(const PfState& s, float out[9])
 {

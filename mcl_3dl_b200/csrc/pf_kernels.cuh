@@ -161,6 +161,43 @@ __global__ void pf_imu_kernel(const PfState* __restrict__ states, uint32_t n, Im
   rec[i] = r;
 }
 
+// cbLandmark's likelihood per particle into lik and a unit record per particle, as pf_imu_kernel
+__global__ void pf_landmark_kernel(const PfState* __restrict__ states, uint32_t n, LandmarkDev m, mcl3dl_result* __restrict__ rec,
+                                   float* __restrict__ lik)
+{
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n)
+    return;
+  lik[i] = pf_landmark_likelihood(states[i], m);
+  mcl3dl_result r;
+  r.score_like = 1.0f;
+  r.match_cnt = 0;
+  r.score_beam = 1.0f;
+  r.n_short = r.n_hit = r.n_long = 0;
+  rec[i] = r;
+}
+
+// the node's integ_reset_func through pf_->predict (src/mcl_3dl.cpp:190-195,653-658), in place
+__global__ void pf_reset_odom_err_kernel(PfState* __restrict__ states, uint32_t n)
+{
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n)
+    pf_reset_odom_err_integ(states[i]);
+}
+
+// publishParticles' poses (src/mcl_3dl.cpp:1101-1125) into out; the resident set is only read
+__global__ void pf_poses_kernel(const PfState* __restrict__ states, uint32_t n, mcl3dl_pose* __restrict__ out)
+{
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n)
+    return;
+  float p[8];
+  pf_published_pose(states[i], p);
+  float4* o = reinterpret_cast<float4*>(out + i);
+  o[0] = make_float4(p[0], p[1], p[2], p[3]);
+  o[1] = make_float4(p[4], p[5], p[6], p[7]);
+}
+
 // ---- pose estimate on the resident set (mcl3dl_particles_estimate): pf_->bias + expectationBiased + max + covariance
 // (src/mcl_3dl.cpp:428-452,704-724; pf.h:246-251,281-374).  Two passes of double sums with a fixed tree (lanes by
 // shuffles, warps and CTAs in order), so the result is deterministic; the reference sums sequentially in float, hence

@@ -113,6 +113,26 @@ class GlobalLocalizationInfo(C.Structure):
         return {k: (float if k in ("probability", "build_ms") else int)(getattr(self, k)) for k, _ in self._fields_}
 
 
+class LandmarkParams(C.Structure):
+    """mcl3dl_landmark_params: the measured pose (mcl3dl_pose as 8 floats) and NormalLikelihoodNd<float, 6>'s a_ and
+    sigma_inv_ (row-major)."""
+    _fields_ = [("measured", C.c_float * 8), ("nd_a", C.c_float), ("sigma_inv", C.c_float * 36)]
+
+
+def landmark_nd(covariance):
+    """(nd_a, sigma_inv) of NormalLikelihoodNd<float, 6> for a 6x6 covariance given as cbLandmark reads it: the 36 values
+    of the message's array taken column-major (so a non-symmetric covariance enters transposed), cast to float.  For
+    callers without Eigen: the determinant and the inverse are numpy's (LAPACK LU in double on the float matrix), so
+    these values are close to, but not, the bits Eigen's float LU gives; a node that wants the reference's values builds
+    its own NormalLikelihoodNd and reads a_ and sigma_inv_ (mcl_3dl_b200/host/lidar_measurement_model_b200.h does)."""
+    cov = np.asarray(covariance, dtype=np.float64).reshape(36)
+    sigma = cov.reshape(6, 6, order="F").astype(np.float32)
+    det = np.float32(np.linalg.det(sigma.astype(np.float64)))
+    nd_a = np.float32(1.0 / ((2.0 * np.pi) ** 3 * np.float64(np.sqrt(det))))   # nd.h: std::sqrt of the float determinant
+    sigma_inv = np.linalg.inv(sigma.astype(np.float64)).astype(np.float32)
+    return nd_a, sigma_inv
+
+
 class Estimate(C.Structure):
     """mcl3dl_estimate"""
     _fields_ = [("mean_biased", C.c_float * 8), ("max_state", C.c_float * 8), ("max_index", C.c_uint32),
@@ -137,7 +157,8 @@ EXPORTED_SYMBOLS = ["mcl3dl_measure_update", "mcl3dl_collect_stats", "mcl3dl_rea
                     "mcl3dl_particles_measure_update", "mcl3dl_particles_resample", "mcl3dl_particles_estimate", "mcl3dl_scan_prepare", "mcl3dl_scan_get",
                     "mcl3dl_particles_measure_update_prepared", "mcl3dl_match_output",
                     "mcl3dl_particles_resize", "mcl3dl_global_localization",
-                    "mcl3dl_particles_redraw_odom_noise", "mcl3dl_particles_noise", "mcl3dl_particles_imu_update"]
+                    "mcl3dl_particles_redraw_odom_noise", "mcl3dl_particles_noise", "mcl3dl_particles_imu_update",
+                    "mcl3dl_particles_landmark_update", "mcl3dl_particles_reset_odom_err_integ", "mcl3dl_particles_get_poses"]
 
 _LIBS = {}
 
@@ -192,6 +213,9 @@ def load_library(path=None):
     L.mcl3dl_particles_redraw_odom_noise.argtypes = [vp, C.c_double, C.c_double, C.c_double, C.c_double, C.c_uint64]
     L.mcl3dl_particles_noise.argtypes = [vp, vp, vp, C.c_uint64]
     L.mcl3dl_particles_imu_update.argtypes = [vp, vp, C.c_double, vp]
+    L.mcl3dl_particles_landmark_update.argtypes = [vp, vp, vp]
+    L.mcl3dl_particles_reset_odom_err_integ.argtypes = [vp]
+    L.mcl3dl_particles_get_poses.argtypes = [vp, vp, sz]
     L.mcl3dl_scan_prepare.argtypes = [vp, vp, sz, vp, vp]
     L.mcl3dl_scan_get.argtypes = [vp, C.c_int, vp, sz, C.POINTER(sz)]
     L.mcl3dl_particles_measure_update_prepared.argtypes = [vp, vp, sz, C.c_float, vp]
@@ -476,6 +500,31 @@ class Engine:
         summ = UpdateSummary()
         self._check(self.L.mcl3dl_particles_imu_update(self.h, _ptr(acc), acc_var, C.byref(summ)))
         return summ.as_dict()
+
+    def particles_landmark_update(self, measured, nd_a, sigma_inv):
+        """cbLandmark's pf_->measure on the resident set (include/mcl3dl_b200.h: mcl3dl_particles_landmark_update).
+        measured: one POSE (RAW rotation); nd_a, sigma_inv: NormalLikelihoodNd<float, 6>'s a_ and sigma_inv_ [6, 6]
+        (landmark_nd builds them from a covariance).  Returns the update summary as a dict."""
+        m = np.ascontiguousarray(measured, dtype=POSE).reshape(1)
+        si = np.ascontiguousarray(sigma_inv, dtype=np.float32)
+        assert si.size == 36
+        prm = LandmarkParams()
+        C.memmove(prm.measured, m.ctypes.data, 32)
+        prm.nd_a = nd_a
+        C.memmove(prm.sigma_inv, si.ctypes.data, 144)
+        summ = UpdateSummary()
+        self._check(self.L.mcl3dl_particles_landmark_update(self.h, C.byref(prm), C.byref(summ)))
+        return summ.as_dict()
+
+    def particles_reset_odom_err_integ(self):
+        """The node's integ_reset_func on the resident set (include/mcl3dl_b200.h: mcl3dl_particles_reset_odom_err_integ)."""
+        self._check(self.L.mcl3dl_particles_reset_odom_err_integ(self.h))
+
+    def particles_get_poses(self):
+        """publishParticles' poses: POSE [n] with normalised rotations (include/mcl3dl_b200.h: mcl3dl_particles_get_poses)."""
+        out = np.zeros(self._n_resident, dtype=POSE)
+        self._check(self.L.mcl3dl_particles_get_poses(self.h, _ptr(out), len(out)))
+        return out
 
     def particles_resize(self, num):
         """pf_->resizeParticle(num) on the resident set (include/mcl3dl_b200.h: mcl3dl_particles_resize)."""

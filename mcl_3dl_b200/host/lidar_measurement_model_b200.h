@@ -30,6 +30,7 @@
 #include <mcl_3dl/lidar_measurement_model_base.h>
 #include <mcl_3dl/lidar_measurement_models/lidar_measurement_model_beam.h>
 #include <mcl_3dl/lidar_measurement_models/lidar_measurement_model_likelihood.h>
+#include <mcl_3dl/nd.h>
 #include <mcl_3dl/parameters.h>
 #include <mcl_3dl/pf.h>
 #include <mcl_3dl/state_6dof.h>
@@ -569,9 +570,11 @@ public:
   //   pf_->predict(model) / pf_->measure(lambda) / pf_->bias + expectationBiased + max + covariance / pf_->resample(sigma)
   // (src/mcl_3dl.cpp:227-232,402-452,704-724,809-815) becomes predictResident / measureResident / estimateResident /
   // resampleResident; only scans, odometry and summaries cross the bus.  redrawOdomNoiseResident, noiseResident and
-  // imuMeasureResident replace the odometry-noise redraw, expansion resetting and cbImu's gravity update.  uploadResident()
-  // after init() / any host-side edit of particles_ (globalLocalizationResident / resizeResident replace the service body
-  // and resizeParticle), downloadResident() whenever host code needs the particles (publishParticles' markers).
+  // imuMeasureResident replace the odometry-noise redraw, expansion resetting and cbImu's gravity update;
+  // landmarkMeasureResident, resetOdomErrIntegResident and posesResident replace cbLandmark's measure, the pose-jump reset
+  // and what publishParticles reads.  uploadResident() after init() / any host-side edit of particles_
+  // (globalLocalizationResident / resizeResident replace the service body and resizeParticle), downloadResident() whenever
+  // host code needs the whole particles.
   // Documented departures (include/mcl3dl_b200.h): counter-based noise instead of the std engine's stream,
   // ties of the accumulated probability go to the lowest index, sums in double.
   static mcl3dl_state toState(const State6DOF& s)
@@ -698,6 +701,51 @@ public:
     if (s.kept)
       entropy_ = s.entropy;
     return UpdateResult{s.match_ratio_min, s.match_ratio_max, s.kept != 0};
+  }
+  // cbLandmark's NormalLikelihoodNd<float, 6> (src/mcl_3dl.cpp:901-905), built by the reference's own class from the
+  // message's 36 doubles exactly as the node builds it (Eigen maps them column-major, so a non-symmetric covariance
+  // enters transposed), read out through a derived type: a_ and sigma_inv_ (row-major).  The class templates are
+  // parameters so that only a caller compiles the Eigen code.
+  template <typename Nd = mcl_3dl::NormalLikelihoodNd<float, 6>, typename Matrix6d = Eigen::Matrix<double, 6, 6>>
+  static void landmarkNd(const double* covariance, mcl3dl_landmark_params& p)
+  {
+    struct Access : Nd
+    {
+      explicit Access(const typename Nd::Matrix& sigma) : Nd(sigma) {}
+      void read(mcl3dl_landmark_params& p) const
+      {
+        p.nd_a = this->a_;
+        for (int r = 0; r < 6; ++r)
+          for (int c = 0; c < 6; ++c) p.sigma_inv[r * 6 + c] = this->sigma_inv_(r, c);
+      }
+    };
+    Access(Matrix6d(covariance).template cast<float>()).read(p);
+  }
+  // cbLandmark's pf_->measure (src/mcl_3dl.cpp:899-931) on the resident set: measured as the node builds it from the
+  // message, covariance = msg->pose.covariance (36 doubles, e.g. its boost::array).  The states do not change.
+  template <typename Covariance>
+  UpdateResult landmarkMeasureResident(MeasurementBatcher& batcher, const State6DOF& measured, const Covariance& covariance)
+  {
+    mcl3dl_landmark_params p;
+    p.measured = mcl3dl_pose{measured.pos_.x_, measured.pos_.y_, measured.pos_.z_, 0.0f,
+                             measured.rot_.x_, measured.rot_.y_, measured.rot_.z_, measured.rot_.w_};
+    landmarkNd(covariance.data(), p);
+    mcl3dl_update_summary s;
+    batcher.checked(mcl3dl_particles_landmark_update(batcher.engine(), &p, &s), "mcl3dl_particles_landmark_update");
+    if (s.kept)
+      entropy_ = s.entropy;
+    return UpdateResult{s.match_ratio_min, s.match_ratio_max, s.kept != 0};
+  }
+  // The node's integ_reset_func through pf_->predict (the pose-jump branch, src/mcl_3dl.cpp:653-658, and cbPosition)
+  void resetOdomErrIntegResident(MeasurementBatcher& batcher)
+  {
+    batcher.checked(mcl3dl_particles_reset_odom_err_integ(batcher.engine()), "mcl3dl_particles_reset_odom_err_integ");
+  }
+  // What publishParticles (src/mcl_3dl.cpp:1101-1125) publishes: position + normalised rotation per resident particle
+  void posesResident(MeasurementBatcher& batcher, std::vector<mcl3dl_pose>& poses)
+  {
+    poses.resize(particles_.size());
+    batcher.checked(mcl3dl_particles_get_poses(batcher.engine(), poses.data(), poses.size()), "mcl3dl_particles_get_poses");
   }
   // The global_localization service body (src/mcl_3dl.cpp:1039-1099) on the device over the map index's cloud (pc_map_,
   // staged here if it is not yet): VoxelGrid, free-space filter and the div_yaw particles per seed replace the resident
