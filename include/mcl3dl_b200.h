@@ -268,8 +268,8 @@ typedef struct
   float odom_err_integ_ang[3];
 } mcl3dl_state; /* 68 bytes */
 
-/* pf_->init() happens on the host (resizeParticle and the global localisation seed have device versions below); set()
- * uploads the result (states + probability_), get() reads the set back (either pointer may be NULL). */
+/* set() uploads a set built on the host (states + probability_), get() reads the set back (either pointer may be NULL).
+ * pf_->init / initUsingNoiseGenerator, resizeParticle and the global localisation seed have device versions below. */
 int mcl3dl_particles_set(mcl3dl_engine*, const mcl3dl_state* states, const float* prob, size_t n_particles);
 int mcl3dl_particles_get(mcl3dl_engine*, mcl3dl_state* states, float* prob, size_t n_particles);
 /* pf_->predict(motion_prediction_model) for MotionPredictionModelDifferentialDrive: setOdoms(odom_prev, odom_current,
@@ -300,7 +300,8 @@ int mcl3dl_particles_resample(mcl3dl_engine*, const float sigma_pos[3], const fl
  *
  * Random numbers: the documented departure of resample, Philox-4x32-10 keyed by seed (key words = its low and high 32
  * bits), one block per counter (particle index, call count, block, event).  The event word keeps the streams apart:
- * 0 resample (blocks 0 and 1), 1 the odometry-noise redraw (block 0), 2 the expansion noise (blocks 0 and 1).  A block's
+ * 0 resample (blocks 0 and 1), 1 the odometry-noise redraw (block 0), 2 the expansion noise (blocks 0 and 1), 3 the
+ * initial seed (particles_init, blocks 0 and 1).  A block's
  * four output words w0..w3 give uniforms u(w) = float((w >> 8) + 1) * 2^-24 in (0, 1], and Box-Muller on a pair (u, v)
  * gives z = sqrtf(-2 logf(u)) * cosf(2 pi v) and z' = ... * sinf(2 pi v) (float, in that order).  Resample and the
  * expansion noise take the pairs (w0, w1), (w2, w3) of block 0 and (w0, w1) of block 1 for x, y, z, roll, pitch, yaw,
@@ -361,6 +362,43 @@ int mcl3dl_particles_reset_odom_err_integ(mcl3dl_engine*);
  * particles_get: out[i] = the position and rot.normalized() (quat.h:175-177: rot * float(1.0 / double(sqrtf(dot)))),
  * _pad = 0.  The resident set is not modified (the reference normalises a copy).  n must equal the resident count. */
 int mcl3dl_particles_get_poses(mcl3dl_engine*, mcl3dl_pose* out, size_t n);
+
+/* init: pf::ParticleFilter::initUsingNoiseGenerator(generator) (pf.h:169-181) on the device, for the configured start
+ * (MCL3dlNode::configure's pf_->init(initial_pose, initial_pose_std): DiagonalNoiseGenerator, multivariate = 0) and for
+ * cbPosition (MultivariateNoiseGenerator<float>(mean, msg->pose.covariance), multivariate = 1; src/mcl_3dl.cpp:155-198).
+ * Creates or replaces the resident set at count n (no particles_set needed; after global localisation the node passes the
+ * enlarged count, as the reference seeds particles_.size() particles).  Every particle gets probability float(1.0 /
+ * double(n)) and the state of State6DOF::generateNoise (state_6dof.h:226-248):
+ *   draws: the layout of resample's noise with event word 3: six standard normals z0..z5 (x y z roll pitch yaw) from
+ *          the pairs (w0, w1), (w2, w3) of block 0 and (w0, w1) of block 1 of Philox (particle index, call count, block,
+ *          3), z = sqrtf(-2 logf(u)) * cosf(2 pi v) and ... * sinf(2 pi v); the call count is init's own (1 on the first
+ *          call of an engine, never reset);
+ *   diagonal (DiagonalNoiseGenerator::operator(), diagonal_noise_generator.h:63-78): org_k = sigma_k == 0 ? mean_k :
+ *          z_k * sigma_k + mean_k in float (libstdc++'s normal_distribution<float>), with sigma = setSigma(State6DOF):
+ *          pos then rpy_.v_;
+ *   multivariate (multivariate_noise_generator.h:51-91): org_i = mean_i + t_i, t_i = sum over k = 0..5 of T(i, k) z_k
+ *          accumulated in float left to right from its first product, T = norm_transform_ = V sqrt(D) of the
+ *          covariance read row-major (cov(i, j) = covariance[j + i * 6]; the eigensolver reads the lower triangle).
+ *          The eigendecomposition stays on the host.  Documented departure: the fixed order of the product (Eigen's
+ *          depends on its vectorisation);
+ *   state: pos = org[0..2]; odom_err_integ_lin = org[0..2], the mean included (a reference quirk, kept);
+ *          odom_err_integ_ang = org[3..5] - mean[3..5]; rot = Quat(Vec3(org[3..5])) (setRPY, quat.h:202-215), NOT
+ *          normalised, as the reference leaves it; noise_ll/la/al/aa = 0.  cbPosition resets both integrals right
+ *          after (particles_reset_odom_err_integ); the configured start does not.
+ * Synchronous; single-device engines.  The other entry points' call counts are unchanged.  Errors, all before the set is
+ * touched: INVALID_ARG for a null engine or params, a multi-device engine, n == 0 or n >= 2^31, multivariate not 0 or 1,
+ * a non-finite mean, a diagonal sigma that is negative or not finite, or a multivariate transform entry that is not
+ * finite.  The last is a documented departure: a covariance with a negative eigenvalue gives the reference NaN
+ * particles (sqrt of a negative eigenvalue); here it is refused.  sigma is ignored when multivariate = 1, norm_transform
+ * when multivariate = 0. */
+typedef struct
+{
+  int32_t multivariate;     /* 0: DiagonalNoiseGenerator, 1: MultivariateNoiseGenerator */
+  float mean[6];            /* NoiseGeneratorBase::getMean(): x y z roll pitch yaw */
+  float sigma[6];           /* diagonal: DiagonalNoiseGenerator::sigma_ */
+  float norm_transform[36]; /* multivariate: norm_transform_, row-major [r * 6 + c] */
+} mcl3dl_init_params;
+int mcl3dl_particles_init(mcl3dl_engine*, size_t n, const mcl3dl_init_params* params, uint64_t seed);
 
 /* pf_->resizeParticle(num) (pf.h:399-436) on the resident set, as the node calls it after every update while the set is
  * larger than num_particles (src/mcl_3dl.cpp:875-888): sequential float prefix sum accum, pstep = accum_total / num in

@@ -510,6 +510,7 @@ struct DeviceCtx
   int r_cur = 0;
   uint32_t r_calls = 0;
   uint32_t r_redraw_calls = 0, r_noise_calls = 0;  // the Philox call words of the odometry-noise redraw and the expansion noise
+  uint32_t r_init_calls = 0;                        // ... and of the initial seed
   // record exchange over peer memory (one process per GPU, mcl3dl_exchange_*): [world * n_local records | world flags]
   DevBuf xchg, x_ticket;  // x_ticket: [0] completed-step counter, [1] error word (device memory, local)
   PeerTable xt{};
@@ -2548,6 +2549,49 @@ int mcl3dl_particles_get_poses(mcl3dl_engine* eng, mcl3dl_pose* out, size_t n)
   eng->launches++;
   CK(cudaMemcpyAsync(out, c.r_poses.p, n * sizeof(mcl3dl_pose), cudaMemcpyDeviceToHost, c.stream));
   CK(cudaStreamSynchronize(c.stream));
+  return MCL3DL_OK;
+}
+
+// ---- the initial seed of the resident set (pf_init_kernel): creates or replaces the set at count n
+int mcl3dl_particles_init(mcl3dl_engine* eng, size_t n, const mcl3dl_init_params* params, uint64_t seed)
+{
+  if (!eng || eng->devs.size() != 1 || !params || n == 0 || n >= (size_t(1) << 31) ||
+      (params->multivariate != 0 && params->multivariate != 1))
+    return MCL3DL_ERR_INVALID_ARG;
+  InitDev g;
+  g.multivariate = params->multivariate;
+  std::memcpy(g.mean, params->mean, sizeof(g.mean));
+  std::memcpy(g.sigma, params->sigma, sizeof(g.sigma));
+  std::memcpy(g.T, params->norm_transform, sizeof(g.T));
+  for (float v : g.mean)
+    if (!std::isfinite(v))
+      return MCL3DL_ERR_INVALID_ARG;
+  if (g.multivariate)
+  {
+    for (float v : g.T)
+      if (!std::isfinite(v))
+        return MCL3DL_ERR_INVALID_ARG;
+  }
+  else
+  {
+    for (float v : g.sigma)
+      if (!finite_nonneg(v))
+        return MCL3DL_ERR_INVALID_ARG;
+  }
+  DeviceCtx& c = eng->devs[0];
+  CK(cudaSetDevice(c.dev));
+  int rc;
+  if ((rc = reserve_resident(eng, c, n)))
+    return rc;
+  const uint32_t n32 = static_cast<uint32_t>(n);
+  ++c.r_init_calls;
+  pf_init_kernel<<<(n32 + 255) / 256, 256, 0, c.stream>>>(static_cast<PfState*>(c.r_states[0].p), static_cast<float*>(c.r_prob.p),
+                                                         n32, seed, c.r_init_calls, g);
+  CK(cudaGetLastError());
+  eng->launches++;
+  CK(cudaStreamSynchronize(c.stream));
+  c.r_n = n;
+  c.r_cur = 0;
   return MCL3DL_OK;
 }
 

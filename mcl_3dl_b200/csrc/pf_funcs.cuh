@@ -1,5 +1,5 @@
 // pf_funcs.cuh — per-particle pieces of scope row f3 (SURVEY.md §8f): motion prediction, systematic resampling, the
-// State6DOF noise and the terms of the pose estimate, as per-thread device functions called by the kernels of
+// State6DOF noise, the initial seed and the terms of the pose estimate, as per-thread device functions called by the kernels of
 // pf_kernels.cuh (the resident particle set, mcl3dl_particles_*).  They are also compiled for the host by tests/hostsim
 // and checked there against the oracle pieces that are pinned bit for bit to the reference build (tests/test_hostsim.py).
 //
@@ -205,20 +205,27 @@ __device__ __forceinline__ uint32_t pf_pick(const float* __restrict__ accum, uin
   return lo == 0 ? 0u : pf_lower_bound(accum, n, pf_pscan(pstep, initial_p, lo - 1));
 }
 
+// Quat(Vec3(rpy)) = Quat::setRPY (quat.h:202-215), rpy = (roll, pitch, yaw); not normalised
+__device__ __forceinline__ Q4 quat_rpy(const float rpy[3])
+{
+  const float t2 = cosf(fdiv(rpy[0], 2.0f)), t3 = sinf(fdiv(rpy[0], 2.0f));
+  const float t4 = cosf(fdiv(rpy[1], 2.0f)), t5 = sinf(fdiv(rpy[1], 2.0f));
+  const float t0 = cosf(fdiv(rpy[2], 2.0f)), t1 = sinf(fdiv(rpy[2], 2.0f));
+  Q4 q;
+  q.x = fsub(fmul(fmul(t0, t3), t4), fmul(fmul(t1, t2), t5));
+  q.y = fadd(fmul(fmul(t0, t2), t5), fmul(fmul(t1, t3), t4));
+  q.z = fsub(fmul(fmul(t1, t2), t4), fmul(fmul(t0, t3), t5));
+  q.w = fadd(fmul(fmul(t0, t2), t4), fmul(fmul(t1, t3), t5));
+  return q;
+}
+
 // state + generateNoise(org[0..6)): State6DOF::generateNoise / operator+ (state_6dof.h:226-261), Quat::setRPY
 // (quat.h:196-209).  org = the six draws (x y z roll pitch yaw); the noise mean is zero (DiagonalNoiseGenerator(State6DOF(),
 // sigma)).  The result is a fresh State6DOF: noise_* = 0, and rot = nrot * rot as it comes, not normalised — what
 // pf::ParticleFilter::addNoiseUsingNoiseGenerator leaves (pf.h:226-237).
 __device__ __forceinline__ PfState pf_add_noise_raw(const PfState& s, const float org[6])
 {
-  const float t2 = cosf(fdiv(org[3], 2.0f)), t3 = sinf(fdiv(org[3], 2.0f));
-  const float t4 = cosf(fdiv(org[4], 2.0f)), t5 = sinf(fdiv(org[4], 2.0f));
-  const float t0 = cosf(fdiv(org[5], 2.0f)), t1 = sinf(fdiv(org[5], 2.0f));
-  Q4 nrot;
-  nrot.x = fsub(fmul(fmul(t0, t3), t4), fmul(fmul(t1, t2), t5));
-  nrot.y = fadd(fmul(fmul(t0, t2), t5), fmul(fmul(t1, t3), t4));
-  nrot.z = fsub(fmul(fmul(t1, t2), t4), fmul(fmul(t0, t3), t5));
-  nrot.w = fadd(fmul(fmul(t0, t2), t4), fmul(fmul(t1, t3), t5));
+  const Q4 nrot = quat_rpy(org + 3);
   PfState r;
   r.noise_ll = r.noise_la = r.noise_al = r.noise_aa = 0.0f;
   for (int k = 0; k < 3; ++k)
@@ -288,26 +295,38 @@ __device__ __forceinline__ float u01(uint32_t x) { return fmul(fadd(static_cast<
 // The counter's fourth word names the event, so that the events of one seed draw from disjoint streams:
 //   (index, call, block, kPfEventResample): resampling's duplicate noise, blocks 0 and 1 (pf_noise6);
 //   (index, call, 0, kPfEventRedraw):       the odometry-noise redraw, one block = two Box-Muller pairs;
-//   (index, call, block, kPfEventNoise):    expansion resetting's noise, blocks 0 and 1, laid out as pf_noise6.
+//   (index, call, block, kPfEventNoise):    expansion resetting's noise, blocks 0 and 1, laid out as pf_noise6;
+//   (index, call, block, kPfEventInit):     the initial seed's six standard normals, blocks 0 and 1, the same layout.
 // `call` is the entry point's own call count (1 on the first call of an engine).
-constexpr uint32_t kPfEventResample = 0, kPfEventRedraw = 1, kPfEventNoise = 2;
+constexpr uint32_t kPfEventResample = 0, kPfEventRedraw = 1, kPfEventNoise = 2, kPfEventInit = 3;
 
-// six N(0, sigma_k) draws for particle `index` of call `call` of `event` (Box-Muller on three pairs)
-__device__ __forceinline__ void pf_noise6_event(uint64_t seed, uint32_t index, uint32_t call, uint32_t event, const float sigma[6],
-                                                float org[6])
+// The six standard normals of particle `index` of call `call` of `event`: the pairs (w0, w1), (w2, w3) of block 0 and
+// (w0, w1) of block 1 give rad = sqrtf(-2 logf(u)) and phi = 2 pi v, and pair p's normals are z_2p = rad * cosf(phi)
+// and z_2p+1 = rad * sinf(phi).  pair(p, rad, phi) forms them, so that a draw whose sigma is 0 needs no sine or cosine.
+template <typename Pair>
+__device__ __forceinline__ void pf_normal6_event(uint64_t seed, uint32_t index, uint32_t call, uint32_t event, Pair pair)
 {
   uint32_t a[4] = {index, call, 0u, event}, b[4] = {index, call, 1u, event};
   const uint32_t k0 = static_cast<uint32_t>(seed), k1 = static_cast<uint32_t>(seed >> 32);
   philox4x32_10(a, k0, k1);
   philox4x32_10(b, k0, k1);
   const uint32_t w[6] = {a[0], a[1], a[2], a[3], b[0], b[1]};
-  for (int pair = 0; pair < 3; ++pair)
+  for (int p = 0; p < 3; ++p)
   {
-    const float rad = __fsqrt_rn(fmul(-2.0f, logf(u01(w[2 * pair]))));
-    const float phi = fmul(6.283185307179586f, u01(w[2 * pair + 1]));
+    const float rad = __fsqrt_rn(fmul(-2.0f, logf(u01(w[2 * p]))));
+    const float phi = fmul(6.283185307179586f, u01(w[2 * p + 1]));
+    pair(p, rad, phi);
+  }
+}
+
+// six N(0, sigma_k) draws for particle `index` of call `call` of `event` (Box-Muller on three pairs)
+__device__ __forceinline__ void pf_noise6_event(uint64_t seed, uint32_t index, uint32_t call, uint32_t event, const float sigma[6],
+                                                float org[6])
+{
+  pf_normal6_event(seed, index, call, event, [&](int pair, float rad, float phi) {
     org[2 * pair] = sigma[2 * pair] == 0.0f ? 0.0f : fmul(fmul(rad, cosf(phi)), sigma[2 * pair]);
     org[2 * pair + 1] = sigma[2 * pair + 1] == 0.0f ? 0.0f : fmul(fmul(rad, sinf(phi)), sigma[2 * pair + 1]);
-  }
+  });
 }
 
 // resampling's draws for output particle `index` of resampling call `call`
@@ -349,6 +368,61 @@ __device__ __forceinline__ PfState pf_expansion_noise(const PfState& s, uint64_t
   float org[6];
   pf_noise6_event(seed, index, call, kPfEventNoise, sigma, org);
   return pf_add_noise_raw(s, org);
+}
+
+// ---- the initial seed: pf::ParticleFilter::initUsingNoiseGenerator (pf.h:169-181) with the configured start's
+// DiagonalNoiseGenerator or cbPosition's MultivariateNoiseGenerator.  mean = NoiseGeneratorBase::getMean() (x y z roll
+// pitch yaw, setMean's getRPY on the host); sigma = DiagonalNoiseGenerator::sigma_; T = norm_transform_ (row-major).
+struct InitDev
+{
+  int multivariate;  // 0: diagonal, 1: multivariate
+  float mean[6];
+  float sigma[6];
+  float T[36];
+};
+
+// State6DOF::generateNoise (state_6dof.h:226-248) for particle `index` of init call `call`, from six standard normals z:
+//   diagonal:     org_k = sigma_k == 0 ? mean_k : z_k * sigma_k + mean_k (libstdc++'s normal_distribution<float>);
+//   multivariate: org_i = mean_i + t_i, t_i = sum over k ascending of T(i, k) z_k from its first product.
+// pos = org[0..2], odom_err_integ_lin = org[0..2] (the mean included, as the reference leaves it), odom_err_integ_ang =
+// org[3..5] - mean[3..5], rot = Quat(Vec3(org[3..5])) not normalised, noise_* = 0.
+__device__ __forceinline__ PfState pf_init_state(uint64_t seed, uint32_t index, uint32_t call, const InitDev& g)
+{
+  float z[6], org[6];
+  pf_normal6_event(seed, index, call, kPfEventInit, [&](int pair, float rad, float phi) {
+    z[2 * pair] = fmul(rad, cosf(phi));
+    z[2 * pair + 1] = fmul(rad, sinf(phi));
+  });
+  if (g.multivariate)
+  {
+#pragma unroll
+    for (int i = 0; i < 6; ++i)
+    {
+      float t = fmul(g.T[i * 6], z[0]);
+#pragma unroll
+      for (int k = 1; k < 6; ++k) t = fadd(t, fmul(g.T[i * 6 + k], z[k]));
+      org[i] = fadd(g.mean[i], t);
+    }
+  }
+  else
+  {
+#pragma unroll
+    for (int k = 0; k < 6; ++k) org[k] = g.sigma[k] == 0.0f ? g.mean[k] : fadd(fmul(z[k], g.sigma[k]), g.mean[k]);
+  }
+  PfState r;
+  r.noise_ll = r.noise_la = r.noise_al = r.noise_aa = 0.0f;
+  for (int k = 0; k < 3; ++k)
+  {
+    r.pos[k] = org[k];
+    r.lin[k] = org[k];
+    r.ang[k] = fsub(org[k + 3], g.mean[k + 3]);
+  }
+  const Q4 rot = quat_rpy(org + 3);
+  r.rot[0] = rot.x;
+  r.rot[1] = rot.y;
+  r.rot[2] = rot.z;
+  r.rot[3] = rot.w;
+  return r;
 }
 
 // ---- IMU gravity update: ImuMeasurementModelGravity::setAccMeasure + measure (imu_measurement_model_gravity.h:45-55)

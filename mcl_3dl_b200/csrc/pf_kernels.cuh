@@ -144,6 +144,17 @@ __global__ void pf_noise_kernel(PfState* __restrict__ states, uint32_t n, uint64
     states[i] = pf_expansion_noise(states[i], seed, i, call, sigma.v);
 }
 
+// pf_->initUsingNoiseGenerator(generator) (pf.h:169-181): every particle's seed and probability float(1.0 / double(n))
+__global__ void pf_init_kernel(PfState* __restrict__ states, float* __restrict__ probs, uint32_t n, uint64_t seed, uint32_t call,
+                               InitDev g)
+{
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n)
+    return;
+  states[i] = pf_init_state(seed, i, call, g);
+  probs[i] = __double2float_rn(ddiv(1.0, static_cast<double>(n)));
+}
+
 // The IMU gravity likelihood per particle into lik, and a unit record (score_beam = score_like = 1, match_cnt = 0) per
 // particle, so that pass 1 of the weight fold computes prior * lik with the extra factor
 __global__ void pf_imu_kernel(const PfState* __restrict__ states, uint32_t n, ImuDev m, mcl3dl_result* __restrict__ rec,

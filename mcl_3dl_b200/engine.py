@@ -133,6 +133,26 @@ def landmark_nd(covariance):
     return nd_a, sigma_inv
 
 
+class InitParams(C.Structure):
+    """mcl3dl_init_params: the generator of the initial seed (diagonal sigma_ or multivariate norm_transform_, row-major)."""
+    _fields_ = [("multivariate", C.c_int32), ("mean", C.c_float * 6), ("sigma", C.c_float * 6),
+                ("norm_transform", C.c_float * 36)]
+
+
+def noise_transform(covariance):
+    """norm_transform_ of MultivariateNoiseGenerator<float> for cbPosition's covariance: the 36 values of the message's
+    array read row-major (cov(i, j) = covariance[j + i * 6]), cast to float, only the lower triangle read, then
+    V * sqrt(D) of the eigendecomposition, as float32 [6, 6].  For callers without Eigen: the eigendecomposition is
+    numpy's (LAPACK in double on the float matrix), so these values are close to, but not, the bits Eigen's float
+    SelfAdjointEigenSolver gives, and the order of the eigenvectors may differ; a node that wants the reference's values
+    builds its own MultivariateNoiseGenerator and reads norm_transform_ (mcl_3dl_b200/host/lidar_measurement_model_b200.h
+    does).  A negative eigenvalue gives NaN entries, which particles_init refuses."""
+    cov = np.asarray(covariance, dtype=np.float64).reshape(6, 6).astype(np.float32).astype(np.float64)
+    w, v = np.linalg.eigh(cov, UPLO="L")
+    with np.errstate(invalid="ignore"):
+        return (v * np.sqrt(w)).astype(np.float32)
+
+
 class Estimate(C.Structure):
     """mcl3dl_estimate"""
     _fields_ = [("mean_biased", C.c_float * 8), ("max_state", C.c_float * 8), ("max_index", C.c_uint32),
@@ -158,7 +178,8 @@ EXPORTED_SYMBOLS = ["mcl3dl_measure_update", "mcl3dl_collect_stats", "mcl3dl_rea
                     "mcl3dl_particles_measure_update_prepared", "mcl3dl_match_output",
                     "mcl3dl_particles_resize", "mcl3dl_global_localization",
                     "mcl3dl_particles_redraw_odom_noise", "mcl3dl_particles_noise", "mcl3dl_particles_imu_update",
-                    "mcl3dl_particles_landmark_update", "mcl3dl_particles_reset_odom_err_integ", "mcl3dl_particles_get_poses"]
+                    "mcl3dl_particles_landmark_update", "mcl3dl_particles_reset_odom_err_integ", "mcl3dl_particles_get_poses",
+                    "mcl3dl_particles_init"]
 
 _LIBS = {}
 
@@ -216,6 +237,7 @@ def load_library(path=None):
     L.mcl3dl_particles_landmark_update.argtypes = [vp, vp, vp]
     L.mcl3dl_particles_reset_odom_err_integ.argtypes = [vp]
     L.mcl3dl_particles_get_poses.argtypes = [vp, vp, sz]
+    L.mcl3dl_particles_init.argtypes = [vp, sz, vp, C.c_uint64]
     L.mcl3dl_scan_prepare.argtypes = [vp, vp, sz, vp, vp]
     L.mcl3dl_scan_get.argtypes = [vp, C.c_int, vp, sz, C.POINTER(sz)]
     L.mcl3dl_particles_measure_update_prepared.argtypes = [vp, vp, sz, C.c_float, vp]
@@ -453,6 +475,28 @@ class Engine:
         assert len(states) == len(prob)
         self._check(self.L.mcl3dl_particles_set(self.h, _ptr(states), _ptr(prob), len(states)))
         self._n_resident = len(states)
+
+    def particles_init(self, n, mean6, seed, sigma=None, norm_transform=None):
+        """pf_->initUsingNoiseGenerator on the device (include/mcl3dl_b200.h: mcl3dl_particles_init): creates or replaces
+        the resident set with n particles.  mean6 = the generator's mean (x y z roll pitch yaw); exactly one of sigma (6,
+        DiagonalNoiseGenerator) and norm_transform ([6, 6], MultivariateNoiseGenerator; noise_transform builds it from a
+        covariance) is given."""
+        assert (sigma is None) != (norm_transform is None)
+        prm = InitParams()
+        prm.multivariate = 0 if norm_transform is None else 1
+        m = np.ascontiguousarray(mean6, dtype=np.float32)
+        assert m.size == 6
+        C.memmove(prm.mean, m.ctypes.data, 24)
+        if sigma is not None:
+            sg = np.ascontiguousarray(sigma, dtype=np.float32)
+            assert sg.size == 6
+            C.memmove(prm.sigma, sg.ctypes.data, 24)
+        else:
+            t = np.ascontiguousarray(norm_transform, dtype=np.float32)
+            assert t.size == 36
+            C.memmove(prm.norm_transform, t.ctypes.data, 144)
+        self._check(self.L.mcl3dl_particles_init(self.h, n, C.byref(prm), seed))
+        self._n_resident = int(n)
 
     def particles_get(self):
         states = np.zeros(self._n_resident, dtype=STATE)

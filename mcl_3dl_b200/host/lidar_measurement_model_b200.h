@@ -19,6 +19,7 @@
 #define MCL_3DL_B200_LIDAR_MEASUREMENT_MODEL_B200_H
 
 #include <algorithm>
+#include <cmath>
 #include <cstring>
 #include <memory>
 #include <random>
@@ -36,6 +37,14 @@
 #include <mcl_3dl/state_6dof.h>
 
 #include "mcl3dl_b200.h"
+
+namespace mcl_3dl
+{
+// include/mcl_3dl/noise_generators/multivariate_noise_generator.h (Eigen's eigensolver): a caller of
+// initUsingCovarianceResident includes it; nothing else here needs it
+template <typename FLT_TYPE>
+class MultivariateNoiseGenerator;
+}  // namespace mcl_3dl
 
 namespace mcl_3dl_b200
 {
@@ -572,9 +581,10 @@ public:
   // resampleResident; only scans, odometry and summaries cross the bus.  redrawOdomNoiseResident, noiseResident and
   // imuMeasureResident replace the odometry-noise redraw, expansion resetting and cbImu's gravity update;
   // landmarkMeasureResident, resetOdomErrIntegResident and posesResident replace cbLandmark's measure, the pose-jump reset
-  // and what publishParticles reads.  uploadResident() after init() / any host-side edit of particles_
-  // (globalLocalizationResident / resizeResident replace the service body and resizeParticle), downloadResident() whenever
-  // host code needs the whole particles.
+  // and what publishParticles reads; initResident and initUsingCovarianceResident replace pf_->init and cbPosition's
+  // initUsingNoiseGenerator.  uploadResident() after any host-side edit of particles_ (globalLocalizationResident /
+  // resizeResident replace the service body and resizeParticle), downloadResident() whenever host code needs the whole
+  // particles.
   // Documented departures (include/mcl3dl_b200.h): counter-based noise instead of the std engine's stream,
   // ties of the accumulated probability go to the lowest index, sums in double.
   static mcl3dl_state toState(const State6DOF& s)
@@ -746,6 +756,63 @@ public:
   {
     poses.resize(particles_.size());
     batcher.checked(mcl3dl_particles_get_poses(batcher.engine(), poses.data(), poses.size()), "mcl3dl_particles_get_poses");
+  }
+  // pf_->init(mean, sigma) (pf.h:169-172; the configured start, src/mcl_3dl.cpp:1276) on the device: the reference's own
+  // DiagonalNoiseGenerator<float>(mean, sigma) gives getMean() (setMean's getRPY) and sigma_, read through a derived
+  // type; particles_.size() particles are seeded.  particles_ is stale until downloadResident().
+  template <typename Gen = mcl_3dl::DiagonalNoiseGenerator<float>>
+  void initResident(MeasurementBatcher& batcher, const State6DOF& mean, const State6DOF& sigma, uint64_t seed)
+  {
+    struct Access : Gen
+    {
+      Access(const State6DOF& m, const State6DOF& s) : Gen(m, s) {}
+      void read(mcl3dl_init_params& p) const
+      {
+        for (int k = 0; k < 6; ++k)
+        {
+          p.mean[k] = this->getMean()[k];
+          p.sigma[k] = this->sigma_[k];
+        }
+      }
+    };
+    mcl3dl_init_params p{};
+    p.multivariate = 0;
+    Access(mean, sigma).read(p);
+    batcher.checked(mcl3dl_particles_init(batcher.engine(), particles_.size(), &p, seed), "mcl3dl_particles_init");
+  }
+  // cbPosition's pf_->initUsingNoiseGenerator(MultivariateNoiseGenerator<float>(mean, msg->pose.covariance))
+  // (src/mcl_3dl.cpp:189-190) on the device: the reference's own generator (its eigendecomposition on the host) gives
+  // mean_vec_ and norm_transform_, read through a derived type.  covariance = the message's 36 doubles, read row-major as
+  // the generator reads them.  Returns false, the resident set as it was, when norm_transform_ is not finite (a
+  // covariance with a negative eigenvalue).  The class template is a parameter, so only a caller compiles the Eigen
+  // code; it includes <mcl_3dl/noise_generators/multivariate_noise_generator.h>.
+  template <typename Covariance, typename Gen = mcl_3dl::MultivariateNoiseGenerator<float>>
+  bool initUsingCovarianceResident(MeasurementBatcher& batcher, const State6DOF& mean, const Covariance& covariance, uint64_t seed)
+  {
+    struct Access : Gen
+    {
+      Access(const State6DOF& m, const Covariance& c) : Gen(m, c) {}
+      bool read(mcl3dl_init_params& p) const
+      {
+        bool finite = true;
+        for (int r = 0; r < 6; ++r)
+        {
+          p.mean[r] = this->mean_vec_[r];
+          for (int c = 0; c < 6; ++c)
+          {
+            p.norm_transform[r * 6 + c] = this->norm_transform_(r, c);
+            finite = finite && std::isfinite(p.norm_transform[r * 6 + c]);
+          }
+        }
+        return finite;
+      }
+    };
+    mcl3dl_init_params p{};
+    p.multivariate = 1;
+    if (!Access(mean, covariance).read(p))
+      return false;
+    batcher.checked(mcl3dl_particles_init(batcher.engine(), particles_.size(), &p, seed), "mcl3dl_particles_init");
+    return true;
   }
   // The global_localization service body (src/mcl_3dl.cpp:1039-1099) on the device over the map index's cloud (pc_map_,
   // staged here if it is not yet): VoxelGrid, free-space filter and the div_yaw particles per seed replace the resident
