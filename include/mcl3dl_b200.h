@@ -500,6 +500,70 @@ int mcl3dl_scan_get(mcl3dl_engine*, int which, mcl3dl_point* out, size_t capacit
 int mcl3dl_particles_measure_update_prepared(mcl3dl_engine*, const float* origins_xyz, size_t n_origins,
                                              float odom_err_integ_lin_sigma, mcl3dl_update_summary* summary);
 
+/* The node's second sampler, PointCloudSamplerWithNormal (use_random_sampler_with_normal; point_cloud_random_samplers/
+ * point_cloud_sampler_with_normal.h), on the clipped clouds the last mcl3dl_scan_prepare left on the device, once per
+ * model.  It REPLACES that call's sampled scans (scan_get(3 | 4), particles_measure_update_prepared); the downsampled and
+ * clipped clouds, the resident set, the staged map and the exchange buffers are untouched.
+ *   Statistics (setParticleStatistics, :75-89): the caller passes SelfAdjointEigenSolver(|3 x 3 position block of
+ *   covariance|)'s eigenvalues (ascending) and its eigenvector column 2, and expectation().rot_ raw.  On the host, in the
+ *   reference's operation order: ratio = sqrt(l2 / l1); max_weight = 1 below perform_weighting_ratio, max_weight above
+ *   max_weight_ratio, linear in between (double); fpc_local = mean_rot.inv() * Vec3(float(v)) (float Quat arithmetic).
+ *   1. clipped <= num: the whole clipped cloud, in order, no draws; clipped == 0 or num == 0: empty.
+ *   2. Normals (pcl::NormalEstimation with a fresh isotropic KdTree and radius r = normal_search_range), restated: the
+ *      neighbours of a finite point q are every finite point p with flann::L2_Simple d2 < float(double r * r), q
+ *      included, found in a grid of cell edge r (1 + 2^-10) (more margin for coordinates beyond ~8000 cells, so that
+ *      the float cell index always keeps a neighbour within one cell); count, sum d and sum d d^T (d = p - q) in
+ *      double, C = S / n - m m^T, the normal is the unit eigenvector of C's smallest eigenvalue from ten cyclic Jacobi
+ *      sweeps in double, stored as float.  Fewer than 3 neighbours or a non-finite point: a NaN normal.  Its sign is
+ *      unspecified; the weight takes |.|.
+ *   3. Weight w = 1 + (max_weight - 1) ((pi/2 - acos(a)) / (pi/2)), a = min(1, |nx fx + ny fy + nz fz|) (float products
+ *      and sums, widened to double; acos in double from +, -, *, /, sqrt), a NaN normal: 1.
+ *   4. Fixed-point weights q = max(1, rint(w 2^F)), F = 32 - ceil(log2(max(1, max_weight))), and their exact uint64
+ *      inclusive sum.
+ *   5. Draw t of stream s (0 likelihood, 1 beam): Philox-4x32-10 keyed by the seed's two words at counter
+ *      (t mod 2^32, s, 0x6e6f726d, t >> 32), r = high 64 bits of (w0 | w1 << 32) * total, index = the first i with
+ *      cum_i > r (probability q_i / total).  Output j = the point of the j-th draw, in draw order, whose index was not
+ *      drawn before; the draws stop at num outputs.  Draws run in rounds (the host reads one word per round); at most
+ *      2^32 draws are made.  The expected number needed is at most n rho H_n (rho = max q / min q <= max(max_weight,
+ *      1 / max_weight)), below 10^8 for the node's parameters and a million clipped points; a call that reaches the cap
+ *      returns the points found so far (n_lik / n_beam < num) with draws = 2^32.
+ * Documented departures: the normals are "parity unpinned" (PCL's NormalEstimation and eigen33 are third-party and
+ * absent here; the restatement uses exact neighbour sets, a double covariance and a double eigen routine); Philox instead
+ * of std::default_random_engine; output in first-draw order instead of std::unordered_set order; weights rounded to
+ * 2^-F; a non-finite max_weight (l1 = l2 = 0, or a ratio exactly equal to equal thresholds: the reference's cumulative
+ * weights are NaN there, its result undefined) becomes 1, uniform weights.  The normals and weights of both clipped
+ * clouds are computed on every call (mcl3dl_scan_normals reads them), whatever num is.
+ * Errors, all before any state changes (the previous samples stay valid): INVALID_ARG for a null engine or params, a
+ * multi-device engine, no scan_prepare before, normal_search_range <= 0 or not finite, max_weight <= 0 or not finite,
+ * or a non-finite ratio parameter, eigen value / vector entry or mean_rot entry; TOO_LARGE when a clipped cloud's
+ * neighbour grid would need 2^31 cells or more (outliers in an unbounded clip window).  Synchronous; single-device. */
+typedef struct
+{
+  double perform_weighting_ratio, max_weight_ratio, max_weight, normal_search_range; /* PointCloudSamplerWithNormalParameters */
+  double eigen_values[3]; /* SelfAdjointEigenSolver(|pos cov|).eigenvalues(), ascending */
+  double eigen_vector[3]; /* .eigenvectors().col(2) */
+  float mean_rot[4];      /* expectation().rot_, raw, x y z w */
+  uint32_t lik_num_points, beam_num_points;
+  uint64_t seed;
+} mcl3dl_normal_sampler_params;
+typedef struct
+{
+  uint32_t n_lik, n_beam;   /* sample sizes: min(num, clipped count) */
+  uint32_t n_normal[2];     /* clipped points with a finite normal (lik, beam) */
+  uint32_t rounds[2];       /* draw rounds (0 when no draw was needed) */
+  uint64_t draws[2];        /* draws made */
+  double max_weight;        /* after step 2 and the non-finite rule */
+  float fpc_local[3];
+  int32_t weight_shift;     /* F of the fixed-point weights */
+} mcl3dl_normal_sampler_info;
+int mcl3dl_scan_sample_with_normal(mcl3dl_engine*, const mcl3dl_normal_sampler_params*, mcl3dl_normal_sampler_info* info);
+/* Diagnostics of the last mcl3dl_scan_sample_with_normal, per clipped point of model `which` (0 likelihood, 1 beam), in
+ * clipped order: the normal (3 floats, NaN where none), the neighbour count and the fixed-point weight q.  Each output
+ * pointer may be NULL; *n_out = the clipped count.  INVALID_ARG with no such call since the last scan_prepare, a bad
+ * `which`, or an output pointer with capacity below the count. */
+int mcl3dl_scan_normals(mcl3dl_engine*, int which, float* normals_xyz, uint32_t* n_neighbours, uint64_t* weights_q, size_t capacity,
+                        size_t* n_out);
+
 /* ---- Matched / unmatched output (src/mcl_3dl.cpp:761-805): the scan transformed by the pose estimate e
  * (State6DOF::transform, normalised rotation) and split by kdtree_->radiusSearch(p, unmatch_output_dist, id, sqdist, 1)
  * on the map index ChunkedKdtree(chunk_length, max_search_radius):

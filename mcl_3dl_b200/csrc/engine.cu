@@ -500,6 +500,12 @@ struct DeviceCtx
   DevBuf s_raw, s_keys[2], s_vals[2], s_key_label[2], s_flags[2], s_pos[2], s_ds, s_clip[2], s_out[2], s_tmp, s_counts;
   mcl3dl_scan_info s_info{};
   bool s_valid = false;
+  // normal-weighted sampler (mcl3dl_scan_sample_with_normal): neighbour-grid sort keys / values (x2), sorted points; per
+  // model the normals, neighbour counts and fixed-point weights of its clipped points (mcl3dl_scan_normals); the inclusive
+  // sum of the weights, each point's first draw, a round's draw indices / flags / scan positions, the new sampled scans,
+  // cub scratch, device-side words (bounding boxes, finite-normal counts, the round's carry)
+  DevBuf n_keys[2], n_vals[2], n_spts, n_normals[2], n_nb[2], n_q[2], n_cum, n_first, n_didx, n_dflag, n_dpos, n_out[2], n_tmp, n_word;
+  bool n_valid = false;
   // matched / unmatched output (mcl3dl_match_output), kept apart from the prepared scans it may read: host cloud,
   // transformed cloud, flags + scan positions per output, cub scratch; the page-locked block the compaction writes
   // both clouds and their counts into
@@ -1645,6 +1651,100 @@ int voxel_grid(mcl3dl_engine* eng, DeviceCtx& c, cudaStream_t st, const mcl3dl_p
   CK(cudaGetLastError());
   eng->launches += 6;
   done = true;
+  return MCL3DL_OK;
+}
+
+// PointCloudSamplerWithNormal on the clipped cloud k (n points, grid ng / end_bit checked by the caller): the normals,
+// neighbour counts and fixed-point weights into n_normals[k] / n_nb[k] / n_q[k], then the distinct weighted draws into
+// n_out[k] (include/mcl3dl_b200.h: mcl3dl_scan_sample_with_normal).  *n_sample, *rounds and *draws as the info reports.
+constexpr uint64_t kNsMaxDraws = uint64_t(1) << 32;  // the documented cap on the draws of one call and model
+constexpr uint32_t kNsMaxRound = 1u << 22;           // draws per round, at most
+int ns_sample_model(mcl3dl_engine* eng, DeviceCtx& c, int k, uint32_t n, const NsGridDev& ng, int end_bit, const float fpc[3],
+                    double max_weight, double scale, uint32_t num, uint64_t seed, uint32_t* n_sample, uint32_t* rounds, uint64_t* draws)
+{
+  cudaStream_t st = c.stream;
+  int rc;
+  *n_sample = 0;
+  *rounds = 0;
+  *draws = 0;
+  const size_t cap = std::max<size_t>(n, 1);
+  if ((rc = reserve(eng, c.n_normals[k], cap * 12)) || (rc = reserve(eng, c.n_nb[k], cap * 4)) || (rc = reserve(eng, c.n_q[k], cap * 8)) ||
+      (rc = reserve(eng, c.n_out[k], std::max<size_t>(std::min<size_t>(num, n), 1) * 16)))
+    return rc;
+  if (n == 0)
+    return MCL3DL_OK;
+  for (int b = 0; b < 2; ++b)
+    if ((rc = reserve(eng, c.n_keys[b], cap * 4)) || (rc = reserve(eng, c.n_vals[b], cap * 4)))
+      return rc;
+  if ((rc = reserve(eng, c.n_spts, cap * 16)) || (rc = reserve(eng, c.n_cum, cap * 8)))
+    return rc;
+  const mcl3dl_point* clipped = static_cast<const mcl3dl_point*>(c.s_clip[k].p);
+  uint32_t* word = static_cast<uint32_t*>(c.n_word.p);  // [0, 12) bounding boxes, [12 + k] finite normals, [14] carry
+  uint32_t *k0 = static_cast<uint32_t*>(c.n_keys[0].p), *k1 = static_cast<uint32_t*>(c.n_keys[1].p);
+  uint32_t *v0 = static_cast<uint32_t*>(c.n_vals[0].p), *v1 = static_cast<uint32_t*>(c.n_vals[1].p);
+  mcl3dl_point* spts = static_cast<mcl3dl_point*>(c.n_spts.p);
+  uint64_t* q = static_cast<uint64_t*>(c.n_q[k].p);
+  uint64_t* cum = static_cast<uint64_t*>(c.n_cum.p);
+  const int nb = static_cast<int>((n + 255) / 256);
+  ns_key_kernel<<<nb, 256, 0, st>>>(clipped, n, ng.g, k0, v0);
+  size_t t_sort = 0, t_scan = 0;
+  CK(cub::DeviceRadixSort::SortPairs(nullptr, t_sort, k0, k1, v0, v1, n, 0, end_bit, st));
+  CK(cub::DeviceScan::InclusiveSum(nullptr, t_scan, q, cum, static_cast<int>(n), st));
+  if ((rc = reserve(eng, c.n_tmp, std::max(t_sort, t_scan) + 256)))
+    return rc;
+  size_t tsz = c.n_tmp.cap;
+  CK(cub::DeviceRadixSort::SortPairs(c.n_tmp.p, tsz, k0, k1, v0, v1, n, 0, end_bit, st));  // stable: ascending index in a cell
+  ns_gather_kernel<<<nb, 256, 0, st>>>(clipped, v1, n, spts);
+  ns_normal_kernel<<<static_cast<int>((n + 127) / 128), 128, 0, st>>>(clipped, n, ng, k1, spts, fpc[0], fpc[1], fpc[2], max_weight, scale,
+                                                                     static_cast<float*>(c.n_normals[k].p),
+                                                                     static_cast<uint32_t*>(c.n_nb[k].p), q, word + 12 + k);
+  tsz = c.n_tmp.cap;
+  CK(cub::DeviceScan::InclusiveSum(c.n_tmp.p, tsz, q, cum, static_cast<int>(n), st));  // exact: the total stays below 2^62
+  CK(cudaGetLastError());
+  eng->launches += 5;
+  mcl3dl_point* out = static_cast<mcl3dl_point*>(c.n_out[k].p);
+  if (num == 0)
+    return MCL3DL_OK;
+  if (n <= num)  // the whole clipped cloud, in order
+  {
+    CK(cudaMemcpyAsync(out, clipped, static_cast<size_t>(n) * 16, cudaMemcpyDeviceToDevice, st));
+    *n_sample = n;
+    return MCL3DL_OK;
+  }
+  if ((rc = reserve(eng, c.n_first, cap * 8)))
+    return rc;
+  unsigned long long* first = static_cast<unsigned long long*>(c.n_first.p);
+  CK(cudaMemsetAsync(first, 0xff, static_cast<size_t>(n) * 8, st));
+  const uint64_t r0 = std::max<uint64_t>(2048, 2 * static_cast<uint64_t>(num));
+  uint32_t carry = 0;
+  uint64_t d0 = 0;
+  while (carry < num && d0 < kNsMaxDraws)
+  {
+    const uint32_t cnt = static_cast<uint32_t>(std::min(std::min(r0 << std::min<uint32_t>(*rounds, 16), uint64_t(kNsMaxRound)), kNsMaxDraws - d0));
+    if ((rc = reserve(eng, c.n_didx, size_t(cnt) * 4)) || (rc = reserve(eng, c.n_dflag, size_t(cnt) * 4)) ||
+        (rc = reserve(eng, c.n_dpos, size_t(cnt) * 4)))
+      return rc;
+    uint32_t *didx = static_cast<uint32_t*>(c.n_didx.p), *flags = static_cast<uint32_t*>(c.n_dflag.p), *pos = static_cast<uint32_t*>(c.n_dpos.p);
+    const int db = static_cast<int>((cnt + 255) / 256);
+    ns_draw_kernel<<<db, 256, 0, st>>>(cum, n, seed, static_cast<uint32_t>(k), d0, cnt, didx, first);
+    ns_first_flag_kernel<<<db, 256, 0, st>>>(didx, first, d0, cnt, flags);
+    size_t t_pos = 0;
+    CK(cub::DeviceScan::ExclusiveSum(nullptr, t_pos, flags, pos, static_cast<int>(cnt), st));
+    if ((rc = reserve(eng, c.n_tmp, t_pos + 256)))
+      return rc;
+    tsz = c.n_tmp.cap;
+    CK(cub::DeviceScan::ExclusiveSum(c.n_tmp.p, tsz, flags, pos, static_cast<int>(cnt), st));
+    ns_take_kernel<<<db, 256, 0, st>>>(clipped, didx, flags, pos, cnt, carry, num, out, word + 14);
+    CK(cudaGetLastError());
+    eng->launches += 4;
+    CK(cudaMemcpyAsync(c.h_pinned.p, word + 14, 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    std::memcpy(&carry, c.h_pinned.p, 4);
+    d0 += cnt;
+    ++*rounds;
+  }
+  *draws = d0;
+  *n_sample = std::min(carry, num);
   return MCL3DL_OK;
 }
 }  // namespace
@@ -2893,6 +2993,7 @@ int mcl3dl_scan_prepare(mcl3dl_engine* eng, const mcl3dl_point* raw, size_t n_ra
   CK(cudaSetDevice(c.dev));
   cudaStream_t st = c.stream;
   c.s_valid = false;
+  c.n_valid = false;
   c.s_info = mcl3dl_scan_info{};
   c.s_info.n_raw = static_cast<uint32_t>(n_raw);
   const uint32_t n = static_cast<uint32_t>(n_raw);
@@ -2989,6 +3090,111 @@ int mcl3dl_scan_get(mcl3dl_engine* eng, int which, mcl3dl_point* out, size_t cap
     return MCL3DL_ERR_INVALID_ARG;
   CK(cudaSetDevice(c.dev));
   CK(cudaMemcpyAsync(out, src[which]->p, static_cast<size_t>(n[which]) * 16, cudaMemcpyDeviceToHost, c.stream));
+  CK(cudaStreamSynchronize(c.stream));
+  return MCL3DL_OK;
+}
+
+// ---- PointCloudSamplerWithNormal on the prepared clipped clouds (scan_kernels.cuh: ns_*_kernel)
+int mcl3dl_scan_sample_with_normal(mcl3dl_engine* eng, const mcl3dl_normal_sampler_params* p, mcl3dl_normal_sampler_info* info)
+{
+  if (!eng || !p || eng->devs.size() != 1)
+    return MCL3DL_ERR_INVALID_ARG;
+  DeviceCtx& c = eng->devs[0];
+  if (!c.s_valid)
+    return MCL3DL_ERR_INVALID_ARG;  // no mcl3dl_scan_prepare before
+  const double r = p->normal_search_range;
+  bool ok = std::isfinite(r) && r > 0.0 && std::isfinite(p->max_weight) && p->max_weight > 0.0 &&
+            std::isfinite(p->perform_weighting_ratio) && std::isfinite(p->max_weight_ratio);
+  for (int k = 0; k < 3; ++k)
+    ok = ok && std::isfinite(p->eigen_values[k]) && std::isfinite(p->eigen_vector[k]);
+  for (int k = 0; k < 4; ++k)
+    ok = ok && std::isfinite(p->mean_rot[k]);
+  if (!ok)
+    return MCL3DL_ERR_INVALID_ARG;
+  mcl3dl_normal_sampler_info out{};
+  int shift = 0;
+  ns_host_consts(*p, &out.max_weight, out.fpc_local, &shift);
+  out.weight_shift = shift;
+  const double scale = std::ldexp(1.0, shift);
+  CK(cudaSetDevice(c.dev));
+  cudaStream_t st = c.stream;
+  const uint32_t n[2] = {c.s_info.n_lik_clipped, c.s_info.n_beam_clipped};
+  const uint32_t num[2] = {p->lik_num_points, p->beam_num_points};
+  int rc;
+  if ((rc = reserve(eng, c.n_word, 256)) || (rc = reserve(eng, c.h_pinned, 256)))
+    return rc;
+  uint32_t* word = static_cast<uint32_t*>(c.n_word.p);
+  // both clouds' neighbour grids first, so that TOO_LARGE leaves everything as it was
+  uint32_t h_bbox[12];
+  for (int k = 0; k < 12; ++k)
+    h_bbox[k] = k % 6 < 3 ? 0xffffffffu : 0u;  // per model: minimum (x y z), maximum (x y z)
+  CK(cudaMemcpyAsync(word, h_bbox, sizeof(h_bbox), cudaMemcpyHostToDevice, st));
+  CK(cudaMemsetAsync(word + 12, 0, 8, st));
+  for (int k = 0; k < 2; ++k)
+    if (n[k])
+    {
+      const int nb = static_cast<int>((n[k] + 255) / 256);
+      scan_bbox_kernel<<<std::min(nb, c.sm_count * 8), 256, 0, st>>>(static_cast<const mcl3dl_point*>(c.s_clip[k].p), n[k], word + 6 * k);
+      CK(cudaGetLastError());
+      eng->launches++;
+    }
+  CK(cudaMemcpyAsync(h_bbox, word, sizeof(h_bbox), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  NsGridDev ng[2] = {};
+  int end_bit[2] = {1, 1};
+  for (int k = 0; k < 2; ++k)
+  {
+    ng[k].r2 = static_cast<float>(r * r);
+    const float mn[3] = {ord2f(h_bbox[6 * k]), ord2f(h_bbox[6 * k + 1]), ord2f(h_bbox[6 * k + 2])};
+    const float mx[3] = {ord2f(h_bbox[6 * k + 3]), ord2f(h_bbox[6 * k + 4]), ord2f(h_bbox[6 * k + 5])};
+    float edge = 0.0f;
+    // no finite point: the zero lattice keys every point as non-finite (key 0 == cells)
+    if (n[k] && mn[0] <= mx[0] && !ns_lattice(r, mn, mx, ng[k].g, end_bit[k], edge))
+      return MCL3DL_ERR_TOO_LARGE;
+  }
+  c.n_valid = false;
+  uint32_t n_sample[2];
+  for (int k = 0; k < 2; ++k)
+    if ((rc = ns_sample_model(eng, c, k, n[k], ng[k], end_bit[k], out.fpc_local, out.max_weight, scale, num[k], p->seed, n_sample + k,
+                              out.rounds + k, out.draws + k)))
+      return rc;
+  CK(cudaMemcpyAsync(c.h_pinned.p, word + 12, 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  std::memcpy(out.n_normal, c.h_pinned.p, 8);
+  // the new samples replace the prepared ones
+  std::swap(c.s_out[0], c.n_out[0]);
+  std::swap(c.s_out[1], c.n_out[1]);
+  out.n_lik = n_sample[0];
+  out.n_beam = n_sample[1];
+  c.s_info.n_lik = n_sample[0];
+  c.s_info.n_beam = n_sample[1];
+  c.n_valid = true;
+  if (info)
+    *info = out;
+  return MCL3DL_OK;
+}
+
+int mcl3dl_scan_normals(mcl3dl_engine* eng, int which, float* normals_xyz, uint32_t* n_neighbours, uint64_t* weights_q, size_t capacity,
+                        size_t* n_out)
+{
+  if (!eng || eng->devs.size() != 1 || which < 0 || which > 1 || !n_out)
+    return MCL3DL_ERR_INVALID_ARG;
+  DeviceCtx& c = eng->devs[0];
+  if (!c.s_valid || !c.n_valid)
+    return MCL3DL_ERR_INVALID_ARG;
+  const uint32_t n = which ? c.s_info.n_beam_clipped : c.s_info.n_lik_clipped;
+  *n_out = n;
+  if (n == 0 || (!normals_xyz && !n_neighbours && !weights_q))
+    return MCL3DL_OK;
+  if (capacity < n)
+    return MCL3DL_ERR_INVALID_ARG;
+  CK(cudaSetDevice(c.dev));
+  if (normals_xyz)
+    CK(cudaMemcpyAsync(normals_xyz, c.n_normals[which].p, size_t(n) * 12, cudaMemcpyDeviceToHost, c.stream));
+  if (n_neighbours)
+    CK(cudaMemcpyAsync(n_neighbours, c.n_nb[which].p, size_t(n) * 4, cudaMemcpyDeviceToHost, c.stream));
+  if (weights_q)
+    CK(cudaMemcpyAsync(weights_q, c.n_q[which].p, size_t(n) * 8, cudaMemcpyDeviceToHost, c.stream));
   CK(cudaStreamSynchronize(c.stream));
   return MCL3DL_OK;
 }

@@ -15,6 +15,10 @@
 //      replacement, uniform over the clipped points.  The reference seeds std::default_random_engine from
 //      std::random_device, i.e. its draws are not reproducible by construction; the device draws from Philox-4x32-10
 //      keyed by (seed, stream, draw index).
+// The node's other sampler, PointCloudSamplerWithNormal, replaces step 3 on demand (mcl3dl_scan_sample_with_normal,
+// ns_*_kernel below): per clipped cloud a stable key sort into a neighbour grid, one thread per point for its normal
+// and fixed-point weight, an exact uint64 inclusive sum, then rounds of weighted draws that keep each point's first
+// draw.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -147,6 +151,85 @@ __global__ void scan_sample_kernel(const mcl3dl_point* __restrict__ clipped, con
   if (t >= num || n == 0)
     return;
   out[t] = clipped[scan_sample_index(seed, stream, t, n)];
+}
+
+// ---- PointCloudSamplerWithNormal (mcl3dl_scan_sample_with_normal; the per-point pieces are ns_* of scan_funcs.cuh)
+// keys / values of the neighbour grid's stable sort: voxel_key on the grid's lattice, clipped index
+__global__ void ns_key_kernel(const mcl3dl_point* __restrict__ pts, uint32_t n, VoxelGridDev g, uint32_t* __restrict__ keys,
+                              uint32_t* __restrict__ vals)
+{
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n)
+    return;
+  keys[i] = voxel_key(g, pts[i]);
+  vals[i] = i;
+}
+
+// the clipped points in sorted order
+__global__ void ns_gather_kernel(const mcl3dl_point* __restrict__ pts, const uint32_t* __restrict__ order, uint32_t n,
+                                 mcl3dl_point* __restrict__ spts)
+{
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n)
+    spts[i] = pts[order[i]];
+}
+
+// one thread per clipped point: its normal, neighbour count and fixed-point weight; n_finite counts the finite normals
+__global__ void ns_normal_kernel(const mcl3dl_point* __restrict__ pts, uint32_t n, NsGridDev ng, const uint32_t* __restrict__ skeys,
+                                 const mcl3dl_point* __restrict__ spts, float f0, float f1, float f2, double max_weight, double scale,
+                                 float* __restrict__ normals, uint32_t* __restrict__ n_nb, uint64_t* __restrict__ q,
+                                 uint32_t* __restrict__ n_finite)
+{
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n)
+    return;
+  float nrm[3];
+  n_nb[i] = ns_point_normal(ng, skeys, spts, n, pts[i], nrm);
+  normals[3 * i + 0] = nrm[0];
+  normals[3 * i + 1] = nrm[1];
+  normals[3 * i + 2] = nrm[2];
+  const float fpc[3] = {f0, f1, f2};
+  q[i] = ns_weight_q(ns_weight(nrm, fpc, max_weight), scale);
+  if (nrm[0] == nrm[0])
+    atomicAdd(n_finite, 1u);
+}
+
+// draws d0 .. d0 + cnt - 1: their indices, and the first draw of each point (a 64-bit minimum over the draw numbers)
+__global__ void ns_draw_kernel(const uint64_t* __restrict__ cum, uint32_t n, uint64_t seed, uint32_t stream, uint64_t d0, uint32_t cnt,
+                               uint32_t* __restrict__ didx, unsigned long long* __restrict__ first)
+{
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= cnt)
+    return;
+  const uint64_t t = d0 + k;
+  const uint32_t i = ns_draw_index(cum, n, ns_draw_value(seed, stream, t, cum[n - 1]));
+  didx[k] = i;
+  atomicMin(first + i, static_cast<unsigned long long>(t));
+}
+
+// 1 where draw d0 + k is the first draw of its point
+__global__ void ns_first_flag_kernel(const uint32_t* __restrict__ didx, const unsigned long long* __restrict__ first, uint64_t d0,
+                                     uint32_t cnt, uint32_t* __restrict__ flags)
+{
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < cnt)
+    flags[k] = first[didx[k]] == d0 + k ? 1u : 0u;
+}
+
+// the round's first draws, in draw order, after the `carry` outputs of the earlier rounds (up to num); *carry_out =
+// carry + the round's first draws
+__global__ void ns_take_kernel(const mcl3dl_point* __restrict__ clipped, const uint32_t* __restrict__ didx, const uint32_t* __restrict__ flags,
+                               const uint32_t* __restrict__ pos, uint32_t cnt, uint32_t carry, uint32_t num, mcl3dl_point* __restrict__ out,
+                               uint32_t* __restrict__ carry_out)
+{
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= cnt)
+    return;
+  const uint32_t j = carry + pos[k];
+  if (k == cnt - 1)
+    *carry_out = j + flags[k];
+  if (flags[k] && j < num)
+    out[j] = clipped[didx[k]];
 }
 
 }  // namespace mcl3dl

@@ -94,6 +94,31 @@ class ScanInfo(C.Structure):
         return {k: int(getattr(self, k)) for k, _ in self._fields_}
 
 
+class NormalSamplerParams(C.Structure):
+    """mcl3dl_normal_sampler_params (Engine.scan_sample_with_normal fills it)."""
+    _fields_ = [("perform_weighting_ratio", C.c_double), ("max_weight_ratio", C.c_double), ("max_weight", C.c_double),
+                ("normal_search_range", C.c_double), ("eigen_values", C.c_double * 3), ("eigen_vector", C.c_double * 3),
+                ("mean_rot", C.c_float * 4), ("lik_num_points", C.c_uint32), ("beam_num_points", C.c_uint32),
+                ("seed", C.c_uint64)]
+
+
+class NormalSamplerInfo(C.Structure):
+    _fields_ = [("n_lik", C.c_uint32), ("n_beam", C.c_uint32), ("n_normal", C.c_uint32 * 2), ("rounds", C.c_uint32 * 2),
+                ("draws", C.c_uint64 * 2), ("max_weight", C.c_double), ("fpc_local", C.c_float * 3),
+                ("weight_shift", C.c_int32)]
+
+    def as_dict(self):
+        return {"n_lik": int(self.n_lik), "n_beam": int(self.n_beam), "n_normal": [int(v) for v in self.n_normal],
+                "rounds": [int(v) for v in self.rounds], "draws": [int(v) for v in self.draws],
+                "max_weight": float(self.max_weight), "fpc_local": np.array(list(self.fpc_local), np.float32),
+                "weight_shift": int(self.weight_shift)}
+
+
+# PointCloudSamplerWithNormalParameters' defaults (parameters.h:50-56), the node's
+NORMAL_SAMPLER_DEFAULTS = {"perform_weighting_ratio": 2.0, "max_weight_ratio": 5.0, "max_weight": 5.0,
+                           "normal_search_range": 0.4}
+
+
 class MatchParams(C.Structure):
     """mcl3dl_match_params (Engine.match_output fills it; its defaults are the node's)."""
     _fields_ = [("match_output_dist", C.c_double), ("unmatch_output_dist", C.c_double), ("chunk_length", C.c_float),
@@ -179,7 +204,7 @@ EXPORTED_SYMBOLS = ["mcl3dl_measure_update", "mcl3dl_collect_stats", "mcl3dl_rea
                     "mcl3dl_particles_resize", "mcl3dl_global_localization",
                     "mcl3dl_particles_redraw_odom_noise", "mcl3dl_particles_noise", "mcl3dl_particles_imu_update",
                     "mcl3dl_particles_landmark_update", "mcl3dl_particles_reset_odom_err_integ", "mcl3dl_particles_get_poses",
-                    "mcl3dl_particles_init"]
+                    "mcl3dl_particles_init", "mcl3dl_scan_sample_with_normal", "mcl3dl_scan_normals"]
 
 _LIBS = {}
 
@@ -241,6 +266,8 @@ def load_library(path=None):
     L.mcl3dl_scan_prepare.argtypes = [vp, vp, sz, vp, vp]
     L.mcl3dl_scan_get.argtypes = [vp, C.c_int, vp, sz, C.POINTER(sz)]
     L.mcl3dl_particles_measure_update_prepared.argtypes = [vp, vp, sz, C.c_float, vp]
+    L.mcl3dl_scan_sample_with_normal.argtypes = [vp, vp, vp]
+    L.mcl3dl_scan_normals.argtypes = [vp, C.c_int, vp, vp, vp, sz, C.POINTER(sz)]
     L.mcl3dl_match_output.argtypes = [vp, vp, vp, sz, vp, vp, C.POINTER(sz), vp, C.POINTER(sz)]
     L.mcl3dl_exchange_create.argtypes = [vp, sz, C.c_int, C.c_int, vp]
     L.mcl3dl_exchange_open.argtypes = [vp, vp]
@@ -607,6 +634,46 @@ class Engine:
         if n.value:
             self._check(self.L.mcl3dl_scan_get(self.h, which, _ptr(out), len(out), C.byref(n)))
         return out
+
+    def scan_sample_with_normal(self, mean_rot, pos_cov, params=None, lik_num_points=96, beam_num_points=3, seed=1):
+        """The node's PointCloudSamplerWithNormal on the clipped clouds of the last scan_prepare; the new samples replace
+        its sampled scans (include/mcl3dl_b200.h: mcl3dl_scan_sample_with_normal).  mean_rot: expectation().rot_ (x y z
+        w, raw); pos_cov: the covariance (its 3 x 3 position block is used; 6 x 6 accepted); params: a dict over
+        NORMAL_SAMPLER_DEFAULTS.  setParticleStatistics is restated with numpy: eigh of |pos_cov| in double (LAPACK, so the
+        eigenvector's bits and sign may differ from Eigen's SelfAdjointEigenSolver; the C++ adapter uses Eigen).
+        Returns the info as a dict."""
+        prm = dict(NORMAL_SAMPLER_DEFAULTS, **(params or {}))
+        cov = np.abs(np.asarray(pos_cov, dtype=np.float64)[:3, :3])
+        w, v = np.linalg.eigh(cov)
+        return self.scan_sample_with_normal_eigen(mean_rot, w, v[:, 2], prm, lik_num_points, beam_num_points, seed)
+
+    def scan_sample_with_normal_eigen(self, mean_rot, eigen_values, eigen_vector, params=None, lik_num_points=96,
+                                      beam_num_points=3, seed=1):
+        """mcl3dl_scan_sample_with_normal with the eigendecomposition given (ascending eigenvalues, the eigenvector of
+        the largest)."""
+        prm = dict(NORMAL_SAMPLER_DEFAULTS, **(params or {}))
+        sp = NormalSamplerParams()
+        for k in NORMAL_SAMPLER_DEFAULTS:
+            setattr(sp, k, float(prm[k]))
+        sp.eigen_values[:] = [float(x) for x in eigen_values]
+        sp.eigen_vector[:] = [float(x) for x in eigen_vector]
+        sp.mean_rot[:] = [float(x) for x in np.asarray(mean_rot, np.float32).reshape(4)]
+        sp.lik_num_points, sp.beam_num_points, sp.seed = lik_num_points, beam_num_points, seed
+        info = NormalSamplerInfo()
+        self._check(self.L.mcl3dl_scan_sample_with_normal(self.h, C.byref(sp), C.byref(info)))
+        return info.as_dict()
+
+    def scan_normals(self, which):
+        """(normals float32[n, 3], neighbour counts uint32[n], fixed-point weights uint64[n]) of the clipped cloud of
+        model `which` (0 likelihood, 1 beam) from the last scan_sample_with_normal."""
+        n = C.c_size_t(0)
+        self._check(self.L.mcl3dl_scan_normals(self.h, which, None, None, None, 0, C.byref(n)))
+        nrm = np.zeros((n.value, 3), np.float32)
+        nb = np.zeros(n.value, np.uint32)
+        q = np.zeros(n.value, np.uint64)
+        if n.value:
+            self._check(self.L.mcl3dl_scan_normals(self.h, which, _ptr(nrm), _ptr(nb), _ptr(q), n.value, C.byref(n)))
+        return nrm, nb, q
 
     def match_output(self, pose, pts=None, match_dist=0.1, unmatch_dist=0.5, chunk_length=20.0, max_search_radius=0.2):
         """The node's matched / unmatched clouds (include/mcl3dl_b200.h: mcl3dl_match_output) -> (matched, unmatched) as

@@ -280,6 +280,41 @@ public:
     for (size_t i = 0; i < n_m; ++i) matched.points.emplace_back(m[i].x, m[i].y, m[i].z);
     for (size_t i = 0; i < n_u; ++i) unmatched.points.emplace_back(u[i].x, u[i].y, u[i].z);
   }
+  // The node's PointCloudSamplerWithNormal (use_random_sampler_with_normal) on the clipped clouds of the last
+  // mcl3dl_scan_prepare, replacing its sampled scans (mcl3dl_scan_sample_with_normal).  The statistics are built exactly
+  // as setParticleStatistics builds them (point_cloud_sampler_with_normal.h:75-89): std::abs of the 3 x 3 position block
+  // of covariances, SelfAdjointEigenSolver of that double matrix, its eigenvalues and column 2, and mean.rot_ raw.
+  // Matrix / Solver are Eigen::MatrixXd and Eigen::SelfAdjointEigenSolver<Eigen::MatrixXd> (template parameters, so
+  // only a caller compiles the Eigen code); mean and covariances are pf_->expectation() and pf_->covariance(...), or for
+  // the resident set the mean rotation and covariance of mcl3dl_particles_estimate(NULL).
+  template <typename Matrix, typename Solver>
+  void sampleWithNormalPrepared(const State6DOF& mean, const std::vector<State6DOF>& covariances,
+                                const mcl_3dl::PointCloudSamplerWithNormalParameters& params, uint32_t lik_num, uint32_t beam_num,
+                                uint64_t seed, mcl3dl_normal_sampler_info* info)
+  {
+    Matrix pos_cov(3, 3);
+    for (size_t i = 0; i < 3; ++i)
+      for (size_t j = 0; j < 3; ++j) pos_cov(i, j) = std::abs(covariances[i][j]);
+    const Solver solver(pos_cov);
+    mcl3dl_normal_sampler_params p{};
+    p.perform_weighting_ratio = params.perform_weighting_ratio_;
+    p.max_weight_ratio = params.max_weight_ratio_;
+    p.max_weight = params.max_weight_;
+    p.normal_search_range = params.normal_search_range_;
+    for (int k = 0; k < 3; ++k)
+    {
+      p.eigen_values[k] = solver.eigenvalues()[k];
+      p.eigen_vector[k] = solver.eigenvectors()(k, 2);
+    }
+    p.mean_rot[0] = mean.rot_.x_;
+    p.mean_rot[1] = mean.rot_.y_;
+    p.mean_rot[2] = mean.rot_.z_;
+    p.mean_rot[3] = mean.rot_.w_;
+    p.lik_num_points = lik_num;
+    p.beam_num_points = beam_num;
+    p.seed = seed;
+    check(mcl3dl_scan_sample_with_normal(engine_, &p, info), "mcl3dl_scan_sample_with_normal");
+  }
   void checked(int rc, const char* what) const { check(rc, what); }
   size_t likPoints() const { return lik_cloud_ ? lik_cloud_->size() : 0; }
   // How each new map reached the engine: appended (mcl3dl_map_append) or staged whole (mcl3dl_set_map).

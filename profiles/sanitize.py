@@ -1,7 +1,7 @@
 """Small end-to-end run for compute-sanitizer (memcheck / racecheck / initcheck / synccheck), covering every kernel the
 library ships: map build incl. the NN field, the likelihood kernels with and without the NN field + the field mode, both
 beam kernels x both raycasters, the fused weight update, the resident particle set (predict / update / estimate /
-resample) and the scan preprocessing.
+resample), the scan preprocessing and the normal-weighted sampler.
    compute-sanitizer --tool racecheck python profiles/sanitize.py"""
 import os
 import sys
@@ -51,5 +51,8 @@ raw = np.tile(np.concatenate([s["lik"], s["beam"]]), 20)
 info = eng.scan_prepare(raw, engine.ScanParams(lik_num_points=50, beam_num_points=7, seed=3))
 sm2 = eng.particles_measure_update_prepared(s["origins"], 0.0)
 print("scan", info, sm2["kept"])
+ns = eng.scan_sample_with_normal((0, 0, 0, 1), np.diag([0.6, 0.05, 0.02]), None, 50, 7, seed=3)
+sm3 = eng.particles_measure_update_prepared(s["origins"], 0.0)
+print("normal sampler", ns["n_lik"], ns["n_beam"], ns["rounds"], len(eng.scan_normals(0)[0]), sm3["kept"])
 eng.close()
 print("sanitize run complete")
