@@ -215,6 +215,30 @@ int mcl3dl_beam_status(mcl3dl_engine*, const mcl3dl_pose* poses, size_t n_partic
                        const mcl3dl_point* beam_pts, size_t n_beam,
                        const float* origins_xyz, size_t n_origins, uint8_t* status);
 
+/* The node's rviz ray markers (src/mcl_3dl.cpp:464-628): every ray of one beam scan cast from ONE pose, the pose
+ * estimate e after e.rot_.normalize(), through LidarMeasurementModelBeam::getBeamStatus with the staged caster.  One
+ * record per ray, in scan order; begin / end / status are the bits the beam kernels compute for that pose.
+ *   pos: CastResult::pos_ of the cast step that decided the status, what the node draws as the collision marker:
+ *        DDA the deciding cell's centre fromIndex(current_index_) (raycast_using_dda.h:219-223, double, stored as float),
+ *        KD the marching position pos_ of the deciding step (raycast_using_kdtree.h:67-109).  NaN for LONG.
+ * beam_pts == NULL: the sampled beam scan the last mcl3dl_scan_prepare left on the device (or the last
+ * mcl3dl_scan_sample_with_normal after it); single-device engines only, n_beam is ignored.  Host scans on a multi-device
+ * engine run on device 0.  Synchronous.  Errors, all found before anything is written:
+ *   INVALID_ARG: a null engine, pose or n_out; out == NULL with rays to write; capacity below the ray count; a label
+ *                >= n_origins; a map staged without beam params, or the KD caster without lik params; beam_pts == NULL
+ *                without a prepared scan or on a multi-device engine;
+ *   NO_MAP:      before set_map.
+ * An empty scan returns OK with *n_out = 0. */
+typedef struct
+{
+  float begin[3];  /* e.pos_ + e.rot_ * origins[label], raw rot_ (mcl_3dl.cpp:475, beam.cpp:145) */
+  float end[3];    /* the scan point transformed by the pose (State6DOF::transform, normalised rot_) */
+  float pos[3];    /* CastResult::pos_ of the deciding cast step; NaN for LONG */
+  uint32_t status; /* 0 SHORT, 1 HIT, 2 LONG, 3 TOTAL_REFLECTION (the codes of mcl3dl_beam_status) */
+} mcl3dl_beam_ray;
+int mcl3dl_beam_cast(mcl3dl_engine*, const mcl3dl_pose* pose, const mcl3dl_point* beam_pts, size_t n_beam,
+                     const float* origins_xyz, size_t n_origins, mcl3dl_beam_ray* out, size_t capacity, size_t* n_out);
+
 /* Summary of one fused weight update (row f2 of the scope table). */
 typedef struct
 {

@@ -1168,4 +1168,54 @@ __device__ __forceinline__ void load_pose(const mcl3dl_pose* pose, F3& pos, Q4& 
   q.w = b.w;
 }
 
+// fromIndex, raycast_using_dda.h:219-223: (i + 0.5) * grid + min_p in double, stored into a float Vec3
+__device__ __forceinline__ F3 dda_centre(const DdaGridDev& g, int cx, int cy, int cz)
+{
+  F3 c;
+  c.x = __double2float_rn(dadd(dmul(dadd(static_cast<double>(cx), 0.5), g.grid), static_cast<double>(g.min_x)));
+  c.y = __double2float_rn(dadd(dmul(dadd(static_cast<double>(cy), 0.5), g.grid), static_cast<double>(g.min_y)));
+  c.z = __double2float_rn(dadd(dmul(dadd(static_cast<double>(cz), 0.5), g.grid), static_cast<double>(g.min_z)));
+  return c;
+}
+
+// cast_ray / cast_ray_kd for the node's ray markers (src/mcl_3dl.cpp:472-523): the same status, and in *at the
+// CastResult::pos_ of the cast step that decided it — the deciding cell's centre (DDA) or the marching position (KD).
+// *at is meaningless for LONG (no step decided; the node reads point.pos_ only for the other statuses).  The KD caster
+// stores every probed position before its probe (a deciding probe does not move it): kept in registers, the position
+// would be spilled around the probe's division subroutines.
+__device__ __forceinline__ int cast_ray_at(const DdaGridDev& g, const F3& b, const F3& e, F3* at)
+{
+  uint32_t n_steps = 0, n_occ = 0, n_tested = 0;
+  DdaRay r;
+  int st = dda_setup(g, b, e, r);
+  while (st < 0)
+  {
+    st = dda_advance(g, r, n_steps);
+    if (st < 0)
+      st = dda_test_cell(g, r, n_occ, n_tested);
+  }
+  if (st != ST_LONG)
+    *at = dda_centre(g, r.cx, r.cy, r.cz);
+  return st;
+}
+
+__device__ __forceinline__ int cast_ray_kd_at(const KdRayDev& k, const NnGridDev& nn, const DdaGridDev& g, const F3& b,
+                                              const F3& e, F3* at)
+{
+  uint32_t n_steps = 0, n_occ = 0, n_tested = 0;
+  KdRay r;
+  kd_setup(k, b, e, r);
+  int st = -1;
+  while (st < 0)
+  {
+    st = kd_march(k, nn, r, n_steps);
+    if (st < 0)
+    {
+      *at = r.pos;
+      st = kd_probe(k, nn, g, r, n_occ, n_tested);
+    }
+  }
+  return st;
+}
+
 }  // namespace mcl3dl

@@ -511,6 +511,10 @@ struct DeviceCtx
   // both clouds and their counts into
   DevBuf m_in, m_tf, m_flags[2], m_pos[2], m_tmp;
   PinnedBuf m_host;
+  // ray markers (mcl3dl_beam_cast): [pose | origins | host scan] on the device; the page-locked block holds the same
+  // inputs for their one copy, the label error word and the records the kernel stores
+  DevBuf b_in;
+  PinnedBuf b_host;
   DevBuf r_states[2], r_prob, r_accum, r_poses, r_extra, r_est;  // r_est: EstHeader + per-CTA partial sums
   size_t r_n = 0;
   int r_cur = 0;
@@ -3699,6 +3703,69 @@ int mcl3dl_beam_status(mcl3dl_engine* eng, const mcl3dl_pose* poses, size_t P, c
   if (n_beam == 0)
     return MCL3DL_OK;
   return measure_host(eng, poses, P, nullptr, 0, beam_pts, n_beam, origins_xyz, n_origins, nullptr, status);
+}
+
+int mcl3dl_beam_cast(mcl3dl_engine* eng, const mcl3dl_pose* pose, const mcl3dl_point* beam_pts, size_t n_beam,
+                     const float* origins_xyz, size_t n_origins, mcl3dl_beam_ray* out, size_t capacity, size_t* n_out)
+{
+  if (!eng || !pose || !n_out)
+    return MCL3DL_ERR_INVALID_ARG;
+  if (!eng->has_map)
+    return MCL3DL_ERR_NO_MAP;
+  const bool kd = !eng->beam.use_raycast_using_dda;
+  if (!eng->has_beam || (kd && !eng->has_lik))
+    return MCL3DL_ERR_INVALID_ARG;
+  DeviceCtx& c = eng->devs[0];
+  const mcl3dl_point* d_scan = nullptr;  // the prepared scan, or the host scan's copy in b_in
+  size_t n = n_beam;
+  if (!beam_pts)
+  {
+    if (eng->devs.size() != 1 || !c.s_valid)
+      return MCL3DL_ERR_INVALID_ARG;
+    d_scan = static_cast<const mcl3dl_point*>(c.s_out[1].p);
+    n = c.s_info.n_beam;
+  }
+  if (n >= (size_t(1) << 24) || (n && (!out || capacity < n || !origins_xyz || n_origins == 0)))
+    return MCL3DL_ERR_INVALID_ARG;
+  if (n == 0)
+  {
+    *n_out = 0;
+    return MCL3DL_OK;
+  }
+  CK(cudaSetDevice(c.dev));
+  cudaStream_t st = c.stream;
+  // page-locked block: [label error word | pad to 64 | pose (32 B) | origins | host scan | records]; the inputs go up in
+  // one copy to b_in (same layout from the pose on), the kernel stores the error word and the records in place
+  const size_t o_org = 64 + sizeof(mcl3dl_pose), o_scan = o_org + pad16(n_origins * 12);
+  const size_t in_end = o_scan + (beam_pts ? n * 16 : 0), o_rec = pad16(in_end);
+  int rc;
+  if ((rc = reserve(eng, c.b_host, o_rec + n * sizeof(mcl3dl_beam_ray))) || (rc = reserve(eng, c.b_in, in_end - 64)))
+    return rc;
+  char* hp = static_cast<char*>(c.b_host.p);
+  char* dp = static_cast<char*>(c.b_in.p);
+  unsigned int* bad = reinterpret_cast<unsigned int*>(hp);
+  *bad = 0;
+  std::memcpy(hp + 64, pose, sizeof(mcl3dl_pose));
+  std::memcpy(hp + o_org, origins_xyz, n_origins * 12);
+  if (beam_pts)
+  {
+    std::memcpy(hp + o_scan, beam_pts, n * 16);
+    d_scan = reinterpret_cast<const mcl3dl_point*>(dp + o_scan - 64);
+  }
+  CK(cudaMemcpyAsync(dp, hp + 64, in_end - 64, cudaMemcpyHostToDevice, st));
+  mcl3dl_beam_ray* h_rec = reinterpret_cast<mcl3dl_beam_ray*>(hp + o_rec);
+  const auto kernel = kd ? beam_cast_kernel<true> : beam_cast_kernel<false>;
+  kernel<<<static_cast<unsigned>((n + kBlockThreads - 1) / kBlockThreads), kBlockThreads, 0, st>>>(
+      reinterpret_cast<const mcl3dl_pose*>(dp), reinterpret_cast<const float4*>(d_scan), static_cast<int>(n),
+      reinterpret_cast<const float*>(dp + o_org - 64), static_cast<uint32_t>(n_origins), c.dda, c.kd, c.nn, h_rec, bad);
+  CK(cudaGetLastError());
+  eng->launches++;
+  CK(cudaStreamSynchronize(st));
+  if (*bad)
+    return MCL3DL_ERR_INVALID_ARG;
+  std::memcpy(out, h_rec, n * sizeof(mcl3dl_beam_ray));
+  *n_out = n;
+  return MCL3DL_OK;
 }
 
 int mcl3dl_collect_stats(mcl3dl_engine* eng, int enable)

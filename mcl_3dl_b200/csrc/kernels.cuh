@@ -1221,6 +1221,53 @@ __global__ void __launch_bounds__(kBlockThreads, 4)
   }
 }
 
+// The node's ray markers (src/mcl_3dl.cpp:464-628, mcl3dl_beam_cast): the rays of one scan from one pose, one thread
+// per ray, with the pose load, transform and ray origin of the kernels above, so that end, begin and status are theirs.
+// A label outside the origins sets *bad_label and leaves the ray's record unwritten (the call then reports INVALID_ARG).
+template <bool KD>
+__global__ void __launch_bounds__(kBlockThreads)
+    beam_cast_kernel(const mcl3dl_pose* __restrict__ pose, const float4* __restrict__ scan, int N,
+                     const float* __restrict__ origins, uint32_t n_origins, DdaGridDev g, KdRayDev kd, NnGridDev nn,
+                     mcl3dl_beam_ray* __restrict__ out, unsigned int* __restrict__ bad_label)
+{
+  const int j = blockIdx.x * kBlockThreads + threadIdx.x;
+  if (j >= N)
+    return;
+  F3 pos;
+  Q4 q;
+  load_pose(pose, pos, q);
+  const Q4 rn = qnormalized(q);
+  const float4 sp = __ldg(scan + j);
+  const uint32_t label = __float_as_uint(sp.w);
+  if (label >= n_origins)
+  {
+    *bad_label = 1u;  // (page-locked host memory: a plain store, read after the stream synchronises)
+    return;
+  }
+  F3 v;
+  v.x = sp.x;
+  v.y = sp.y;
+  v.z = sp.z;
+  const F3 end = transform_point(rn, pos, v);  // beam.cpp:138-139
+  const F3 begin = ray_origin(pos, q, origins, label);
+  // begin and end are stored before the cast, so that they need no registers across its division subroutines
+  mcl3dl_beam_ray* r = out + j;
+  r->begin[0] = begin.x;
+  r->begin[1] = begin.y;
+  r->begin[2] = begin.z;
+  r->end[0] = end.x;
+  r->end[1] = end.y;
+  r->end[2] = end.z;
+  __shared__ F3 s_at[kBlockThreads];
+  F3* at = s_at + threadIdx.x;
+  const int st = KD ? cast_ray_kd_at(kd, nn, g, begin, end, at) : cast_ray_at(g, begin, end, at);
+  const float nan = __int_as_float(0x7fc00000);
+  r->pos[0] = st == ST_LONG ? nan : at->x;
+  r->pos[1] = st == ST_LONG ? nan : at->y;
+  r->pos[2] = st == ST_LONG ? nan : at->z;
+  r->status = static_cast<uint32_t>(st);
+}
+
 // ============================================================================================
 // Fused weight update (scope row f2): pf::ParticleFilter::measure's arithmetic on the records that
 // the two kernels above left on the device.  Deterministic: every reduction has a fixed tree

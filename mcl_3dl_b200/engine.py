@@ -14,6 +14,9 @@ import numpy as np
 from . import build as _build
 from .synth import POINT, POSE, RESULT, STATE
 
+# mcl3dl_beam_ray: one ray of mcl3dl_beam_cast (40 bytes)
+BEAM_RAY = np.dtype([("begin", "<f4", 3), ("end", "<f4", 3), ("pos", "<f4", 3), ("status", "<u4")])
+
 ERR = {0: "ok", -1: "invalid argument", -2: "measure() before set_map()", -3: "CUDA runtime error",
        -4: "no usable CUDA device", -5: "grid exceeds 2^31-1 cells", -6: "search radius out of range"}
 
@@ -204,7 +207,7 @@ EXPORTED_SYMBOLS = ["mcl3dl_measure_update", "mcl3dl_collect_stats", "mcl3dl_rea
                     "mcl3dl_particles_resize", "mcl3dl_global_localization",
                     "mcl3dl_particles_redraw_odom_noise", "mcl3dl_particles_noise", "mcl3dl_particles_imu_update",
                     "mcl3dl_particles_landmark_update", "mcl3dl_particles_reset_odom_err_integ", "mcl3dl_particles_get_poses",
-                    "mcl3dl_particles_init", "mcl3dl_scan_sample_with_normal", "mcl3dl_scan_normals"]
+                    "mcl3dl_particles_init", "mcl3dl_scan_sample_with_normal", "mcl3dl_scan_normals", "mcl3dl_beam_cast"]
 
 _LIBS = {}
 
@@ -269,6 +272,7 @@ def load_library(path=None):
     L.mcl3dl_scan_sample_with_normal.argtypes = [vp, vp, vp]
     L.mcl3dl_scan_normals.argtypes = [vp, C.c_int, vp, vp, vp, sz, C.POINTER(sz)]
     L.mcl3dl_match_output.argtypes = [vp, vp, vp, sz, vp, vp, C.POINTER(sz), vp, C.POINTER(sz)]
+    L.mcl3dl_beam_cast.argtypes = [vp, vp, vp, sz, vp, sz, vp, sz, C.POINTER(sz)]
     L.mcl3dl_exchange_create.argtypes = [vp, sz, C.c_int, C.c_int, vp]
     L.mcl3dl_exchange_open.argtypes = [vp, vp]
     L.mcl3dl_measure_exchange_device.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp, sz, vp, C.POINTER(vp)]
@@ -486,6 +490,26 @@ class Engine:
         self._check(self.L.mcl3dl_beam_status(self.h, _ptr(poses), len(poses), _ptr(beam_pts), len(beam_pts),
                                               _ptr(origins), len(origins), _ptr(st)))
         return st
+
+    def beam_cast(self, pose, beam_pts=None, origins=((0.0, 0.0, 0.0),)):
+        """The node's ray markers from one pose (include/mcl3dl_b200.h: mcl3dl_beam_cast) -> BEAM_RAY[n_rays] in scan
+        order: begin, end, the deciding cast step's position (NaN for LONG) and the status.  beam_pts=None: the sampled
+        beam scan of the last scan_prepare / scan_sample_with_normal."""
+        pose = np.ascontiguousarray(pose, dtype=POSE).reshape(1)
+        origins = np.ascontiguousarray(origins, dtype=np.float32).reshape(-1, 3)
+        if beam_pts is not None:
+            beam_pts = np.ascontiguousarray(beam_pts, dtype=POINT)
+            cap = len(beam_pts)
+        else:  # the prepared scan's size (no prepared scan: the call below reports the error)
+            n_b = C.c_size_t(0)
+            cap = n_b.value if self.L.mcl3dl_scan_get(self.h, 4, None, 0, C.byref(n_b)) == 0 else 0
+        out = np.zeros(cap, dtype=BEAM_RAY)
+        n = C.c_size_t(0)
+        # (an empty host scan still needs a pointer: NULL selects the prepared scan)
+        self._check(self.L.mcl3dl_beam_cast(self.h, _ptr(pose), beam_pts.ctypes.data if beam_pts is not None else None,
+                                            len(beam_pts) if beam_pts is not None else 0, _ptr(origins), len(origins),
+                                            _ptr(out), cap, C.byref(n)))
+        return out[:n.value]
 
     def collect_stats(self, enable=True):
         self._check(self.L.mcl3dl_collect_stats(self.h, 1 if enable else 0))

@@ -315,6 +315,68 @@ public:
     p.seed = seed;
     check(mcl3dl_scan_sample_with_normal(engine_, &p, info), "mcl3dl_scan_sample_with_normal");
   }
+  // The map source of a node that does not fill its CPU map index (INTEGRATION.md, "the node without its CPU map index"):
+  // cbMapUpdateTimer hands pc_map2_ here in place of kdtree_->setInputCloud(pc_map2_), and the map is staged at once, by
+  // the rule of every entry point: the same cloud grown with a new stamp and its staged points unchanged in front is
+  // appended (mcl3dl_map_append), anything else is staged whole.  The entry points that take the index read this cloud
+  // while the index has none.
+  void setMapCloud(const Cloud::ConstPtr& map)
+  {
+    map_cloud_ = map;
+    stageCloud(map);
+    if (!staged_map_)
+      stageCloud(map);
+  }
+  // One ray of the node's rviz markers (src/mcl_3dl.cpp:472-523): what the marker loop takes from its getBeamStatus call.
+  struct BeamRay
+  {
+    Vec3 begin;  // pos, e.pos_ + e.rot_ * origins[label]
+    Vec3 end;    // end, the scan point transformed by e
+    Vec3 pos;    // point.pos_, the deciding cast step's position (NaN for LONG, where the node does not read it)
+    mcl_3dl::LidarMeasurementModelBeam::BeamStatus status;
+  };
+  // The marker loop's casts from the pose estimate e (after e.rot_.normalize()) on the device (mcl3dl_beam_cast) over the
+  // staged map; pc_beam == nullptr takes the sampled beam scan of the last mcl3dl_scan_prepare.
+  void castBeams(const State6DOF& e, const Cloud::ConstPtr& pc_beam, const std::vector<Vec3>& origins, std::vector<BeamRay>& out)
+  {
+    using BeamStatus = mcl_3dl::LidarMeasurementModelBeam::BeamStatus;
+    static_assert(static_cast<int>(BeamStatus::SHORT) == 0 && static_cast<int>(BeamStatus::HIT) == 1 &&
+                      static_cast<int>(BeamStatus::LONG) == 2 && static_cast<int>(BeamStatus::TOTAL_REFLECTION) == 3,
+                  "mcl3dl_beam_ray::status codes follow the order of LidarMeasurementModelBeam::BeamStatus");
+    std::vector<mcl3dl_point> in;
+    size_t cap = 0;
+    if (pc_beam)
+    {
+      pack(pc_beam, in);
+      cap = in.size();
+    }
+    else
+    {
+      check(mcl3dl_scan_get(engine_, 4, nullptr, 0, &cap), "mcl3dl_scan_get");
+    }
+    std::vector<float> o(origins.size() * 3);
+    for (size_t k = 0; k < origins.size(); ++k)
+    {
+      o[3 * k] = origins[k].x_;
+      o[3 * k + 1] = origins[k].y_;
+      o[3 * k + 2] = origins[k].z_;
+    }
+    std::vector<mcl3dl_beam_ray> rays(cap);
+    const mcl3dl_pose pose = toPose(e);
+    const mcl3dl_point none{};  // an empty host scan still needs a pointer: NULL selects the prepared scan
+    size_t n = 0;
+    check(mcl3dl_beam_cast(engine_, &pose, pc_beam ? (in.empty() ? &none : in.data()) : nullptr, in.size(), o.data(), origins.size(),
+                           rays.data(), rays.size(), &n),
+          "mcl3dl_beam_cast");
+    out.clear();
+    out.reserve(n);
+    for (size_t i = 0; i < n; ++i)
+    {
+      const mcl3dl_beam_ray& r = rays[i];
+      out.push_back(BeamRay{Vec3(r.begin[0], r.begin[1], r.begin[2]), Vec3(r.end[0], r.end[1], r.end[2]),
+                            Vec3(r.pos[0], r.pos[1], r.pos[2]), static_cast<BeamStatus>(r.status)});
+    }
+  }
   void checked(int rc, const char* what) const { check(rc, what); }
   size_t likPoints() const { return lik_cloud_ ? lik_cloud_->size() : 0; }
   // How each new map reached the engine: appended (mcl3dl_map_append) or staged whole (mcl3dl_set_map).
@@ -364,9 +426,13 @@ private:
     if (rc != MCL3DL_OK)
       throw std::runtime_error(std::string(what) + ": " + mcl3dl_strerror(rc) + " " + mcl3dl_last_error_detail(engine_));
   }
+  // The map of an entry point that takes the index: the index's cloud, or while it has none the last setMapCloud's.
   void stageMap(ChunkedKdtree<PointType>::Ptr& kdtree)
   {
-    const Cloud::ConstPtr& map = kdtree->getInputCloud();
+    stageCloud(kdtree->getInputCloud() ? kdtree->getInputCloud() : map_cloud_);
+  }
+  void stageCloud(const Cloud::ConstPtr& map)
+  {
     if (!map || map->empty())
       throw std::runtime_error("mcl_3dl_b200: measure() without a map cloud");
     // same trigger as RaycastUsingDDA::updatePointCloud (raycast_using_dda.h:162-171): cloud + header.stamp
@@ -497,6 +563,7 @@ private:
   decltype(pcl::PCLHeader().stamp) staged_stamp_ = 0;
   size_t staged_size_ = 0;
   std::vector<mcl3dl_point> staged_pts_;  // the staged map as packed: recognises an append to it
+  Cloud::ConstPtr map_cloud_;              // the last setMapCloud's cloud
   uint64_t stamp_counter_ = 0;
   size_t map_appends_ = 0, map_restages_ = 0;
   Cloud::ConstPtr lik_cloud_, beam_cloud_;
