@@ -524,6 +524,61 @@ int mcl3dl_scan_get(mcl3dl_engine*, int which, mcl3dl_point* out, size_t capacit
 int mcl3dl_particles_measure_update_prepared(mcl3dl_engine*, const float* origins_xyz, size_t n_origins,
                                              float odom_err_integ_lin_sigma, mcl3dl_update_summary* summary);
 
+/* ---- Cloud accumulation on the device (src/mcl_3dl.cpp:248-342): the cloud mcl3dl_scan_prepare receives, built where it
+ * is used.  cbCloud -> CloudAccumulationLogic::push (src/cloud_accum.cpp:53-119) calls accumCloud / accumClear / measure();
+ * with these entry points each incoming PointCloud2 crosses the bus once, as raw bytes, and measure() sends nothing but
+ * the origins.
+ *   accumulate (accumCloud, :274-302): tf2::doTransform of every point into the odom frame (odom_from_sensor), the
+ *     conversion, label = the cloud's accumulation index k (k-th call since the last clear, from 0; :295-298), appended
+ *     in row-major order.  Point (r, c) is read at data + r row_step + c point_step + offset[i] (FLOAT32, little-endian);
+ *     the call reads (height - 1) row_step + width point_step bytes from data and returns after it no longer needs them.
+ *     *n_clouds_out (may be NULL): the clouds accumulated, this one included.  Errors, all checked before data is read,
+ *     leave the accumulation as it was: INVALID_ARG for a null engine / view / data / transform, a multi-device engine,
+ *     width height == 0, an offset + 4 > point_step or row_step < width point_step; TOO_LARGE when the accumulated total
+ *     would reach 2^30 points (mcl3dl_scan_prepare's limit).
+ *   clear (accumClear, :266-272): empties the accumulation; the prepared scans stay.
+ *   accumulated_get: the accumulated points in the odom frame, as they are (the prepare below does not change them).
+ *   prepare_accumulated (measure(), :319-367): pcl::transformPointCloud of the accumulation into base_link
+ *     (base_from_odom), then exactly mcl3dl_scan_prepare's pipeline on it (VoxelGrid, clip, uniform sample; scan_get,
+ *     particles_measure_update_prepared, scan_sample_with_normal, match_output(pts = NULL) and beam_cast(beam_pts = NULL)
+ *     read its result).  The beam labels are accumulation indices, so the caller's origins (one per accumulated header,
+ *     :343-359) cover them.  The accumulation is not consumed.  INVALID_ARG, with nothing changed (the previous
+ *     prepared scans stay valid), for a null engine / transform / params, a multi-device engine or an empty accumulation
+ *     (the node logs and returns, :312-316).
+ * The transforms (both; restating Eigen and PCL): R = Eigen::Quaternion<float>(float(w), float(x), float(y),
+ * float(z)).toRotationMatrix() on the RAW quaternion (no normalisation; Eigen's formula: tx = 2x, .., twz = tz w, ..,
+ * R00 = 1 - (tyy + tzz), R01 = txy - twz, ..), t = float(translation), out_i = ((R_i0 x + R_i1 y) + R_i2 z) + t_i with every
+ * operation rounded on its own.  They are applied as two transforms, in the node's order, never composed.  The first
+ * applies to every point (tf2_sensor_msgs iterates over all of them); the second, as pcl::transformPointCloud, to every
+ * point when every accumulated cloud had is_dense, otherwise it leaves a point with any non-finite coordinate as it is
+ * (visible without downsampling: the models' clip keeps NaN points and drops infinite ones).
+ * Departures: PCL, tf2 and Eigen are third-party and absent from the reference tree, so the operation order above is
+ * restated, "parity unpinned" as the VoxelGrid: PCL's SSE2 Transformer<float>::se3 may nest the sum the other way
+ * (x c0 + (y c1 + (z c2 + t))), which would differ in the last ulp; this has not been checked against a PCL build.  The C++
+ * adapter rejects what fromROSMsg would (no x / y / z field, an empty cloud) and, beyond it, x / y / z that are not
+ * FLOAT32, a big-endian cloud, and a layout that does not hold its points (row_step < width point_step, data shorter
+ * than (height - 1) row_step + width point_step, or a field that does not fit in point_step), which pcl::fromROSMsg
+ * does not check and would read past the message's data.  Synchronous; single-device engines. */
+typedef struct
+{
+  const void* data;                           /* PointCloud2::data */
+  uint32_t width, height, point_step, row_step;
+  uint32_t offset[3];                         /* byte offsets of the FLOAT32 fields x, y, z */
+  int32_t is_dense;                           /* PointCloud2::is_dense */
+} mcl3dl_cloud_view;
+typedef struct
+{
+  double translation[3];
+  double rotation[4]; /* x y z w, raw */
+} mcl3dl_transform;
+int mcl3dl_scan_accumulate(mcl3dl_engine*, const mcl3dl_cloud_view* cloud, const mcl3dl_transform* odom_from_sensor,
+                           uint32_t* n_clouds_out);
+int mcl3dl_scan_accumulate_clear(mcl3dl_engine*);
+/* *n_out = the accumulated point count; out == NULL: count only; INVALID_ARG when capacity is below it. */
+int mcl3dl_scan_accumulated_get(mcl3dl_engine*, mcl3dl_point* out, size_t capacity, size_t* n_out);
+int mcl3dl_scan_prepare_accumulated(mcl3dl_engine*, const mcl3dl_transform* base_from_odom, const mcl3dl_scan_params*,
+                                    mcl3dl_scan_info* info);
+
 /* The node's second sampler, PointCloudSamplerWithNormal (use_random_sampler_with_normal; point_cloud_random_samplers/
  * point_cloud_sampler_with_normal.h), on the clipped clouds the last mcl3dl_scan_prepare left on the device, once per
  * model.  It REPLACES that call's sampled scans (scan_get(3 | 4), particles_measure_update_prepared); the downsampled and

@@ -500,6 +500,12 @@ struct DeviceCtx
   DevBuf s_raw, s_keys[2], s_vals[2], s_key_label[2], s_flags[2], s_pos[2], s_ds, s_clip[2], s_out[2], s_tmp, s_counts;
   mcl3dl_scan_info s_info{};
   bool s_valid = false;
+  // cloud accumulation (mcl3dl_scan_accumulate): the accumulated points in the odom frame, the last cloud's raw bytes;
+  // points and clouds since the last clear, and whether every one of those clouds was dense
+  DevBuf a_pts, a_raw;
+  size_t a_n = 0;
+  uint32_t a_clouds = 0;
+  bool a_dense = true;
   // normal-weighted sampler (mcl3dl_scan_sample_with_normal): neighbour-grid sort keys / values (x2), sorted points; per
   // model the normals, neighbour counts and fixed-point weights of its clipped points (mcl3dl_scan_normals); the inclusive
   // sum of the weights, each point's first draw, a round's draw indices / flags / scan positions, the new sampled scans,
@@ -2989,11 +2995,13 @@ int mcl3dl_particles_measure_update_prepared(mcl3dl_engine* eng, const float* or
 }
 
 // ---- scan preprocessing on the device (scan_kernels.cuh)
-int mcl3dl_scan_prepare(mcl3dl_engine* eng, const mcl3dl_point* raw, size_t n_raw, const mcl3dl_scan_params* sp, mcl3dl_scan_info* info)
+// mcl3dl_scan_prepare from its raw cloud on: `fill(st)` writes the n_raw (< 2^30) raw points into c.s_raw on the stream
+// (a host upload, or the accumulation's transform), then VoxelGrid, clip, uniform sample and the counts
+extern "C++" {
+template <typename Fill>
+static int scan_prepare_from(mcl3dl_engine* eng, DeviceCtx& c, size_t n_raw, const mcl3dl_scan_params* sp, mcl3dl_scan_info* info,
+                             Fill fill)
 {
-  if (!eng || eng->devs.size() != 1 || !sp || (n_raw && !raw) || n_raw >= (size_t(1) << 30))
-    return MCL3DL_ERR_INVALID_ARG;
-  DeviceCtx& c = eng->devs[0];
   CK(cudaSetDevice(c.dev));
   cudaStream_t st = c.stream;
   c.s_valid = false;
@@ -3021,7 +3029,8 @@ int mcl3dl_scan_prepare(mcl3dl_engine* eng, const mcl3dl_point* raw, size_t n_ra
   }
   if ((rc = reserve(eng, c.h_pinned, 256)))
     return rc;
-  CK(cudaMemcpyAsync(c.s_raw.p, raw, n_raw * 16, cudaMemcpyHostToDevice, st));
+  if ((rc = fill(st)))
+    return rc;
   const mcl3dl_point* d_raw = static_cast<const mcl3dl_point*>(c.s_raw.p);
   const mcl3dl_point* d_ds = d_raw;
   const int nb = static_cast<int>((n + 255) / 256);
@@ -3076,6 +3085,116 @@ int mcl3dl_scan_prepare(mcl3dl_engine* eng, const mcl3dl_point* raw, size_t n_ra
   c.s_valid = true;
   if (info) *info = c.s_info;
   return MCL3DL_OK;
+}
+}  // extern "C++"
+
+int mcl3dl_scan_prepare(mcl3dl_engine* eng, const mcl3dl_point* raw, size_t n_raw, const mcl3dl_scan_params* sp, mcl3dl_scan_info* info)
+{
+  if (!eng || eng->devs.size() != 1 || !sp || (n_raw && !raw) || n_raw >= (size_t(1) << 30))
+    return MCL3DL_ERR_INVALID_ARG;
+  DeviceCtx& c = eng->devs[0];
+  return scan_prepare_from(eng, c, n_raw, sp, info, [&](cudaStream_t st) -> int {
+    CK(cudaMemcpyAsync(c.s_raw.p, raw, n_raw * 16, cudaMemcpyHostToDevice, st));
+    return MCL3DL_OK;
+  });
+}
+
+// ---- cloud accumulation (scan_kernels.cuh: accum_*_kernel)
+int mcl3dl_scan_accumulate(mcl3dl_engine* eng, const mcl3dl_cloud_view* v, const mcl3dl_transform* tf, uint32_t* n_clouds_out)
+{
+  if (!eng || eng->devs.size() != 1 || !v || !v->data || !tf)
+    return MCL3DL_ERR_INVALID_ARG;
+  const uint64_t n = static_cast<uint64_t>(v->width) * v->height;
+  if (n == 0 || static_cast<uint64_t>(v->row_step) < static_cast<uint64_t>(v->width) * v->point_step)
+    return MCL3DL_ERR_INVALID_ARG;
+  for (int k = 0; k < 3; ++k)
+    if (static_cast<uint64_t>(v->offset[k]) + 4 > v->point_step)
+      return MCL3DL_ERR_INVALID_ARG;
+  DeviceCtx& c = eng->devs[0];
+  const uint64_t total = c.a_n + n;
+  if (total >= (uint64_t(1) << 30))
+    return MCL3DL_ERR_TOO_LARGE;
+  // the bytes the points span (the last row ends at its last point)
+  const size_t bytes = static_cast<size_t>(v->height - 1) * v->row_step + static_cast<size_t>(v->width) * v->point_step;
+  CK(cudaSetDevice(c.dev));
+  cudaStream_t st = c.stream;
+  int rc;
+  if (!c.a_pts.p || total * 16 > c.a_pts.cap)
+  {
+    // reserve() drops the contents: grow into a new buffer and carry the accumulated points over on the device
+    DevBuf grown;
+    if ((rc = reserve(eng, grown, std::max<uint64_t>(total, std::min<uint64_t>(2 * c.a_n, uint64_t(1) << 30)) * 16)))
+      return rc;
+    if (c.a_n)
+      CK(cudaMemcpyAsync(grown.p, c.a_pts.p, c.a_n * 16, cudaMemcpyDeviceToDevice, st));
+    CK(cudaStreamSynchronize(st));
+    c.a_pts = std::move(grown);
+  }
+  if ((rc = reserve(eng, c.a_raw, bytes)))
+    return rc;
+  CK(cudaMemcpyAsync(c.a_raw.p, v->data, bytes, cudaMemcpyHostToDevice, st));
+  const uint32_t n32 = static_cast<uint32_t>(n);
+  const double* t = tf->translation;
+  const double* q = tf->rotation;
+  accum_cloud_kernel<<<(n32 + 255) / 256, 256, 0, st>>>(static_cast<const unsigned char*>(c.a_raw.p), v->width, n32, v->row_step,
+                                                        v->point_step, v->offset[0], v->offset[1], v->offset[2], t[0], t[1], t[2],
+                                                        q[0], q[1], q[2], q[3], c.a_clouds,
+                                                        static_cast<mcl3dl_point*>(c.a_pts.p) + c.a_n);
+  CK(cudaGetLastError());
+  eng->launches++;
+  CK(cudaStreamSynchronize(st));  // the caller may reuse data as soon as this returns
+  c.a_n = total;
+  c.a_clouds++;
+  c.a_dense = c.a_dense && v->is_dense;
+  if (n_clouds_out)
+    *n_clouds_out = c.a_clouds;
+  return MCL3DL_OK;
+}
+
+int mcl3dl_scan_accumulate_clear(mcl3dl_engine* eng)
+{
+  if (!eng || eng->devs.size() != 1)
+    return MCL3DL_ERR_INVALID_ARG;
+  DeviceCtx& c = eng->devs[0];
+  c.a_n = 0;
+  c.a_clouds = 0;
+  c.a_dense = true;
+  return MCL3DL_OK;
+}
+
+int mcl3dl_scan_accumulated_get(mcl3dl_engine* eng, mcl3dl_point* out, size_t capacity, size_t* n_out)
+{
+  if (!eng || eng->devs.size() != 1 || !n_out)
+    return MCL3DL_ERR_INVALID_ARG;
+  DeviceCtx& c = eng->devs[0];
+  *n_out = c.a_n;
+  if (!out || c.a_n == 0)
+    return MCL3DL_OK;
+  if (capacity < c.a_n)
+    return MCL3DL_ERR_INVALID_ARG;
+  CK(cudaSetDevice(c.dev));
+  CK(cudaMemcpyAsync(out, c.a_pts.p, c.a_n * 16, cudaMemcpyDeviceToHost, c.stream));
+  CK(cudaStreamSynchronize(c.stream));
+  return MCL3DL_OK;
+}
+
+int mcl3dl_scan_prepare_accumulated(mcl3dl_engine* eng, const mcl3dl_transform* tf, const mcl3dl_scan_params* sp, mcl3dl_scan_info* info)
+{
+  if (!eng || eng->devs.size() != 1 || !tf || !sp)
+    return MCL3DL_ERR_INVALID_ARG;
+  DeviceCtx& c = eng->devs[0];
+  if (c.a_clouds == 0)
+    return MCL3DL_ERR_INVALID_ARG;  // "MCL measure function is called without available pointcloud" (:312-316)
+  const uint32_t n = static_cast<uint32_t>(c.a_n);
+  return scan_prepare_from(eng, c, c.a_n, sp, info, [&](cudaStream_t st) -> int {
+    const double* t = tf->translation;
+    const double* q = tf->rotation;
+    accum_transform_kernel<<<(n + 255) / 256, 256, 0, st>>>(static_cast<const mcl3dl_point*>(c.a_pts.p), n, t[0], t[1], t[2], q[0], q[1],
+                                                           q[2], q[3], c.a_dense ? 1 : 0, static_cast<mcl3dl_point*>(c.s_raw.p));
+    CK(cudaGetLastError());
+    eng->launches++;
+    return MCL3DL_OK;
+  });
 }
 
 int mcl3dl_scan_get(mcl3dl_engine* eng, int which, mcl3dl_point* out, size_t capacity, size_t* n_out)

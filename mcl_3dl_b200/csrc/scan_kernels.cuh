@@ -24,6 +24,7 @@
 #include <stdint.h>
 
 #include "../../include/mcl3dl_b200.h"
+#include "accum_funcs.cuh"
 #include "scan_funcs.cuh"
 
 namespace mcl3dl
@@ -230,6 +231,34 @@ __global__ void ns_take_kernel(const mcl3dl_point* __restrict__ clipped, const u
     *carry_out = j + flags[k];
   if (flags[k] && j < num)
     out[j] = clipped[didx[k]];
+}
+
+// ---- cloud accumulation (mcl3dl_scan_accumulate / mcl3dl_scan_prepare_accumulated; per-point pieces: accum_funcs.cuh)
+// accumCloud: point i of the uploaded PointCloud2 (row-major), moved into the odom frame and labelled with the
+// accumulation index, at out[i]
+__global__ void accum_cloud_kernel(const unsigned char* __restrict__ data, uint32_t width, uint32_t n, uint32_t row_step,
+                                   uint32_t point_step, uint32_t ox, uint32_t oy, uint32_t oz, double tx, double ty, double tz,
+                                   double qx, double qy, double qz, double qw, uint32_t label, mcl3dl_point* __restrict__ out)
+{
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n)
+    return;
+  const AccumXform m = accum_xform(tx, ty, tz, qx, qy, qz, qw);
+  const F3 p = accum_apply(m, accum_read(data, i / width, i % width, row_step, point_step, ox, oy, oz));
+  out[i] = mcl3dl_point{p.x, p.y, p.z, label};
+}
+
+// measure()'s pcl::transformPointCloud of the whole accumulation into base_link, labels kept
+__global__ void accum_transform_kernel(const mcl3dl_point* __restrict__ in, uint32_t n, double tx, double ty, double tz, double qx,
+                                       double qy, double qz, double qw, int dense, mcl3dl_point* __restrict__ out)
+{
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n)
+    return;
+  const AccumXform m = accum_xform(tx, ty, tz, qx, qy, qz, qw);
+  const mcl3dl_point a = in[i];
+  const F3 p = accum_second(m, dense != 0, F3{a.x, a.y, a.z});
+  out[i] = mcl3dl_point{p.x, p.y, p.z, a.label};
 }
 
 }  // namespace mcl3dl

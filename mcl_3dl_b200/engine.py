@@ -97,6 +97,29 @@ class ScanInfo(C.Structure):
         return {k: int(getattr(self, k)) for k, _ in self._fields_}
 
 
+class CloudView(C.Structure):
+    """mcl3dl_cloud_view: a PointCloud2's data and layout (x, y, z FLOAT32, little-endian)."""
+    _fields_ = [("data", C.c_void_p), ("width", C.c_uint32), ("height", C.c_uint32), ("point_step", C.c_uint32),
+                ("row_step", C.c_uint32), ("offset", C.c_uint32 * 3), ("is_dense", C.c_int32)]
+
+
+class Transform(C.Structure):
+    """mcl3dl_transform: translation and RAW rotation (x y z w), doubles as a geometry_msgs/Transform carries them."""
+    _fields_ = [("translation", C.c_double * 3), ("rotation", C.c_double * 4)]
+
+    def __init__(self, translation=(0.0, 0.0, 0.0), rotation=(0.0, 0.0, 0.0, 1.0)):
+        super().__init__()
+        self.translation[:] = [float(v) for v in translation]
+        self.rotation[:] = [float(v) for v in rotation]
+
+
+def cloud_span(width, height, point_step, row_step):
+    """Bytes mcl3dl_scan_accumulate reads from a view's data: (height - 1) row_step + width point_step (0 when empty)."""
+    if width * height == 0:
+        return 0
+    return (height - 1) * row_step + width * point_step
+
+
 class NormalSamplerParams(C.Structure):
     """mcl3dl_normal_sampler_params (Engine.scan_sample_with_normal fills it)."""
     _fields_ = [("perform_weighting_ratio", C.c_double), ("max_weight_ratio", C.c_double), ("max_weight", C.c_double),
@@ -207,7 +230,9 @@ EXPORTED_SYMBOLS = ["mcl3dl_measure_update", "mcl3dl_collect_stats", "mcl3dl_rea
                     "mcl3dl_particles_resize", "mcl3dl_global_localization",
                     "mcl3dl_particles_redraw_odom_noise", "mcl3dl_particles_noise", "mcl3dl_particles_imu_update",
                     "mcl3dl_particles_landmark_update", "mcl3dl_particles_reset_odom_err_integ", "mcl3dl_particles_get_poses",
-                    "mcl3dl_particles_init", "mcl3dl_scan_sample_with_normal", "mcl3dl_scan_normals", "mcl3dl_beam_cast"]
+                    "mcl3dl_particles_init", "mcl3dl_scan_sample_with_normal", "mcl3dl_scan_normals", "mcl3dl_beam_cast",
+                    "mcl3dl_scan_accumulate", "mcl3dl_scan_accumulate_clear", "mcl3dl_scan_accumulated_get",
+                    "mcl3dl_scan_prepare_accumulated"]
 
 _LIBS = {}
 
@@ -269,6 +294,10 @@ def load_library(path=None):
     L.mcl3dl_scan_prepare.argtypes = [vp, vp, sz, vp, vp]
     L.mcl3dl_scan_get.argtypes = [vp, C.c_int, vp, sz, C.POINTER(sz)]
     L.mcl3dl_particles_measure_update_prepared.argtypes = [vp, vp, sz, C.c_float, vp]
+    L.mcl3dl_scan_accumulate.argtypes = [vp, vp, vp, C.POINTER(C.c_uint32)]
+    L.mcl3dl_scan_accumulate_clear.argtypes = [vp]
+    L.mcl3dl_scan_accumulated_get.argtypes = [vp, vp, sz, C.POINTER(sz)]
+    L.mcl3dl_scan_prepare_accumulated.argtypes = [vp, vp, vp, vp]
     L.mcl3dl_scan_sample_with_normal.argtypes = [vp, vp, vp]
     L.mcl3dl_scan_normals.argtypes = [vp, C.c_int, vp, vp, vp, sz, C.POINTER(sz)]
     L.mcl3dl_match_output.argtypes = [vp, vp, vp, sz, vp, vp, C.POINTER(sz), vp, C.POINTER(sz)]
@@ -658,6 +687,49 @@ class Engine:
         if n.value:
             self._check(self.L.mcl3dl_scan_get(self.h, which, _ptr(out), len(out), C.byref(n)))
         return out
+
+    # ---- cloud accumulation on the device (include/mcl3dl_b200.h: mcl3dl_scan_accumulate)
+    def scan_accumulate(self, data, width, height, point_step, row_step, offsets, is_dense=True,
+                        translation=(0.0, 0.0, 0.0), rotation=(0.0, 0.0, 0.0, 1.0)):
+        """accumCloud on the device: one PointCloud2 (data: a C-contiguous numpy byte or structured array holding its
+        bytes; offsets: the byte offsets of the FLOAT32 x, y, z) moved into the odom frame by (translation, RAW rotation x
+        y z w) and appended with the next accumulation index as its label.  A view that would read past the end of data
+        raises ValueError before the engine is called.  Returns the number of clouds accumulated."""
+        if not isinstance(data, np.ndarray) or not data.flags.c_contiguous:
+            raise ValueError("data must be a C-contiguous numpy array")
+        span = cloud_span(int(width), int(height), int(point_step), int(row_step))
+        if span > data.nbytes:
+            raise ValueError("the view spans %d bytes, data holds %d" % (span, data.nbytes))
+        offsets = [int(o) for o in offsets]
+        if len(offsets) != 3:
+            raise ValueError("offsets: the byte offsets of x, y, z")
+        view = CloudView(data.ctypes.data_as(C.c_void_p) if data.nbytes else None, width, height, point_step, row_step,
+                         (C.c_uint32 * 3)(*offsets), 1 if is_dense else 0)
+        tf = Transform(translation, rotation)
+        n = C.c_uint32(0)
+        self._check(self.L.mcl3dl_scan_accumulate(self.h, C.byref(view), C.byref(tf), C.byref(n)))
+        return int(n.value)
+
+    def scan_accumulate_clear(self):
+        """accumClear: empties the accumulation (the prepared scans stay)."""
+        self._check(self.L.mcl3dl_scan_accumulate_clear(self.h))
+
+    def scan_accumulated_get(self):
+        """The accumulated points in the odom frame (POINT array; label = accumulation index)."""
+        n = C.c_size_t(0)
+        self._check(self.L.mcl3dl_scan_accumulated_get(self.h, None, 0, C.byref(n)))
+        out = np.zeros(n.value, dtype=POINT)
+        if n.value:
+            self._check(self.L.mcl3dl_scan_accumulated_get(self.h, _ptr(out), len(out), C.byref(n)))
+        return out
+
+    def scan_prepare_accumulated(self, params, translation=(0.0, 0.0, 0.0), rotation=(0.0, 0.0, 0.0, 1.0)):
+        """measure() on the device: the accumulation moved into base_link by (translation, RAW rotation), then
+        scan_prepare's pipeline (params: ScanParams).  Returns the scan info as a dict."""
+        tf = Transform(translation, rotation)
+        info = ScanInfo()
+        self._check(self.L.mcl3dl_scan_prepare_accumulated(self.h, C.byref(tf), C.byref(params), C.byref(info)))
+        return info.as_dict()
 
     def scan_sample_with_normal(self, mean_rot, pos_cov, params=None, lik_num_points=96, beam_num_points=3, seed=1):
         """The node's PointCloudSamplerWithNormal on the clipped clouds of the last scan_prepare; the new samples replace

@@ -35,6 +35,7 @@
 #include <mcl_3dl/parameters.h>
 #include <mcl_3dl/pf.h>
 #include <mcl_3dl/state_6dof.h>
+#include <sensor_msgs/PointCloud2.h>
 
 #include "mcl3dl_b200.h"
 
@@ -377,6 +378,61 @@ public:
                             Vec3(r.pos[0], r.pos[1], r.pos[2]), static_cast<BeamStatus>(r.status)});
     }
   }
+  // The node's cloud accumulation on the device (mcl3dl_scan_accumulate; INTEGRATION.md, "cloud accumulation").
+  // accumCloud (src/mcl_3dl.cpp:274-302) after its tf lookup: false exactly where mcl_3dl::fromROSMsg fails (no x / y / z
+  // field, an empty cloud) and, beyond it, where x / y / z are not FLOAT32, the cloud is big-endian or its layout does
+  // not hold the points; the accumulation is then unchanged.  odom_from_sensor: the looked-up transform (translation,
+  // raw rotation x y z w).
+  bool accumulateCloud(const sensor_msgs::PointCloud2& msg, const mcl3dl_transform& odom_from_sensor)
+  {
+    mcl3dl_cloud_view v{};
+    const char* names[3] = {"x", "y", "z"};
+    for (int k = 0; k < 3; ++k)
+    {
+      const sensor_msgs::PointField* f = nullptr;
+      for (const auto& fl : msg.fields)
+        if (fl.name == names[k])
+        {
+          f = &fl;
+          break;
+        }
+      if (!f || f->datatype != sensor_msgs::PointField::FLOAT32)
+        return false;
+      v.offset[k] = f->offset;
+    }
+    const uint64_t n = static_cast<uint64_t>(msg.width) * msg.height;
+    if (msg.is_bigendian || n == 0)
+      return false;
+    const uint64_t span = static_cast<uint64_t>(msg.height - 1) * msg.row_step + static_cast<uint64_t>(msg.width) * msg.point_step;
+    if (static_cast<uint64_t>(msg.row_step) < static_cast<uint64_t>(msg.width) * msg.point_step || span > msg.data.size())
+      return false;
+    for (int k = 0; k < 3; ++k)
+      if (static_cast<uint64_t>(v.offset[k]) + 4 > msg.point_step)
+        return false;
+    v.data = msg.data.data();
+    v.width = msg.width;
+    v.height = msg.height;
+    v.point_step = msg.point_step;
+    v.row_step = msg.row_step;
+    v.is_dense = msg.is_dense ? 1 : 0;
+    check(mcl3dl_scan_accumulate(engine_, &v, &odom_from_sensor, &accumulated_clouds_), "mcl3dl_scan_accumulate");
+    return true;
+  }
+  // accumClear (:266-272)
+  void clearAccumulated()
+  {
+    check(mcl3dl_scan_accumulate_clear(engine_), "mcl3dl_scan_accumulate_clear");
+    accumulated_clouds_ = 0;
+  }
+  // measure()'s transform into base_link and the VoxelGrid / clip / sample after it (:319-383), leaving the prepared
+  // scans on the device for measureResidentPrepared-style calls (mcl3dl_particles_measure_update_prepared), matchOutput
+  // and castBeams with nullptr clouds.  Throws on an empty accumulation (the node checks pc_accum_header_ first).
+  void prepareAccumulated(const mcl3dl_transform& base_from_odom, const mcl3dl_scan_params& params, mcl3dl_scan_info* info)
+  {
+    check(mcl3dl_scan_prepare_accumulated(engine_, &base_from_odom, &params, info), "mcl3dl_scan_prepare_accumulated");
+  }
+  // clouds accumulated since the last clear (the node's pc_accum_header_.size())
+  uint32_t accumulatedClouds() const { return accumulated_clouds_; }
   void checked(int rc, const char* what) const { check(rc, what); }
   size_t likPoints() const { return lik_cloud_ ? lik_cloud_->size() : 0; }
   // How each new map reached the engine: appended (mcl3dl_map_append) or staged whole (mcl3dl_set_map).
@@ -566,6 +622,7 @@ private:
   Cloud::ConstPtr map_cloud_;              // the last setMapCloud's cloud
   uint64_t stamp_counter_ = 0;
   size_t map_appends_ = 0, map_restages_ = 0;
+  uint32_t accumulated_clouds_ = 0;
   Cloud::ConstPtr lik_cloud_, beam_cloud_;
   std::vector<mcl3dl_point> lik_pts_, beam_pts_;
   PinnedArray<mcl3dl_pose> poses_;
