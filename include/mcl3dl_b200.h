@@ -579,6 +579,68 @@ int mcl3dl_scan_accumulated_get(mcl3dl_engine*, mcl3dl_point* out, size_t capaci
 int mcl3dl_scan_prepare_accumulated(mcl3dl_engine*, const mcl3dl_transform* base_from_odom, const mcl3dl_scan_params*,
                                     mcl3dl_scan_info* info);
 
+/* ---- Map intake on the device (src/mcl_3dl.cpp:127-153, 1150-1192, 1350-1378): the received map and its update patches
+ * are converted and downsampled where they are staged, so the node runs no VoxelGrid on the map and keeps no host copy.
+ *   load (cbMapcloud / cbLoadPCD -> loadMapCloud, :1150-1170): conversion, VoxelGrid at map_downsample, then staged
+ *     exactly as mcl3dl_set_map(result, stamp, lik, beam) (it replaces the map; the same params rules and the same
+ *     rebuild trigger).  A pending patch is dropped (pc_update_.reset(), :1154).
+ *   update_set (cbMapcloudUpdate, :141-153): conversion and VoxelGrid at update_downsample into a pending patch on the
+ *     device; it replaces a pending patch.  Allowed before any map; the staged map is untouched.
+ *   update_commit (cbMapUpdateTimer, :1350-1378): mcl3dl_map_append(pending patch, stamp, info), moved device to device:
+ *     the incremental and full paths and info are those of an append of the same points.  The patch is consumed.  NO_MAP
+ *     before any map (the patch stays pending); with no pending patch OK and nothing changes (info: n_before = n_after =
+ *     the staged count, incremental = 1).  A commit appends to the staged map: after load / commit / commit the map is
+ *     the load's points, then the first patch's, then the second's.
+ *   update_clear (cbPosition, :189): drops the pending patch.
+ *   map_get: the staged map (pc_map2_, published as updated_map at :1371-1373) in staged order and one intensity per
+ *     point.  *n_out = the staged count; out == NULL: count only; INVALID_ARG when capacity is below it;
+ *     intensity_out may be NULL.  NO_MAP before any map.
+ * Conversion (fromROSMsg into PointXYZIL): point (r, c) is read at data + r row_step + c point_step + offset, points in
+ * row-major order; x / y / z (FLOAT32) are copied bit for bit; intensity from the FLOAT32 field at intensity_offset,
+ * label from the UINT32 field at label_offset, each 0 when its offset is -1 (the PointXYZIL() defaults pcl::fromROSMsg
+ * leaves when no field of that name and type exists; the caller passes an offset only for a field of the right type).
+ * VoxelGrid: exactly mcl3dl_scan_prepare's (lattice, PCL's INT32_MAX overflow rule, centroid and label
+ * vote); any leaf component <= 0 (or NaN) means no downsampling.  The intensity of a voxel is the float sum of its
+ * points' intensities in input order over float(cnt), like x / y / z.
+ * Departure: non-finite points never reach the staged map.  Downsampled, the VoxelGrid skips them; unfiltered (the
+ * overflow rule, or no leaf) they are dropped with the order kept, as KdTreeFLANN::setInputCloud does with a cloud that
+ * is not dense.  (mcl3dl_set_map takes its points as given: a NaN coordinate is ignored by the bounding box but
+ * converts to cell 0 of the likelihood grid (clamped) and of the DDA grid, where it marks the corner cell occupied; an
+ * infinite one makes the bounding box infinite, so the lattices' float-to-int conversions have no defined result.)
+ * A load that leaves no point returns INVALID_ARG with the previous map kept; a patch that leaves none is a valid
+ * empty patch, and its commit only sets the stamp (map_append with n == 0).
+ * Intensity storage: one float per staged point.  Intake stores the VoxelGrid's; mcl3dl_set_map and mcl3dl_map_append
+ * store 0 (host arrays carry none).  No kernel other than map_get's copy reads it.  It costs 4 more bytes of device
+ * memory per staged point on every device, on the set_map / map_append paths as well (not counted in device_bytes).
+ * Checks, all before data is read: INVALID_ARG for a null engine / map / data / leaf, width height == 0, row_step <
+ * width point_step, an x / y / z offset + 4 > point_step, an intensity or label offset below -1 or with offset + 4 >
+ * point_step, and (load) no params or set_map's lik params rules; TOO_LARGE for 2^30 raw points or more (the VoxelGrid's
+ * key limit, as mcl3dl_scan_prepare) and (commit) a staged total of 2^31 or more.  An error leaves the staged map and
+ * the pending patch as they were, except an error of the map build itself, which drops the map as mcl3dl_set_map's
+ * does.  The resident particle set, the prepared scans, the accumulation and the exchange buffers are untouched; in
+ * field mode the volume is restaged as by set_map / map_append.  Multi-device engines: the map and the pending patch
+ * are built on every device, with byte-identical results.  Synchronous: data is not read after the call returns.
+ * info (may be NULL): raw points, points staged (load) or pending (update_set), whether the VoxelGrid filtered, and the
+ * device time of the intake (max over devices; the map build is mcl3dl_map_info.build_ms / append_info.build_ms). */
+typedef struct
+{
+  mcl3dl_cloud_view view;   /* data, layout, FLOAT32 x / y / z offsets, is_dense */
+  int32_t intensity_offset; /* FLOAT32 "intensity" field, -1: absent */
+  int32_t label_offset;     /* UINT32 "label" field, -1: absent */
+} mcl3dl_map_cloud;
+typedef struct
+{
+  uint64_t n_input, n_staged;
+  int32_t downsampled;
+  double device_ms;
+} mcl3dl_map_intake_info;
+int mcl3dl_map_load(mcl3dl_engine*, const mcl3dl_map_cloud* map, const float leaf[3], uint64_t stamp, const mcl3dl_lik_params* lik,
+                    const mcl3dl_beam_params* beam, mcl3dl_map_intake_info* info);
+int mcl3dl_map_update_set(mcl3dl_engine*, const mcl3dl_map_cloud* patch, const float leaf[3], mcl3dl_map_intake_info* info);
+int mcl3dl_map_update_commit(mcl3dl_engine*, uint64_t stamp, mcl3dl_map_append_info* info);
+int mcl3dl_map_update_clear(mcl3dl_engine*);
+int mcl3dl_map_get(mcl3dl_engine*, mcl3dl_point* out, float* intensity_out, size_t capacity, size_t* n_out);
+
 /* The node's second sampler, PointCloudSamplerWithNormal (use_random_sampler_with_normal; point_cloud_random_samplers/
  * point_cloud_sampler_with_normal.h), on the clipped clouds the last mcl3dl_scan_prepare left on the device, once per
  * model.  It REPLACES that call's sampled scans (scan_get(3 | 4), particles_measure_update_prepared); the downsampled and

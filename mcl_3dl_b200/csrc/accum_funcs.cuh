@@ -75,16 +75,48 @@ __device__ __forceinline__ float accum_load_f32(const unsigned char* p)
   return __uint_as_float(b);
 }
 
+// the first byte of point (r, c) of a PointCloud2: data + r row_step + c point_step
+__device__ __forceinline__ const unsigned char* cloud_point_at(const unsigned char* data, uint32_t r, uint32_t c, uint32_t row_step,
+                                                               uint32_t point_step)
+{
+  return data + static_cast<uint64_t>(r) * row_step + static_cast<uint64_t>(c) * point_step;
+}
+
 // point (r, c) of a PointCloud2: data + r row_step + c point_step + offset[i]
 __device__ __forceinline__ F3 accum_read(const unsigned char* data, uint32_t r, uint32_t c, uint32_t row_step, uint32_t point_step,
                                          uint32_t ox, uint32_t oy, uint32_t oz)
 {
-  const unsigned char* p = data + static_cast<uint64_t>(r) * row_step + static_cast<uint64_t>(c) * point_step;
+  const unsigned char* p = cloud_point_at(data, r, c, row_step, point_step);
   F3 o;
   o.x = accum_load_f32(p + ox);
   o.y = accum_load_f32(p + oy);
   o.z = accum_load_f32(p + oz);
   return o;
+}
+
+// ---- map intake (mcl3dl_map_load / mcl3dl_map_update_set): fromROSMsg into PointXYZIL, no transform
+// point (r, c) of a map cloud: x / y / z bits as they are; label from the UINT32 field at lo, intensity from the FLOAT32
+// field at io, each 0 when its offset is negative (the PointXYZIL() defaults fromROSMsg leaves for a missing field)
+__device__ __forceinline__ mcl3dl_point map_read(const unsigned char* data, uint32_t r, uint32_t c, uint32_t row_step, uint32_t point_step,
+                                                 uint32_t ox, uint32_t oy, uint32_t oz, int32_t io, int32_t lo, float& intensity)
+{
+  const unsigned char* p = cloud_point_at(data, r, c, row_step, point_step);
+  mcl3dl_point o;
+  o.x = accum_load_f32(p + ox);
+  o.y = accum_load_f32(p + oy);
+  o.z = accum_load_f32(p + oz);
+  o.label = lo >= 0 ? __float_as_uint(accum_load_f32(p + lo)) : 0u;
+  intensity = io >= 0 ? accum_load_f32(p + io) : 0.0f;
+  return o;
+}
+
+// the intensity of one voxel: the float sum of in[order[0..cnt)] in input order over float(cnt), as x / y / z in
+// scan_voxel_point
+__device__ __forceinline__ float map_voxel_intensity(const float* __restrict__ in, const uint32_t* __restrict__ order, uint32_t cnt)
+{
+  float s = 0.0f;
+  for (uint32_t j = 0; j < cnt; ++j) s = fadd(s, in[order[j]]);
+  return fdiv(s, static_cast<float>(cnt));
 }
 
 }  // namespace mcl3dl

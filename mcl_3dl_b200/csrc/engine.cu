@@ -506,6 +506,12 @@ struct DeviceCtx
   size_t a_n = 0;
   uint32_t a_clouds = 0;
   bool a_dense = true;
+  // map intake (mcl3dl_map_load / mcl3dl_map_update_*): one intensity per staged point (mcl3dl_map_get; no kernel of the
+  // models reads it); the pending patch and its intensities; the intake's raw bytes, converted cloud and intensities,
+  // result and its intensities, VoxelGrid sort keys / values / (voxel, label) keys (x2), flags + scan positions, cub
+  // scratch, device-side count
+  DevBuf map_int, p_pts, p_int;
+  DevBuf i_raw, i_cloud, i_cloud_int, i_pts, i_int, i_keys[2], i_vals[2], i_kl[2], i_flags, i_pos, i_tmp, i_count;
   // normal-weighted sampler (mcl3dl_scan_sample_with_normal): neighbour-grid sort keys / values (x2), sorted points; per
   // model the normals, neighbour counts and fixed-point weights of its clipped points (mcl3dl_scan_normals); the inclusive
   // sum of the weights, each point's first draw, a round's draw indices / flags / scan positions, the new sampled scans,
@@ -545,6 +551,8 @@ struct mcl3dl_engine
 {
   std::vector<DeviceCtx> devs;
   bool has_map = false;
+  bool has_patch = false;  // mcl3dl_map_update_set left a pending patch (DeviceCtx::p_pts) of patch_n points
+  size_t patch_n = 0;
   bool has_lik = false, has_beam = false;
   uint64_t stamp = 0;
   size_t n_points = 0;
@@ -1609,10 +1617,20 @@ struct VoxelBufs
 // one centroid per voxel in ascending voxel index).  done: the pass wrote the downsampled cloud to out and its size to
 // *d_count; false when the cloud passes unfiltered (out and *d_count untouched).  With no finite point, done is true and
 // nothing is written: the caller's zeroed count stands.  cap: the capacity the vote's keys are reserved for (>= n).
+// runs (may be NULL): when the pass sorted, the voxel runs stay for the caller (map_intensity_kernel): b.keys[1] the
+// sorted keys, b.vals[1] the input index in that order, b.flags the run heads, b.pos their output positions, and the
+// run with key runs->nonfinite_key holds the non-finite points (no voxel).
+struct VoxelRuns
+{
+  bool sorted = false;
+  uint32_t nonfinite_key = 0;
+};
 int voxel_grid(mcl3dl_engine* eng, DeviceCtx& c, cudaStream_t st, const mcl3dl_point* in, uint32_t n, size_t cap, const float leaf[3],
-               const VoxelBufs& b, mcl3dl_point* out, uint32_t* d_count, bool& done)
+               const VoxelBufs& b, mcl3dl_point* out, uint32_t* d_count, bool& done, VoxelRuns* runs = nullptr)
 {
   done = false;
+  if (runs)
+    *runs = VoxelRuns{};
   int rc;
   const int nb = static_cast<int>((n + 255) / 256);
   // bounding box of the finite points -> VoxelGrid lattice and PCL's overflow rule (scan_voxel_lattice)
@@ -1661,6 +1679,8 @@ int voxel_grid(mcl3dl_engine* eng, DeviceCtx& c, cudaStream_t st, const mcl3dl_p
   CK(cudaGetLastError());
   eng->launches += 6;
   done = true;
+  if (runs)
+    *runs = VoxelRuns{true, g.cells};
   return MCL3DL_OK;
 }
 
@@ -1922,13 +1942,14 @@ void mcl3dl_destroy(mcl3dl_engine* eng)
   delete eng;
 }
 
-int mcl3dl_set_map(mcl3dl_engine* eng, const mcl3dl_point* pts, size_t n, uint64_t stamp, const mcl3dl_lik_params* lik,
-                   const mcl3dl_beam_params* beam)
+// mcl3dl_set_map from its points on: `fill(c, d_pts, d_int)` leaves the n points and their intensities in the two
+// buffers of device c on c.stream (a host upload, or the map intake's result moved in), then the build on every device.
+// fill is not called when the reference's rebuild trigger finds nothing to do.
+extern "C++" {
+template <typename Fill>
+static int set_map_from(mcl3dl_engine* eng, size_t n, uint64_t stamp, const mcl3dl_lik_params* lik, const mcl3dl_beam_params* beam,
+                        Fill fill)
 {
-  if (!eng || !pts || n == 0 || (!lik && !beam))
-    return MCL3DL_ERR_INVALID_ARG;
-  if (n >= (size_t(1) << 31))
-    return MCL3DL_ERR_TOO_LARGE;
   // the reference's rebuild trigger: same header.stamp (and a non-empty index) -> nothing to do
   // (raycast_using_dda.h:168)
   if (eng->has_map && eng->stamp == stamp && eng->n_points == n &&
@@ -1952,16 +1973,16 @@ int mcl3dl_set_map(mcl3dl_engine* eng, const mcl3dl_point* pts, size_t n, uint64
   eng->info.n_points = n;
   for (DeviceCtx& c : eng->devs)
   {
-    DevBuf d_pts;
+    DevBuf d_pts, d_int;
     int rc = MCL3DL_OK;
     CK(cudaSetDevice(c.dev));
-    if ((rc = reserve(eng, d_pts, n * sizeof(mcl3dl_point))))
+    if ((rc = fill(c, d_pts, d_int)))
       return rc;
-    CK(cudaMemcpyAsync(d_pts.p, pts, n * sizeof(mcl3dl_point), cudaMemcpyHostToDevice, c.stream));
     uint64_t reselected = 0;
     bool incremental = false;
     if ((rc = build_map_on_device(eng, c, d_pts, n, 0, reselected, incremental)) || (rc = restage_field(eng, c)))
       return rc;
+    c.map_int = std::move(d_int);
   }
   eng->has_map = true;
   eng->stamp = stamp;
@@ -1969,17 +1990,12 @@ int mcl3dl_set_map(mcl3dl_engine* eng, const mcl3dl_point* pts, size_t n, uint64
   return MCL3DL_OK;
 }
 
-int mcl3dl_map_append(mcl3dl_engine* eng, const mcl3dl_point* pts, size_t n, uint64_t stamp, mcl3dl_map_append_info* info)
+// mcl3dl_map_append from its count on: `fill(c, pts, inten)` writes the n new points and their intensities at the two
+// device pointers (after the staged ones) on c.stream
+template <typename Fill>
+static int map_append_from(mcl3dl_engine* eng, size_t n, uint64_t stamp, mcl3dl_map_append_info* info, Fill fill)
 {
-  if (!eng)
-    return MCL3DL_ERR_INVALID_ARG;
-  if (!eng->has_map)
-    return MCL3DL_ERR_NO_MAP;
-  if (!pts && n > 0)
-    return MCL3DL_ERR_INVALID_ARG;
   const size_t n_before = eng->n_points;
-  if (n >= (size_t(1) << 31) || n_before + n >= (size_t(1) << 31))
-    return MCL3DL_ERR_TOO_LARGE;
   mcl3dl_map_append_info r{};
   r.n_before = n_before;
   r.n_appended = n;
@@ -1994,19 +2010,21 @@ int mcl3dl_map_append(mcl3dl_engine* eng, const mcl3dl_point* pts, size_t n, uin
     for (DeviceCtx& c : eng->devs)
     {
       // the staged points followed by the new ones, joined on the device: the base map does not cross the bus again
-      DevBuf d_pts;
+      DevBuf d_pts, d_int;
       int rc = MCL3DL_OK;
       CK(cudaSetDevice(c.dev));
-      if ((rc = reserve(eng, d_pts, r.n_after * sizeof(mcl3dl_point))))
+      if ((rc = reserve(eng, d_pts, r.n_after * sizeof(mcl3dl_point))) || (rc = reserve(eng, d_int, r.n_after * sizeof(float))))
         return rc;
       CK(cudaEventRecord(c.ev[2], c.stream));
       CK(cudaMemcpyAsync(d_pts.p, c.raw_pts.p, n_before * sizeof(mcl3dl_point), cudaMemcpyDeviceToDevice, c.stream));
-      CK(cudaMemcpyAsync(static_cast<mcl3dl_point*>(d_pts.p) + n_before, pts, n * sizeof(mcl3dl_point),
-                         cudaMemcpyHostToDevice, c.stream));
+      CK(cudaMemcpyAsync(d_int.p, c.map_int.p, n_before * sizeof(float), cudaMemcpyDeviceToDevice, c.stream));
+      if ((rc = fill(c, static_cast<mcl3dl_point*>(d_pts.p) + n_before, static_cast<float*>(d_int.p) + n_before)))
+        return rc;
       uint64_t reselected = 0;
       bool incremental = false;
       if ((rc = build_map_on_device(eng, c, d_pts, r.n_after, n_before, reselected, incremental)))
         return rc;
+      c.map_int = std::move(d_int);
       r.incremental = &c == &eng->devs[0] ? incremental : r.incremental && incremental;
       r.cells_reselected = std::max(r.cells_reselected, reselected);
       float ms = 0;
@@ -2021,6 +2039,285 @@ int mcl3dl_map_append(mcl3dl_engine* eng, const mcl3dl_point* pts, size_t n, uin
   eng->stamp = stamp;
   if (info)
     *info = r;
+  return MCL3DL_OK;
+}
+}  // extern "C++"
+
+int mcl3dl_set_map(mcl3dl_engine* eng, const mcl3dl_point* pts, size_t n, uint64_t stamp, const mcl3dl_lik_params* lik,
+                   const mcl3dl_beam_params* beam)
+{
+  if (!eng || !pts || n == 0 || (!lik && !beam))
+    return MCL3DL_ERR_INVALID_ARG;
+  if (n >= (size_t(1) << 31))
+    return MCL3DL_ERR_TOO_LARGE;
+  return set_map_from(eng, n, stamp, lik, beam, [&](DeviceCtx& c, DevBuf& d_pts, DevBuf& d_int) -> int {
+    int rc;
+    if ((rc = reserve(eng, d_pts, n * sizeof(mcl3dl_point))) || (rc = reserve(eng, d_int, n * sizeof(float))))
+      return rc;
+    CK(cudaMemcpyAsync(d_pts.p, pts, n * sizeof(mcl3dl_point), cudaMemcpyHostToDevice, c.stream));
+    CK(cudaMemsetAsync(d_int.p, 0, n * sizeof(float), c.stream));  // host arrays carry no intensity
+    return MCL3DL_OK;
+  });
+}
+
+int mcl3dl_map_append(mcl3dl_engine* eng, const mcl3dl_point* pts, size_t n, uint64_t stamp, mcl3dl_map_append_info* info)
+{
+  if (!eng)
+    return MCL3DL_ERR_INVALID_ARG;
+  if (!eng->has_map)
+    return MCL3DL_ERR_NO_MAP;
+  if (!pts && n > 0)
+    return MCL3DL_ERR_INVALID_ARG;
+  if (n >= (size_t(1) << 31) || eng->n_points + n >= (size_t(1) << 31))
+    return MCL3DL_ERR_TOO_LARGE;
+  return map_append_from(eng, n, stamp, info, [&](DeviceCtx& c, mcl3dl_point* d_pts, float* d_int) -> int {
+    CK(cudaMemcpyAsync(d_pts, pts, n * sizeof(mcl3dl_point), cudaMemcpyHostToDevice, c.stream));
+    CK(cudaMemsetAsync(d_int, 0, n * sizeof(float), c.stream));
+    return MCL3DL_OK;
+  });
+}
+
+// ---- map intake (scan_kernels.cuh: map_*_kernel)
+// The checks of mcl3dl_map_load / mcl3dl_map_update_set, all before data is read
+static int check_map_cloud(const mcl3dl_engine* eng, const mcl3dl_map_cloud* m, const float* leaf)
+{
+  if (!eng || !m || !m->view.data || !leaf)
+    return MCL3DL_ERR_INVALID_ARG;
+  const mcl3dl_cloud_view& v = m->view;
+  const uint64_t n = static_cast<uint64_t>(v.width) * v.height;
+  if (n == 0 || static_cast<uint64_t>(v.row_step) < static_cast<uint64_t>(v.width) * v.point_step)
+    return MCL3DL_ERR_INVALID_ARG;
+  for (int k = 0; k < 3; ++k)
+    if (static_cast<uint64_t>(v.offset[k]) + 4 > v.point_step)
+      return MCL3DL_ERR_INVALID_ARG;
+  for (const int32_t o : {m->intensity_offset, m->label_offset})
+    if (o < -1 || (o >= 0 && static_cast<uint64_t>(o) + 4 > v.point_step))
+      return MCL3DL_ERR_INVALID_ARG;
+  if (n >= (uint64_t(1) << 30))
+    return MCL3DL_ERR_TOO_LARGE;  // the VoxelGrid's key limit, as mcl3dl_scan_prepare's
+  return MCL3DL_OK;
+}
+
+// One map cloud on device c: its bytes up, the conversion, then the VoxelGrid at `leaf` with the intensity centroid, or,
+// when the cloud passes unfiltered, its finite points in order.  The result goes to c.i_pts / c.i_int (n_out points);
+// downsampled: the VoxelGrid filtered.  Nothing but the intake's own buffers changes.
+static int map_intake(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_map_cloud* m, const float leaf[3], uint32_t& n_out, bool& downsampled,
+                      float& ms)
+{
+  const mcl3dl_cloud_view& v = m->view;
+  const uint32_t n = v.width * v.height;
+  const size_t bytes = static_cast<size_t>(v.height - 1) * v.row_step + static_cast<size_t>(v.width) * v.point_step;
+  CK(cudaSetDevice(c.dev));
+  cudaStream_t st = c.stream;
+  int rc;
+  if ((rc = reserve(eng, c.i_raw, bytes)) || (rc = reserve(eng, c.i_cloud, size_t(n) * 16)) || (rc = reserve(eng, c.i_cloud_int, size_t(n) * 4)) ||
+      (rc = reserve(eng, c.i_pts, size_t(n) * 16)) || (rc = reserve(eng, c.i_int, size_t(n) * 4)) ||
+      (rc = reserve(eng, c.i_flags, size_t(n) * 4)) || (rc = reserve(eng, c.i_pos, size_t(n) * 4)) || (rc = reserve(eng, c.i_count, 64)) ||
+      (rc = reserve(eng, c.h_pinned, 256)))
+    return rc;
+  for (int k = 0; k < 2; ++k)
+    if ((rc = reserve(eng, c.i_keys[k], size_t(n) * 4)) || (rc = reserve(eng, c.i_vals[k], size_t(n) * 4)))
+      return rc;
+  CK(cudaEventRecord(c.ev[0], st));
+  CK(cudaMemcpyAsync(c.i_raw.p, v.data, bytes, cudaMemcpyHostToDevice, st));
+  mcl3dl_point* in = static_cast<mcl3dl_point*>(c.i_cloud.p);
+  float* in_int = static_cast<float*>(c.i_cloud_int.p);
+  const int nb = static_cast<int>((n + 255) / 256);
+  map_read_kernel<<<nb, 256, 0, st>>>(static_cast<const unsigned char*>(c.i_raw.p), v.width, n, v.row_step, v.point_step, v.offset[0],
+                                      v.offset[1], v.offset[2], m->intensity_offset, m->label_offset, in, in_int);
+  CK(cudaGetLastError());
+  eng->launches++;
+  uint32_t* count = static_cast<uint32_t*>(c.i_count.p);
+  CK(cudaMemsetAsync(count, 0, 64, st));
+  mcl3dl_point* out = static_cast<mcl3dl_point*>(c.i_pts.p);
+  float* out_int = static_cast<float*>(c.i_int.p);
+  bool done = false;
+  VoxelRuns runs;
+  if (leaf[0] > 0.0f && leaf[1] > 0.0f && leaf[2] > 0.0f)
+  {
+    const VoxelBufs vb{{&c.i_keys[0], &c.i_keys[1]}, {&c.i_vals[0], &c.i_vals[1]}, {&c.i_kl[0], &c.i_kl[1]}, &c.i_flags, &c.i_pos, &c.i_tmp};
+    if ((rc = voxel_grid(eng, c, st, in, n, n, leaf, vb, out, count, done, &runs)))
+      return rc;
+  }
+  if (runs.sorted)
+  {
+    map_intensity_kernel<<<nb, 256, 0, st>>>(static_cast<const uint32_t*>(c.i_keys[1].p), static_cast<const uint32_t*>(c.i_vals[1].p),
+                                             static_cast<const uint32_t*>(c.i_flags.p), static_cast<const uint32_t*>(c.i_pos.p), n,
+                                             runs.nonfinite_key, in_int, out_int);
+    CK(cudaGetLastError());
+    eng->launches++;
+  }
+  downsampled = done;
+  if (!done)
+  {
+    // unfiltered: the finite points in order (a KdTreeFLANN input drops the others; the grids would index them)
+    uint32_t* fl = static_cast<uint32_t*>(c.i_flags.p);
+    uint32_t* ps = static_cast<uint32_t*>(c.i_pos.p);
+    map_finite_flags_kernel<<<nb, 256, 0, st>>>(in, n, fl);
+    CK(cudaGetLastError());
+    size_t t_scan = 0;
+    CK(cub::DeviceScan::ExclusiveSum(nullptr, t_scan, fl, ps, n, st));
+    if ((rc = reserve(eng, c.i_tmp, t_scan + 256)))
+      return rc;
+    size_t tsz = c.i_tmp.cap;
+    CK(cub::DeviceScan::ExclusiveSum(c.i_tmp.p, tsz, fl, ps, n, st));
+    map_compact_kernel<<<nb, 256, 0, st>>>(in, in_int, fl, ps, n, out, out_int, count);
+    CK(cudaGetLastError());
+    eng->launches += 3;
+  }
+  CK(cudaMemcpyAsync(c.h_pinned.p, count, 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaEventRecord(c.ev[1], st));
+  CK(cudaStreamSynchronize(st));  // the caller may reuse data as soon as this returns
+  CK(cudaEventElapsedTime(&ms, c.ev[0], c.ev[1]));
+  n_out = *static_cast<const uint32_t*>(c.h_pinned.p);
+  return MCL3DL_OK;
+}
+
+// The intake's result (c.i_pts / c.i_int, reserved for the raw count) into buffers of its own size
+static int exact_copy(mcl3dl_engine* eng, DeviceCtx& c, size_t n, DevBuf& pts, DevBuf& inten)
+{
+  int rc;
+  CK(cudaSetDevice(c.dev));
+  if ((rc = reserve(eng, pts, std::max<size_t>(n, 1) * sizeof(mcl3dl_point))) || (rc = reserve(eng, inten, std::max<size_t>(n, 1) * sizeof(float))))
+    return rc;
+  CK(cudaMemcpyAsync(pts.p, c.i_pts.p, n * sizeof(mcl3dl_point), cudaMemcpyDeviceToDevice, c.stream));
+  CK(cudaMemcpyAsync(inten.p, c.i_int.p, n * sizeof(float), cudaMemcpyDeviceToDevice, c.stream));
+  return MCL3DL_OK;
+}
+
+// map_intake on every device; an engine whose devices disagree on the count is a fault of the engine
+static int map_intake_all(mcl3dl_engine* eng, const mcl3dl_map_cloud* m, const float leaf[3], mcl3dl_map_intake_info& info)
+{
+  info = mcl3dl_map_intake_info{};
+  info.n_input = static_cast<uint64_t>(m->view.width) * m->view.height;
+  for (DeviceCtx& c : eng->devs)
+  {
+    uint32_t n_out = 0;
+    bool ds = false;
+    float ms = 0;
+    const int rc = map_intake(eng, c, m, leaf, n_out, ds, ms);
+    if (rc)
+      return rc;
+    if (&c != &eng->devs[0] && (n_out != info.n_staged || (ds ? 1 : 0) != info.downsampled))
+    {
+      eng->err = "map intake: the devices disagree";
+      return MCL3DL_ERR_CUDA;
+    }
+    info.n_staged = n_out;
+    info.downsampled = ds ? 1 : 0;
+    info.device_ms = std::max(info.device_ms, static_cast<double>(ms));
+  }
+  return MCL3DL_OK;
+}
+
+int mcl3dl_map_load(mcl3dl_engine* eng, const mcl3dl_map_cloud* map, const float leaf[3], uint64_t stamp, const mcl3dl_lik_params* lik,
+                    const mcl3dl_beam_params* beam, mcl3dl_map_intake_info* info)
+{
+  int rc;
+  if ((rc = check_map_cloud(eng, map, leaf)))
+    return rc;
+  if ((!lik && !beam) || (lik && (!(lik->match_dist_min > 0.0f) || !(lik->dist_weight[0] > 0.0f) ||
+                                  !(lik->dist_weight[1] > 0.0f) || !(lik->dist_weight[2] > 0.0f))))
+    return MCL3DL_ERR_INVALID_ARG;
+  mcl3dl_map_intake_info r;
+  if ((rc = map_intake_all(eng, map, leaf, r)))
+    return rc;
+  if (r.n_staged == 0)
+    return MCL3DL_ERR_INVALID_ARG;  // no finite point: the previous map stays, as set_map refuses n == 0
+  const size_t n = r.n_staged;
+  rc = set_map_from(eng, n, stamp, lik, beam, [&](DeviceCtx& c, DevBuf& d_pts, DevBuf& d_int) -> int {
+    return exact_copy(eng, c, n, d_pts, d_int);
+  });
+  if (rc)
+    return rc;
+  eng->has_patch = false;  // loadMapCloud: pc_update_.reset()
+  if (info)
+    *info = r;
+  return MCL3DL_OK;
+}
+
+int mcl3dl_map_update_set(mcl3dl_engine* eng, const mcl3dl_map_cloud* patch, const float leaf[3], mcl3dl_map_intake_info* info)
+{
+  int rc;
+  if ((rc = check_map_cloud(eng, patch, leaf)))
+    return rc;
+  mcl3dl_map_intake_info r;
+  if ((rc = map_intake_all(eng, patch, leaf, r)))
+    return rc;
+  // the new patch replaces the pending one (copied first on every device: an error keeps the pending patch)
+  std::vector<DevBuf> pts(eng->devs.size()), inten(eng->devs.size());
+  for (size_t k = 0; k < eng->devs.size(); ++k)
+    if ((rc = exact_copy(eng, eng->devs[k], r.n_staged, pts[k], inten[k])))
+      return rc;
+  for (size_t k = 0; k < eng->devs.size(); ++k)
+  {
+    eng->devs[k].p_pts = std::move(pts[k]);
+    eng->devs[k].p_int = std::move(inten[k]);
+  }
+  eng->has_patch = true;
+  eng->patch_n = r.n_staged;
+  if (info)
+    *info = r;
+  return MCL3DL_OK;
+}
+
+int mcl3dl_map_update_commit(mcl3dl_engine* eng, uint64_t stamp, mcl3dl_map_append_info* info)
+{
+  if (!eng)
+    return MCL3DL_ERR_INVALID_ARG;
+  if (!eng->has_map)
+    return MCL3DL_ERR_NO_MAP;  // the patch stays pending
+  if (!eng->has_patch)
+  {
+    // cbMapUpdateTimer without pc_update_: nothing changes
+    if (info)
+    {
+      *info = mcl3dl_map_append_info{};
+      info->n_before = info->n_after = eng->n_points;
+      info->incremental = 1;
+    }
+    return MCL3DL_OK;
+  }
+  const size_t n = eng->patch_n;
+  if (eng->n_points + n >= (size_t(1) << 31))
+    return MCL3DL_ERR_TOO_LARGE;
+  const int rc = map_append_from(eng, n, stamp, info, [&](DeviceCtx& c, mcl3dl_point* d_pts, float* d_int) -> int {
+    CK(cudaMemcpyAsync(d_pts, c.p_pts.p, n * sizeof(mcl3dl_point), cudaMemcpyDeviceToDevice, c.stream));
+    CK(cudaMemcpyAsync(d_int, c.p_int.p, n * sizeof(float), cudaMemcpyDeviceToDevice, c.stream));
+    return MCL3DL_OK;
+  });
+  if (rc)
+    return rc;
+  eng->has_patch = false;
+  return MCL3DL_OK;
+}
+
+int mcl3dl_map_update_clear(mcl3dl_engine* eng)
+{
+  if (!eng)
+    return MCL3DL_ERR_INVALID_ARG;
+  eng->has_patch = false;
+  return MCL3DL_OK;
+}
+
+int mcl3dl_map_get(mcl3dl_engine* eng, mcl3dl_point* out, float* intensity_out, size_t capacity, size_t* n_out)
+{
+  if (!eng || !n_out)
+    return MCL3DL_ERR_INVALID_ARG;
+  if (!eng->has_map)
+    return MCL3DL_ERR_NO_MAP;
+  const size_t n = eng->n_points;
+  *n_out = n;
+  if (!out)
+    return MCL3DL_OK;
+  if (capacity < n)
+    return MCL3DL_ERR_INVALID_ARG;
+  DeviceCtx& c = eng->devs[0];
+  CK(cudaSetDevice(c.dev));
+  CK(cudaMemcpyAsync(out, c.raw_pts.p, n * sizeof(mcl3dl_point), cudaMemcpyDeviceToHost, c.stream));
+  if (intensity_out)
+    CK(cudaMemcpyAsync(intensity_out, c.map_int.p, n * sizeof(float), cudaMemcpyDeviceToHost, c.stream));
+  CK(cudaStreamSynchronize(c.stream));
   return MCL3DL_OK;
 }
 

@@ -261,4 +261,61 @@ __global__ void accum_transform_kernel(const mcl3dl_point* __restrict__ in, uint
   out[i] = mcl3dl_point{p.x, p.y, p.z, a.label};
 }
 
+// ---- map intake (mcl3dl_map_load / mcl3dl_map_update_set; per-point pieces: accum_funcs.cuh)
+// fromROSMsg: point i of the uploaded map cloud (row-major) at pts[i], its intensity at inten[i]
+__global__ void map_read_kernel(const unsigned char* __restrict__ data, uint32_t width, uint32_t n, uint32_t row_step, uint32_t point_step,
+                                uint32_t ox, uint32_t oy, uint32_t oz, int32_t io, int32_t lo, mcl3dl_point* __restrict__ pts,
+                                float* __restrict__ inten)
+{
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n)
+    return;
+  float v;
+  pts[i] = map_read(data, i / width, i % width, row_step, point_step, ox, oy, oz, io, lo, v);
+  inten[i] = v;
+}
+
+// one thread per voxel head of voxel_grid's sorted runs (keys, order, flags, pos as scan_centroid_kernel reads them; see
+// VoxelRuns in engine.cu): the voxel's intensity at out[pos[i]], the index its centroid has.  The run with key
+// nonfinite_key (the non-finite points) is no voxel, as in scan_centroid_kernel.
+__global__ void map_intensity_kernel(const uint32_t* __restrict__ keys, const uint32_t* __restrict__ order,
+                                     const uint32_t* __restrict__ flags, const uint32_t* __restrict__ pos, uint32_t n,
+                                     uint32_t nonfinite_key, const float* __restrict__ inten, float* __restrict__ out)
+{
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n || !flags[i])
+    return;
+  const uint32_t key = keys[i];
+  if (key == nonfinite_key)
+    return;
+  uint32_t cnt = 1;
+  while (i + cnt < n && keys[i + cnt] == key) ++cnt;
+  out[pos[i]] = map_voxel_intensity(inten, order + i, cnt);
+}
+
+// the unfiltered map (PCL's overflow rule, or no leaf): flag[i] = 1 for a finite point
+__global__ void map_finite_flags_kernel(const mcl3dl_point* __restrict__ pts, uint32_t n, uint32_t* __restrict__ flags)
+{
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n)
+    flags[i] = point_finite(pts[i]) ? 1u : 0u;
+}
+
+// the flagged points and their intensities, order kept; *n_out = their count
+__global__ void map_compact_kernel(const mcl3dl_point* __restrict__ pts, const float* __restrict__ inten,
+                                   const uint32_t* __restrict__ flags, const uint32_t* __restrict__ pos, uint32_t n,
+                                   mcl3dl_point* __restrict__ out, float* __restrict__ out_inten, uint32_t* __restrict__ n_out)
+{
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n)
+    return;
+  if (i == n - 1)
+    *n_out = pos[i] + flags[i];
+  if (flags[i])
+  {
+    out[pos[i]] = pts[i];
+    out_inten[pos[i]] = inten[i];
+  }
+}
+
 }  // namespace mcl3dl

@@ -113,6 +113,19 @@ class Transform(C.Structure):
         self.rotation[:] = [float(v) for v in rotation]
 
 
+class MapCloud(C.Structure):
+    """mcl3dl_map_cloud: a map PointCloud2's view (x, y, z FLOAT32) and the byte offsets of its FLOAT32 "intensity" and
+    UINT32 "label" fields (-1: absent)."""
+    _fields_ = [("view", CloudView), ("intensity_offset", C.c_int32), ("label_offset", C.c_int32)]
+
+
+class MapIntakeInfo(C.Structure):
+    _fields_ = [("n_input", C.c_uint64), ("n_staged", C.c_uint64), ("downsampled", C.c_int32), ("device_ms", C.c_double)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
 def cloud_span(width, height, point_step, row_step):
     """Bytes mcl3dl_scan_accumulate reads from a view's data: (height - 1) row_step + width point_step (0 when empty)."""
     if width * height == 0:
@@ -232,7 +245,8 @@ EXPORTED_SYMBOLS = ["mcl3dl_measure_update", "mcl3dl_collect_stats", "mcl3dl_rea
                     "mcl3dl_particles_landmark_update", "mcl3dl_particles_reset_odom_err_integ", "mcl3dl_particles_get_poses",
                     "mcl3dl_particles_init", "mcl3dl_scan_sample_with_normal", "mcl3dl_scan_normals", "mcl3dl_beam_cast",
                     "mcl3dl_scan_accumulate", "mcl3dl_scan_accumulate_clear", "mcl3dl_scan_accumulated_get",
-                    "mcl3dl_scan_prepare_accumulated"]
+                    "mcl3dl_scan_prepare_accumulated", "mcl3dl_map_load", "mcl3dl_map_update_set",
+                    "mcl3dl_map_update_commit", "mcl3dl_map_update_clear", "mcl3dl_map_get"]
 
 _LIBS = {}
 
@@ -296,6 +310,11 @@ def load_library(path=None):
     L.mcl3dl_particles_measure_update_prepared.argtypes = [vp, vp, sz, C.c_float, vp]
     L.mcl3dl_scan_accumulate.argtypes = [vp, vp, vp, C.POINTER(C.c_uint32)]
     L.mcl3dl_scan_accumulate_clear.argtypes = [vp]
+    L.mcl3dl_map_load.argtypes = [vp, vp, vp, C.c_uint64, vp, vp, vp]
+    L.mcl3dl_map_update_set.argtypes = [vp, vp, vp, vp]
+    L.mcl3dl_map_update_commit.argtypes = [vp, C.c_uint64, vp]
+    L.mcl3dl_map_update_clear.argtypes = [vp]
+    L.mcl3dl_map_get.argtypes = [vp, vp, vp, sz, C.POINTER(sz)]
     L.mcl3dl_scan_accumulated_get.argtypes = [vp, vp, sz, C.POINTER(sz)]
     L.mcl3dl_scan_prepare_accumulated.argtypes = [vp, vp, vp, vp]
     L.mcl3dl_scan_sample_with_normal.argtypes = [vp, vp, vp]
@@ -730,6 +749,81 @@ class Engine:
         info = ScanInfo()
         self._check(self.L.mcl3dl_scan_prepare_accumulated(self.h, C.byref(tf), C.byref(params), C.byref(info)))
         return info.as_dict()
+
+    # ---- map intake on the device (include/mcl3dl_b200.h: mcl3dl_map_load)
+    @staticmethod
+    def _map_cloud(data, width, height, point_step, row_step, offsets, intensity_offset, label_offset, is_dense):
+        if not isinstance(data, np.ndarray) or not data.flags.c_contiguous:
+            raise ValueError("data must be a C-contiguous numpy array")
+        span = cloud_span(int(width), int(height), int(point_step), int(row_step))
+        if span > data.nbytes:
+            raise ValueError("the view spans %d bytes, data holds %d" % (span, data.nbytes))
+        offsets = [int(o) for o in offsets]
+        if len(offsets) != 3:
+            raise ValueError("offsets: the byte offsets of x, y, z")
+        io = -1 if intensity_offset is None else int(intensity_offset)
+        lo = -1 if label_offset is None else int(label_offset)
+        view = CloudView(data.ctypes.data_as(C.c_void_p) if data.nbytes else None, width, height, point_step, row_step,
+                         (C.c_uint32 * 3)(*offsets), 1 if is_dense else 0)
+        return MapCloud(view, io, lo)
+
+    @staticmethod
+    def _leaf(leaf):
+        leaf = np.ascontiguousarray(leaf, dtype=np.float32)
+        if leaf.shape != (3,):
+            raise ValueError("leaf: three leaf sizes")
+        return leaf
+
+    def map_load(self, data, width, height, point_step, row_step, offsets, leaf, lik=None, beam=None, intensity_offset=None,
+                 label_offset=None, is_dense=True, stamp=None):
+        """loadMapCloud on the device: one map PointCloud2 (data: a C-contiguous numpy array holding its bytes; offsets:
+        the byte offsets of the FLOAT32 x, y, z; intensity_offset / label_offset: the FLOAT32 intensity and UINT32 label
+        fields, None when absent) converted, downsampled at leaf and staged as set_map stages a map (stamp as there).  A
+        view that would read past the end of data raises ValueError before the engine is called.  Returns
+        {"n_input", "n_staged", "downsampled", "device_ms"}."""
+        m = self._map_cloud(data, width, height, point_step, row_step, offsets, intensity_offset, label_offset, is_dense)
+        leaf = self._leaf(leaf)
+        if stamp is None:
+            self._stamp = getattr(self, "_stamp", 0) + 1
+            stamp = (1 << 40) + self._stamp
+        info = MapIntakeInfo()
+        self._check(self.L.mcl3dl_map_load(self.h, C.byref(m), leaf.ctypes.data_as(C.c_void_p), stamp,
+                                           C.byref(lik) if lik is not None else None,
+                                           C.byref(beam) if beam is not None else None, C.byref(info)))
+        return info.as_dict()
+
+    def map_update_set(self, data, width, height, point_step, row_step, offsets, leaf, intensity_offset=None,
+                       label_offset=None, is_dense=True):
+        """cbMapcloudUpdate on the device: the patch converted and downsampled at leaf, pending until
+        map_update_commit (it replaces a pending patch).  Arguments and the overrun check as map_load."""
+        m = self._map_cloud(data, width, height, point_step, row_step, offsets, intensity_offset, label_offset, is_dense)
+        leaf = self._leaf(leaf)
+        info = MapIntakeInfo()
+        self._check(self.L.mcl3dl_map_update_set(self.h, C.byref(m), leaf.ctypes.data_as(C.c_void_p), C.byref(info)))
+        return info.as_dict()
+
+    def map_update_commit(self, stamp=None):
+        """The map update timer: the pending patch appended to the staged map (map_append's info dict)."""
+        if stamp is None:
+            self._stamp = getattr(self, "_stamp", 0) + 1
+            stamp = (1 << 40) + self._stamp
+        info = MapAppendInfo()
+        self._check(self.L.mcl3dl_map_update_commit(self.h, stamp, C.byref(info)))
+        return info.as_dict()
+
+    def map_update_clear(self):
+        """cbPosition's pc_update_.reset(): drops the pending patch."""
+        self._check(self.L.mcl3dl_map_update_clear(self.h))
+
+    def map_get(self):
+        """The staged map: (POINT array, float32 intensities), in staged order."""
+        n = C.c_size_t(0)
+        self._check(self.L.mcl3dl_map_get(self.h, None, None, 0, C.byref(n)))
+        pts = np.zeros(n.value, dtype=POINT)
+        inten = np.zeros(n.value, dtype=np.float32)
+        if n.value:
+            self._check(self.L.mcl3dl_map_get(self.h, _ptr(pts), inten.ctypes.data_as(C.c_void_p), len(pts), C.byref(n)))
+        return pts, inten
 
     def scan_sample_with_normal(self, mean_rot, pos_cov, params=None, lik_num_points=96, beam_num_points=3, seed=1):
         """The node's PointCloudSamplerWithNormal on the clipped clouds of the last scan_prepare; the new samples replace

@@ -19,6 +19,7 @@
 #define MCL_3DL_B200_LIDAR_MEASUREMENT_MODEL_B200_H
 
 #include <algorithm>
+#include <cstddef>
 #include <cmath>
 #include <cstring>
 #include <memory>
@@ -323,6 +324,7 @@ public:
   // while the index has none.
   void setMapCloud(const Cloud::ConstPtr& map)
   {
+    intake_map_ = false;  // supersedes an intake map
     map_cloud_ = map;
     stageCloud(map);
     if (!staged_map_)
@@ -386,35 +388,8 @@ public:
   bool accumulateCloud(const sensor_msgs::PointCloud2& msg, const mcl3dl_transform& odom_from_sensor)
   {
     mcl3dl_cloud_view v{};
-    const char* names[3] = {"x", "y", "z"};
-    for (int k = 0; k < 3; ++k)
-    {
-      const sensor_msgs::PointField* f = nullptr;
-      for (const auto& fl : msg.fields)
-        if (fl.name == names[k])
-        {
-          f = &fl;
-          break;
-        }
-      if (!f || f->datatype != sensor_msgs::PointField::FLOAT32)
-        return false;
-      v.offset[k] = f->offset;
-    }
-    const uint64_t n = static_cast<uint64_t>(msg.width) * msg.height;
-    if (msg.is_bigendian || n == 0)
+    if (!cloudView(msg, v))
       return false;
-    const uint64_t span = static_cast<uint64_t>(msg.height - 1) * msg.row_step + static_cast<uint64_t>(msg.width) * msg.point_step;
-    if (static_cast<uint64_t>(msg.row_step) < static_cast<uint64_t>(msg.width) * msg.point_step || span > msg.data.size())
-      return false;
-    for (int k = 0; k < 3; ++k)
-      if (static_cast<uint64_t>(v.offset[k]) + 4 > msg.point_step)
-        return false;
-    v.data = msg.data.data();
-    v.width = msg.width;
-    v.height = msg.height;
-    v.point_step = msg.point_step;
-    v.row_step = msg.row_step;
-    v.is_dense = msg.is_dense ? 1 : 0;
     check(mcl3dl_scan_accumulate(engine_, &v, &odom_from_sensor, &accumulated_clouds_), "mcl3dl_scan_accumulate");
     return true;
   }
@@ -431,6 +406,95 @@ public:
   {
     check(mcl3dl_scan_prepare_accumulated(engine_, &base_from_odom, &params, info), "mcl3dl_scan_prepare_accumulated");
   }
+  // ---- The map intake on the device (mcl3dl_map_load / mcl3dl_map_update_*; INTEGRATION.md, "the map intake").
+  // Staging rules: after an intake load the entry points that take the index use the engine's map while the index and
+  // setMapCloud have none; a later setMapCloud, or an index that holds a cloud, supersedes it (staged whole).  The node
+  // then keeps no host copy of the map: mapCloud reads it back for updated_map.
+  // cbMapcloud -> loadMapCloud (src/mcl_3dl.cpp:127-140, 1150-1170): fromROSMsg and the VoxelGrid at map_downsample on
+  // the device, staged as the map; a pending patch is dropped.  False, with nothing changed, where accumulateCloud is
+  // false (fromROSMsg's failures and its documented departures), for an intensity / label field of the right type that
+  // does not fit in point_step, and for a map that keeps no finite point.  An intensity (label) field that is not
+  // FLOAT32 (UINT32) is not read: fromROSMsg leaves 0 there.  stamp: the map's header.stamp, as mapCloud reports it.
+  bool loadMapMessage(const sensor_msgs::PointCloud2& msg, const float leaf[3], uint64_t stamp)
+  {
+    mcl3dl_map_cloud m{};
+    return mapView(msg, m) && loadMap(m, leaf, stamp);
+  }
+  // cbLoadPCD (:1172-1192) after loadPCDFile: the PointXYZIL array itself as the view.  False for an empty cloud and as
+  // loadMapMessage.
+  bool loadMapCloud(const Cloud& cloud, const float leaf[3], uint64_t stamp)
+  {
+    if (cloud.points.empty())
+      return false;
+    mcl3dl_map_cloud m{};
+    m.view.data = cloud.points.data();
+    m.view.width = static_cast<uint32_t>(cloud.points.size());
+    m.view.height = 1;
+    m.view.point_step = sizeof(PointType);
+    m.view.row_step = m.view.width * m.view.point_step;
+    m.view.offset[0] = offsetof(PointType, x);
+    m.view.offset[1] = offsetof(PointType, y);
+    m.view.offset[2] = offsetof(PointType, z);
+    m.view.is_dense = cloud.is_dense ? 1 : 0;
+    m.intensity_offset = offsetof(PointType, intensity);
+    m.label_offset = offsetof(PointType, label);
+    return loadMap(m, leaf, stamp);
+  }
+  // cbMapcloudUpdate (:141-153): the patch's fromROSMsg and VoxelGrid at update_downsample into the engine's pending
+  // patch (it replaces one).  False, with nothing changed, as loadMapMessage (an empty patch after the VoxelGrid is valid).
+  bool setMapUpdate(const sensor_msgs::PointCloud2& msg, const float leaf[3])
+  {
+    mcl3dl_map_cloud m{};
+    if (!mapView(msg, m))
+      return false;
+    check(mcl3dl_map_update_set(engine_, &m, leaf, nullptr), "mcl3dl_map_update_set");
+    return true;
+  }
+  // cbMapUpdateTimer (:1350-1378): the pending patch appended to the intake map on the device (mcl3dl_map_update_commit);
+  // no pending patch changes nothing.  False, with the patch kept, when the engine's map is not an intake map (no load
+  // yet, or setMapCloud / the index superseded it).  stamp: the new header.stamp of the published map.
+  bool commitMapUpdate(uint64_t stamp)
+  {
+    if (!intake_map_)
+      return false;
+    mcl3dl_map_append_info info{};
+    check(mcl3dl_map_update_commit(engine_, ++stamp_counter_, &info), "mcl3dl_map_update_commit");
+    if (info.n_appended > 0)
+    {
+      ++map_intake_commits_;
+      map_stamp_ = stamp;
+    }
+    return true;
+  }
+  // cbPosition's pc_update_.reset() (:189)
+  void clearMapUpdate() { check(mcl3dl_map_update_clear(engine_), "mcl3dl_map_update_clear"); }
+  // The staged map with x / y / z / intensity / label (updated_map, :1371-1373); header.stamp: the load's or the last
+  // commit's.  Intensities of maps staged from host clouds are 0.
+  void mapCloud(Cloud& out)
+  {
+    size_t n = 0;
+    check(mcl3dl_map_get(engine_, nullptr, nullptr, 0, &n), "mcl3dl_map_get");
+    std::vector<mcl3dl_point> pts(n);
+    std::vector<float> inten(n);
+    check(mcl3dl_map_get(engine_, pts.data(), inten.data(), n, &n), "mcl3dl_map_get");
+    out.points.resize(n);
+    for (size_t i = 0; i < n; ++i)
+    {
+      PointType& p = out.points[i];
+      p.x = pts[i].x;
+      p.y = pts[i].y;
+      p.z = pts[i].z;
+      p.intensity = inten[i];
+      p.label = pts[i].label;
+    }
+    out.width = static_cast<uint32_t>(n);
+    out.height = 1;
+    out.is_dense = true;
+    out.header.stamp = intake_map_ ? map_stamp_ : staged_stamp_;
+  }
+  // Intake loads, and commits that appended points, since construction
+  size_t mapIntakeLoads() const { return map_intake_loads_; }
+  size_t mapIntakeCommits() const { return map_intake_commits_; }
   // clouds accumulated since the last clear (the node's pc_accum_header_.size())
   uint32_t accumulatedClouds() const { return accumulated_clouds_; }
   void checked(int rc, const char* what) const { check(rc, what); }
@@ -482,10 +546,89 @@ private:
     if (rc != MCL3DL_OK)
       throw std::runtime_error(std::string(what) + ": " + mcl3dl_strerror(rc) + " " + mcl3dl_last_error_detail(engine_));
   }
-  // The map of an entry point that takes the index: the index's cloud, or while it has none the last setMapCloud's.
+  // The map of an entry point that takes the index: the index's cloud, or while it has none the intake map, or else the
+  // last setMapCloud's.
   void stageMap(ChunkedKdtree<PointType>::Ptr& kdtree)
   {
+    if (!kdtree->getInputCloud() && intake_map_)
+    {
+      // no host cloud to restage from: a grid-shaping parameter change needs a new load
+      const mcl3dl_lik_params l0 = lik_c_;
+      const mcl3dl_beam_params b0 = beam_c_;
+      deriveParams();
+      if (std::memcmp(&l0, &lik_c_, sizeof(l0)) != 0 || std::memcmp(&b0, &beam_c_, sizeof(b0)) != 0)
+        check(mcl3dl_set_params(engine_, &lik_c_, &beam_c_), "mcl3dl_set_params (the intake map needs a new load)");
+      staged_map_ = &intake_marker_;
+      return;
+    }
+    intake_map_ = false;
     stageCloud(kdtree->getInputCloud() ? kdtree->getInputCloud() : map_cloud_);
+  }
+  // Field lookup and layout checks of a PointCloud2 (accumulateCloud, loadMapMessage, setMapUpdate): false where
+  // mcl_3dl::fromROSMsg fails (no x / y / z field, an empty cloud) and where x / y / z are not FLOAT32, the cloud is
+  // big-endian or its layout does not hold its points.
+  static bool cloudView(const sensor_msgs::PointCloud2& msg, mcl3dl_cloud_view& v)
+  {
+    const char* names[3] = {"x", "y", "z"};
+    for (int k = 0; k < 3; ++k)
+    {
+      const sensor_msgs::PointField* f = findField(msg, names[k]);
+      if (!f || f->datatype != sensor_msgs::PointField::FLOAT32)
+        return false;
+      v.offset[k] = f->offset;
+    }
+    const uint64_t n = static_cast<uint64_t>(msg.width) * msg.height;
+    if (msg.is_bigendian || n == 0)
+      return false;
+    const uint64_t span = static_cast<uint64_t>(msg.height - 1) * msg.row_step + static_cast<uint64_t>(msg.width) * msg.point_step;
+    if (static_cast<uint64_t>(msg.row_step) < static_cast<uint64_t>(msg.width) * msg.point_step || span > msg.data.size())
+      return false;
+    for (int k = 0; k < 3; ++k)
+      if (static_cast<uint64_t>(v.offset[k]) + 4 > msg.point_step)
+        return false;
+    v.data = msg.data.data();
+    v.width = msg.width;
+    v.height = msg.height;
+    v.point_step = msg.point_step;
+    v.row_step = msg.row_step;
+    v.is_dense = msg.is_dense ? 1 : 0;
+    return true;
+  }
+  static const sensor_msgs::PointField* findField(const sensor_msgs::PointCloud2& msg, const char* name)
+  {
+    for (const auto& fl : msg.fields)
+      if (fl.name == name)
+        return &fl;
+    return nullptr;
+  }
+  // cloudView, plus the intensity (FLOAT32) and label (UINT32) offsets where a field of that name and type exists
+  static bool mapView(const sensor_msgs::PointCloud2& msg, mcl3dl_map_cloud& m)
+  {
+    if (!cloudView(msg, m.view))
+      return false;
+    const auto offset = [&](const char* name, uint8_t type, int32_t& out) {
+      const sensor_msgs::PointField* f = findField(msg, name);
+      out = (f && f->datatype == type) ? static_cast<int32_t>(f->offset) : -1;
+      return out < 0 || static_cast<uint64_t>(f->offset) + 4 <= msg.point_step;
+    };
+    return offset("intensity", sensor_msgs::PointField::FLOAT32, m.intensity_offset) &&
+           offset("label", sensor_msgs::PointField::UINT32, m.label_offset);
+  }
+  bool loadMap(const mcl3dl_map_cloud& m, const float leaf[3], uint64_t stamp)
+  {
+    deriveParams();
+    const int rc = mcl3dl_map_load(engine_, &m, leaf, ++stamp_counter_, &lik_c_, &beam_c_, nullptr);
+    if (rc == MCL3DL_ERR_INVALID_ARG && m.view.data)
+      return false;  // no finite point (the view itself was checked above): the previous map stays
+    check(rc, "mcl3dl_map_load");
+    staged_map_ = &intake_marker_;
+    staged_pts_.clear();
+    staged_size_ = 0;
+    map_cloud_.reset();
+    intake_map_ = true;
+    map_stamp_ = stamp;
+    ++map_intake_loads_;
+    return true;
   }
   void stageCloud(const Cloud::ConstPtr& map)
   {
@@ -622,6 +765,10 @@ private:
   Cloud::ConstPtr map_cloud_;              // the last setMapCloud's cloud
   uint64_t stamp_counter_ = 0;
   size_t map_appends_ = 0, map_restages_ = 0;
+  bool intake_map_ = false;     // the engine's map came from loadMapMessage / loadMapCloud (and commitMapUpdate)
+  const Cloud intake_marker_{};  // staged_map_ while the intake map is staged: no host cloud is that object
+  uint64_t map_stamp_ = 0;      // the intake map's header.stamp
+  size_t map_intake_loads_ = 0, map_intake_commits_ = 0;
   uint32_t accumulated_clouds_ = 0;
   Cloud::ConstPtr lik_cloud_, beam_cloud_;
   std::vector<mcl3dl_point> lik_pts_, beam_pts_;
