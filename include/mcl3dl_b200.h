@@ -805,7 +805,8 @@ int mcl3dl_collect_timing(mcl3dl_engine*, int enable);
 int mcl3dl_last_timing(const mcl3dl_engine*, double* h2d_ms, double* lik_kernel_ms, double* beam_kernel_ms,
                        double* d2h_ms);
 
-/* Number of this library's kernels launched since create (the bench's gpu_launches counter). */
+/* Device work this engine enqueued since create (the bench's gpu_launches counter): one per successful kernel launch and
+   one per device-wide CUB call (sort, scan, reduce), however many kernels CUB runs inside it. */
 uint64_t mcl3dl_kernel_launches(const mcl3dl_engine*);
 
 const char* mcl3dl_strerror(int code);

@@ -683,10 +683,28 @@ int opt_in_smem(mcl3dl_engine* eng, DeviceCtx& c, K kernel, int bytes)
   return MCL3DL_OK;
 }
 
+// ---- every kernel launch and every device-wide CUB call goes through launch / launch_pdl / cub_call: each returns its
+// own error (CK at the call site names it) and counts one in mcl3dl_kernel_launches when it succeeded.  None of them
+// allocates or synchronises, except that cub_call grows its scratch.
+cudaError_t counted(mcl3dl_engine* eng, cudaError_t e)
+{
+  if (e == cudaSuccess)
+    eng->launches++;
+  return e;
+}
+
+template <typename... KArgs, typename... Args>
+cudaError_t launch(mcl3dl_engine* eng, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
+                   Args... args)
+{
+  kernel<<<grid, block, smem, st>>>(static_cast<KArgs>(args)...);
+  return counted(eng, cudaGetLastError());
+}
+
 // Launch with programmatic stream serialization (kernels.cuh: pdl_start): the kernel's launch and CTA dispatch overlap
 // the drain of the grid before it in the stream; the kernel itself waits for that grid before its first global read.
 template <typename... KArgs, typename... Args>
-cudaError_t launch_pdl(void (*kernel)(KArgs...), int grid, size_t smem, cudaStream_t st, Args... args)
+cudaError_t launch_pdl(mcl3dl_engine* eng, void (*kernel)(KArgs...), int grid, size_t smem, cudaStream_t st, Args... args)
 {
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
@@ -698,7 +716,35 @@ cudaError_t launch_pdl(void (*kernel)(KArgs...), int grid, size_t smem, cudaStre
   cfg.stream = st;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+  return counted(eng, cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...));
+}
+
+// A device-wide CUB call is a lambda f(void* temp, size_t& bytes) around one cub::Device* call.  cub_reserve grows `tmp`
+// to the largest size query of the calls fs.  A function that runs several calls on one scratch sizes it for all of them
+// before the first one, so that it never grows (and is freed, which waits for the device) between two of them.
+template <typename... F>
+cudaError_t cub_reserve(DevBuf& tmp, const F&... fs)
+{
+  cudaError_t e = cudaSuccess;
+  size_t need = 0;
+  const auto query = [&](const auto& f) {
+    size_t bytes = 0;
+    if (e == cudaSuccess)
+      e = f(nullptr, bytes);
+    need = std::max(need, bytes);
+  };
+  (query(fs), ...);
+  return e != cudaSuccess ? e : tmp.reserve(need);
+}
+
+// One CUB call on scratch `tmp`, counted as one launch however many kernels CUB runs inside it
+template <typename F>
+cudaError_t cub_call(mcl3dl_engine* eng, DevBuf& tmp, const F& f)
+{
+  if (const cudaError_t e = cub_reserve(tmp, f))
+    return e;
+  size_t bytes = tmp.cap;
+  return counted(eng, f(tmp.p, bytes));
 }
 
 // CSR-window likelihood kernel (no NN field staged)
@@ -714,9 +760,8 @@ int launch_lik_wi_t(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_pose* poses, 
   const auto kernel = staged ? lik_kernel_wi<TPP, true> : lik_kernel_wi<TPP, false>;
   if (staged)
     if (int rc = opt_in_smem(eng, c, kernel, kMaxStagedSorted)) return rc;
-  kernel<<<grid, kBlockThreads, staged ? bytes : 0, st>>>(poses, P, scan, N, c.nn, eng->likdev, out, beam_defaults, c.stats_ptr(), sink);
-  CK(cudaGetLastError());
-  eng->launches++;
+  CK(launch(eng, kernel, grid, kBlockThreads, staged ? bytes : 0, st, poses, P, scan, N, c.nn, eng->likdev, out, beam_defaults,
+            c.stats_ptr(), sink));
   return MCL3DL_OK;
 }
 
@@ -756,9 +801,8 @@ int launch_lik_nf_t(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_pose* poses, 
                              : (ovf ? lik_kernel_nf<TPP, false, true> : lik_kernel_nf<TPP, false, false>);
   if (staged)
     if (int rc = opt_in_smem(eng, c, kernel, kMaxStagedBytes / 2)) return rc;
-  CK(launch_pdl(kernel, grid, staged ? bytes : 0, st, poses, P, scan, N, c.nn, eng->likdev, out, beam_defaults,
+  CK(launch_pdl(eng, kernel, grid, staged ? bytes : 0, st, poses, P, scan, N, c.nn, eng->likdev, out, beam_defaults,
                 c.stats_ptr(), sink));
-  eng->launches++;
   return MCL3DL_OK;
 }
 
@@ -772,9 +816,8 @@ int launch_lik_nf_pm(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_pose* poses,
     return rc;
   auto* acc = static_cast<unsigned long long*>(c.d_lacc.p);
   const auto kernel = eng->nnf_overflow_cells != 0 ? lik_kernel_nf_pm<true> : lik_kernel_nf_pm<false>;
-  CK(launch_pdl(kernel, blocks * sh.n_slices, 0, st, poses, P, scan, N, c.nn, eng->likdev, out, beam_defaults,
+  CK(launch_pdl(eng, kernel, blocks * sh.n_slices, 0, st, poses, P, scan, N, c.nn, eng->likdev, out, beam_defaults,
                 c.stats_ptr(), sink, sh, acc));
-  eng->launches++;
   return MCL3DL_OK;
 }
 
@@ -845,14 +888,11 @@ int stage_field(mcl3dl_engine* eng, DeviceCtx& c, const float* host_nodes)
     g.near.bits = nullptr;
 #endif
     const size_t total = static_cast<size_t>(nnx) * nny * nnz;
-    field_nodes_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(g, lp, c.fld_nodes, nnx, nny, nnz, clamp);
-    CK(cudaGetLastError());
-    eng->launches++;
+    CK(launch(eng, field_nodes_kernel, static_cast<unsigned>((total + 255) / 256), 256, 0, st, g, lp, c.fld_nodes, nnx, nny, nnz,
+              clamp));
   }
-  field_expand_kernel<<<static_cast<unsigned>((n_cells + 255) / 256), 256, 0, st>>>(c.fld_nodes, f.nx, f.ny, f.nz,
-                                                                                    static_cast<float4*>(c.fld_cells.p));
-  CK(cudaGetLastError());
-  eng->launches++;
+  CK(launch(eng, field_expand_kernel, static_cast<unsigned>((n_cells + 255) / 256), 256, 0, st, c.fld_nodes, f.nx, f.ny, f.nz,
+            static_cast<float4*>(c.fld_cells.p)));
   CK(cudaStreamSynchronize(st));
   FieldDev d{};
   d.cells = static_cast<const float4*>(c.fld_cells.p);
@@ -878,15 +918,11 @@ int launch_lik_field_t(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_pose* pose
   const int grid = std::max(1, std::min(groups, c.sm_count * kNfCtasPerSm));
   const size_t bytes = static_cast<size_t>(N) * 16;
   const bool staged = bytes <= static_cast<size_t>(kMaxStagedBytes) / 2 && (PPB >= 4 || groups > grid);
+  const auto kernel = staged ? lik_kernel_field<TPP, true> : lik_kernel_field<TPP, false>;
   if (staged)
-  {
-    if (int rc = opt_in_smem(eng, c, lik_kernel_field<TPP, true>, kMaxStagedBytes / 2)) return rc;
-    lik_kernel_field<TPP, true><<<grid, kBlockThreads, bytes, st>>>(poses, P, scan, N, c.nn, eng->likdev, out, beam_defaults, c.stats_ptr(), sink);
-  }
-  else
-    lik_kernel_field<TPP, false><<<grid, kBlockThreads, 0, st>>>(poses, P, scan, N, c.nn, eng->likdev, out, beam_defaults, c.stats_ptr(), sink);
-  CK(cudaGetLastError());
-  eng->launches++;
+    if (int rc = opt_in_smem(eng, c, kernel, kMaxStagedBytes / 2)) return rc;
+  CK(launch(eng, kernel, grid, kBlockThreads, staged ? bytes : 0, st, poses, P, scan, N, c.nn, eng->likdev, out, beam_defaults,
+            c.stats_ptr(), sink));
   return MCL3DL_OK;
 }
 
@@ -946,11 +982,9 @@ int launch_beam_pl(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_pose* poses, s
   const int groups = static_cast<int>(((P + 31) / 32 + gpc - 1) / gpc);
   const size_t smem = static_cast<size_t>(kPlWarps) * sh.ppl * 16;
   const auto kernel = eng->beam.use_raycast_using_dda ? beam_kernel_pl<false> : beam_kernel_pl<true>;
-  kernel<<<groups * sh.cb, kBlockThreads, smem, st>>>(
-      poses, static_cast<int>(P), reinterpret_cast<const float4*>(scan), static_cast<int>(N), origins, c.dda, c.kd, c.nn, out, status,
-      lik_defaults, c.stats_ptr(), sh, static_cast<uint32_t*>(c.d_partial.p), static_cast<unsigned int*>(c.d_tickets.p), sink);
-  CK(cudaGetLastError());
-  eng->launches++;
+  CK(launch(eng, kernel, groups * sh.cb, kBlockThreads, smem, st, poses, static_cast<int>(P), reinterpret_cast<const float4*>(scan),
+            static_cast<int>(N), origins, c.dda, c.kd, c.nn, out, status, lik_defaults, c.stats_ptr(), sh,
+            static_cast<uint32_t*>(c.d_partial.p), static_cast<unsigned int*>(c.d_tickets.p), sink));
   return MCL3DL_OK;
 }
 
@@ -970,12 +1004,10 @@ int launch_beam_dq(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_pose* poses, s
       (rc = reserve_zeroed(eng, c.d_queue, 256, st)))
     return rc;
   const auto kernel = eng->beam.use_raycast_using_dda ? beam_kernel_dq<false> : beam_kernel_dq<true>;
-  kernel<<<grid, kBlockThreads, 0, st>>>(poses, static_cast<int>(P), reinterpret_cast<const float4*>(scan), static_cast<int>(N),
-                                         origins, c.dda, c.kd, c.nn, out, status, lik_defaults, c.stats_ptr(),
-                                         static_cast<int>(ppl), n_chunks, static_cast<uint32_t*>(c.d_tally.p),
-                                         static_cast<unsigned int*>(c.d_tickets.p), static_cast<unsigned int*>(c.d_queue.p), sink);
-  CK(cudaGetLastError());
-  eng->launches++;
+  CK(launch(eng, kernel, grid, kBlockThreads, 0, st, poses, static_cast<int>(P), reinterpret_cast<const float4*>(scan),
+            static_cast<int>(N), origins, c.dda, c.kd, c.nn, out, status, lik_defaults, c.stats_ptr(), static_cast<int>(ppl),
+            n_chunks, static_cast<uint32_t*>(c.d_tally.p), static_cast<unsigned int*>(c.d_tickets.p),
+            static_cast<unsigned int*>(c.d_queue.p), sink));
   return MCL3DL_OK;
 }
 
@@ -1066,9 +1098,8 @@ int build_near_field(mcl3dl_engine* eng, DeviceCtx& c, cudaStream_t st, const mc
     return rc;
   if (first == 0)
     CK(cudaMemsetAsync(buf.p, 0, bytes, st));
-  near_mark_kernel<<<(n - first + 255) / 256, 256, 0, st>>>(pts + first, n - first, wx, wy, wz, f, static_cast<uint32_t*>(buf.p), k);
-  CK(cudaGetLastError());
-  eng->launches++;
+  CK(launch(eng, near_mark_kernel, (n - first + 255) / 256, 256, 0, st, pts + first, n - first, wx, wy, wz, f,
+            static_cast<uint32_t*>(buf.p), k));
   f.bits = static_cast<const uint32_t*>(buf.p);
   out = f;
   c.map_bytes += bytes;
@@ -1116,26 +1147,22 @@ int build_nn_field(mcl3dl_engine* eng, DeviceCtx& c, cudaStream_t st, const mcl3
       (rc = reserve(eng, c.nnf_dir, n_cells * sizeof(uint2))) || (rc = reserve(eng, c.nnf_wide, static_cast<size_t>(wide_cap) * sizeof(uint4))))
     return rc;
   CK(cudaMemsetAsync(d_bits.p, 0, bits_bytes, st));
-  near_mark_kernel<<<(n + 255) / 256, 256, 0, st>>>(pts, n, g.wx, g.wy, g.wz, lay, static_cast<uint32_t*>(d_bits.p), 2);
+  CK(launch(eng, near_mark_kernel, (n + 255) / 256, 256, 0, st, pts, n, g.wx, g.wy, g.wz, lay, static_cast<uint32_t*>(d_bits.p), 2));
   const unsigned blocks = static_cast<unsigned>((n_cells * 8 + 255) / 256);
   uint2* dir = static_cast<uint2*>(c.nnf_dir.p);
   uint32_t* tot = static_cast<uint32_t*>(d_tot.p);
   CK(cudaMemsetAsync(tot + n_cells, 0, 16, st));  // [n_cells]: scan tail, [n_cells + 2] wide cells, [n_cells + 3] overflow cells
   f.wide = static_cast<const uint4*>(c.nnf_wide.p);
-  nnf_count_kernel<<<blocks, 256, 0, st>>>(g, f, static_cast<const uint32_t*>(d_bits.p), lay.pitch, dir, tot, nullptr, n_cells,
-                                           static_cast<uint4*>(c.nnf_wide.p), wide_cap, tot + n_cells + 2);
-  CK(cudaGetLastError());
+  CK(launch(eng, nnf_count_kernel, blocks, 256, 0, st, g, f, static_cast<const uint32_t*>(d_bits.p), lay.pitch, dir, tot, nullptr,
+            n_cells, static_cast<uint4*>(c.nnf_wide.p), wide_cap, tot + n_cells + 2));
   // exclusive scan of the per-cell totals (in place); the grand total sizes the candidate array.  A candidate index
   // must stay below 2^31 (bit 31 of a directory entry marks wide / overflow cells): the total is first summed in 64 bits.
   cub::TransformInputIterator<unsigned long long, WidenU32, const uint32_t*> wide_in(tot, WidenU32());
   unsigned long long* d_sum = reinterpret_cast<unsigned long long*>(tot + sum_at);
-  size_t tmp_bytes = 0, tmp_sum = 0;
-  CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, tot, tot, static_cast<int>(n_cells + 1), st));
-  CK(cub::DeviceReduce::Sum(nullptr, tmp_sum, wide_in, d_sum, static_cast<int>(n_cells), st));
-  if ((rc = reserve(eng, d_tmp, std::max(tmp_bytes, tmp_sum))))
-    return rc;
-  tmp_sum = d_tmp.cap;
-  CK(cub::DeviceReduce::Sum(d_tmp.p, tmp_sum, wide_in, d_sum, static_cast<int>(n_cells), st));
+  const auto scan = [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, tot, tot, static_cast<int>(n_cells + 1), st); };
+  const auto sum = [&](void* t, size_t& b) { return cub::DeviceReduce::Sum(t, b, wide_in, d_sum, static_cast<int>(n_cells), st); };
+  CK(cub_reserve(d_tmp, scan, sum));
+  CK(cub_call(eng, d_tmp, sum));
   unsigned long long sum64 = 0;
   CK(cudaMemcpyAsync(&sum64, d_sum, 8, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
@@ -1145,8 +1172,7 @@ int build_nn_field(mcl3dl_engine* eng, DeviceCtx& c, cudaStream_t st, const mcl3
     c.nnf_wide = DevBuf();
     return MCL3DL_OK;
   }
-  tmp_bytes = d_tmp.cap;
-  CK(cub::DeviceScan::ExclusiveSum(d_tmp.p, tmp_bytes, tot, tot, static_cast<int>(n_cells + 1), st));
+  CK(cub_call(eng, d_tmp, scan));
   uint32_t tail[4] = {0, 0, 0, 0};
   CK(cudaMemcpyAsync(tail, tot + n_cells, sizeof(tail), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
@@ -1162,13 +1188,11 @@ int build_nn_field(mcl3dl_engine* eng, DeviceCtx& c, cudaStream_t st, const mcl3
   }
   if ((rc = reserve(eng, c.nnf_cand, std::max<size_t>(cand_bytes, 16))))
     return rc;
-  nnf_base_kernel<<<static_cast<unsigned>((n_cells + 255) / 256), 256, 0, st>>>(dir, tot, 0u, nullptr, n_cells,
-                                                                                 static_cast<uint4*>(c.nnf_wide.p));
-  nnf_fill_kernel<<<blocks, 256, 0, st>>>(g, f, static_cast<const uint32_t*>(d_bits.p), lay.pitch, dir,
-                                          static_cast<float4*>(c.nnf_cand.p), nullptr, n_cells);
-  CK(cudaGetLastError());
+  CK(launch(eng, nnf_base_kernel, static_cast<unsigned>((n_cells + 255) / 256), 256, 0, st, dir, tot, 0u, nullptr, n_cells,
+            static_cast<uint4*>(c.nnf_wide.p)));
+  CK(launch(eng, nnf_fill_kernel, blocks, 256, 0, st, g, f, static_cast<const uint32_t*>(d_bits.p), lay.pitch, dir,
+            static_cast<float4*>(c.nnf_cand.p), nullptr, n_cells));
   CK(cudaStreamSynchronize(st));
-  eng->launches += 4;
   f.dir = dir;
   f.cand = static_cast<const float4*>(c.nnf_cand.p);
   g.field = f;
@@ -1214,17 +1238,15 @@ int update_nn_field(mcl3dl_engine* eng, DeviceCtx& c, cudaStream_t st, const mcl
   uint32_t* tot = static_cast<uint32_t*>(d_tot.p);
   // the field's k = 2 near field of the whole map, as the build makes it
   CK(cudaMemsetAsync(d_bits.p, 0, bits_bytes, st));
-  near_mark_kernel<<<(n + 255) / 256, 256, 0, st>>>(pts, n, g.wx, g.wy, g.wz, lay, static_cast<uint32_t*>(d_bits.p), 2);
+  CK(launch(eng, near_mark_kernel, (n + 255) / 256, 256, 0, st, pts, n, g.wx, g.wy, g.wz, lay, static_cast<uint32_t*>(d_bits.p), 2));
   CK(cudaMemsetAsync(d_mark.p, 0, mark_words * 4, st));
   const uint32_t init[8] = {c.nnf_wide_used, 0, 0, 0, 0, 0, 0, 0};
   CK(cudaMemcpyAsync(cnt, init, sizeof(init), cudaMemcpyHostToDevice, st));
-  nnf_mark_kernel<<<(n_new + 255) / 256, 256, 0, st>>>(pts + n_before, n_new, g, f, static_cast<uint32_t*>(d_mark.p), list,
-                                                        static_cast<uint32_t>(list_cap), cnt + 5);
-  CK(cudaGetLastError());
+  CK(launch(eng, nnf_mark_kernel, (n_new + 255) / 256, 256, 0, st, pts + n_before, n_new, g, f, static_cast<uint32_t*>(d_mark.p),
+            list, static_cast<uint32_t>(list_cap), cnt + 5));
   uint32_t n_list = 0;
   CK(cudaMemcpyAsync(&n_list, cnt + 5, 4, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
-  eng->launches += 2;
   if (n_list > list_cap)
     return MCL3DL_OK;
   reselected = n_list;
@@ -1238,22 +1260,18 @@ int update_nn_field(mcl3dl_engine* eng, DeviceCtx& c, cudaStream_t st, const mcl
   uint2* dir = const_cast<uint2*>(f.dir);
   CK(cudaMemsetAsync(tot + n_list, 0, 4, st));
   const unsigned blocks = static_cast<unsigned>((static_cast<size_t>(n_list) * 8 + 255) / 256);
-  nnf_count_kernel<<<blocks, 256, 0, st>>>(g, f, static_cast<const uint32_t*>(d_bits.p), lay.pitch, dir, tot, list, n_list,
-                                           static_cast<uint4*>(c.nnf_wide.p), c.nnf_wide_cap, cnt);
-  CK(cudaGetLastError());
+  CK(launch(eng, nnf_count_kernel, blocks, 256, 0, st, g, f, static_cast<const uint32_t*>(d_bits.p), lay.pitch, dir, tot, list,
+            n_list, static_cast<uint4*>(c.nnf_wide.p), c.nnf_wide_cap, cnt));
   // at most 8 x 41 candidates per listed cell, fewer than 2^31 listed: the sum is taken in 64 bits
   cub::TransformInputIterator<unsigned long long, WidenU32, const uint32_t*> wide_in(tot, WidenU32());
   DevBuf d_sum;
   if ((rc = reserve(eng, d_sum, 8)))
     return rc;
   unsigned long long* sum = static_cast<unsigned long long*>(d_sum.p);
-  size_t tmp_scan = 0, tmp_sum = 0;
-  CK(cub::DeviceScan::ExclusiveSum(nullptr, tmp_scan, tot, tot, static_cast<int>(n_list + 1), st));
-  CK(cub::DeviceReduce::Sum(nullptr, tmp_sum, wide_in, sum, static_cast<int>(n_list), st));
-  if ((rc = reserve(eng, d_tmp, std::max(tmp_scan, tmp_sum))))
-    return rc;
-  tmp_sum = d_tmp.cap;
-  CK(cub::DeviceReduce::Sum(d_tmp.p, tmp_sum, wide_in, sum, static_cast<int>(n_list), st));
+  const auto scan = [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, tot, tot, static_cast<int>(n_list + 1), st); };
+  const auto reduce = [&](void* t, size_t& b) { return cub::DeviceReduce::Sum(t, b, wide_in, sum, static_cast<int>(n_list), st); };
+  CK(cub_reserve(d_tmp, scan, reduce));
+  CK(cub_call(eng, d_tmp, reduce));
   uint32_t h_cnt[5];
   unsigned long long added = 0;
   CK(cudaMemcpyAsync(h_cnt, cnt, sizeof(h_cnt), cudaMemcpyDeviceToHost, st));
@@ -1277,16 +1295,13 @@ int update_nn_field(mcl3dl_engine* eng, DeviceCtx& c, cudaStream_t st, const mcl
     c.nnf_cand = std::move(grown);
     eng->nnf_bytes = n_cells * 8 + cap * sizeof(float4) + wide_bytes;
   }
-  size_t tsz = d_tmp.cap;
-  CK(cub::DeviceScan::ExclusiveSum(d_tmp.p, tsz, tot, tot, static_cast<int>(n_list + 1), st));
+  CK(cub_call(eng, d_tmp, scan));
   f.cand = static_cast<const float4*>(c.nnf_cand.p);
-  nnf_base_kernel<<<(n_list + 255) / 256, 256, 0, st>>>(dir, tot, static_cast<uint32_t>(c.nnf_cand_used), list, n_list,
-                                                        static_cast<uint4*>(c.nnf_wide.p));
-  nnf_fill_kernel<<<blocks, 256, 0, st>>>(g, f, static_cast<const uint32_t*>(d_bits.p), lay.pitch, dir,
-                                          static_cast<float4*>(c.nnf_cand.p), list, n_list);
-  CK(cudaGetLastError());
+  CK(launch(eng, nnf_base_kernel, (n_list + 255) / 256, 256, 0, st, dir, tot, static_cast<uint32_t>(c.nnf_cand_used), list, n_list,
+            static_cast<uint4*>(c.nnf_wide.p)));
+  CK(launch(eng, nnf_fill_kernel, blocks, 256, 0, st, g, f, static_cast<const uint32_t*>(d_bits.p), lay.pitch, dir,
+            static_cast<float4*>(c.nnf_cand.p), list, n_list));
   CK(cudaStreamSynchronize(st));
-  eng->launches += 4;
   eng->nnf_cands = live;
   eng->nnf_overflow_cells = eng->nnf_overflow_cells - h_cnt[3] + h_cnt[1];
   eng->nnf_wide_cells = eng->nnf_wide_cells - h_cnt[4] + (h_cnt[0] - c.nnf_wide_used);
@@ -1314,15 +1329,15 @@ int sort_csr(mcl3dl_engine* eng, cudaStream_t st, uint32_t n, size_t cells, uint
 {
   int end_bit = 1;
   while ((size_t(1) << end_bit) < cells && end_bit < 32) ++end_bit;
-  size_t tmp_sort = 0, tmp_scan = 0;
-  CK(cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, keys[0], keys[1], vals[0], vals[1], n, 0, end_bit, st));
-  CK(cub::DeviceScan::InclusiveSum(nullptr, tmp_scan, cell_start, cell_start, static_cast<int>(cells + 1), st));
-  if (int r = reserve(eng, tmp, std::max(tmp_sort, tmp_scan)))
-    return r;
-  size_t tsz = tmp.cap;
-  CK(cub::DeviceRadixSort::SortPairs(tmp.p, tsz, keys[0], keys[1], vals[0], vals[1], n, 0, end_bit, st));
-  tsz = tmp.cap;
-  CK(cub::DeviceScan::InclusiveSum(tmp.p, tsz, cell_start, cell_start, static_cast<int>(cells + 1), st));
+  const auto sort = [&](void* t, size_t& b) {
+    return cub::DeviceRadixSort::SortPairs(t, b, keys[0], keys[1], vals[0], vals[1], n, 0, end_bit, st);
+  };
+  const auto scan = [&](void* t, size_t& b) {
+    return cub::DeviceScan::InclusiveSum(t, b, cell_start, cell_start, static_cast<int>(cells + 1), st);
+  };
+  CK(cub_reserve(tmp, sort, scan));
+  CK(cub_call(eng, tmp, sort));
+  CK(cub_call(eng, tmp, scan));
   return MCL3DL_OK;
 }
 
@@ -1360,14 +1375,10 @@ int build_nn_csr(mcl3dl_engine* eng, cudaStream_t st, const mcl3dl_point* pts, u
 {
   const int nb = static_cast<int>((static_cast<size_t>(n) + 255) / 256);
   CK(cudaMemsetAsync(cell_start, 0, (cells + 1) * 4, st));
-  nn_key_kernel<<<nb, 256, 0, st>>>(pts, n, g, keys[0], vals[0], cell_start);
-  CK(cudaGetLastError());
-  eng->launches++;
+  CK(launch(eng, nn_key_kernel, nb, 256, 0, st, pts, n, g, keys[0], vals[0], cell_start));
   if (int rc = sort_csr(eng, st, n, cells, cell_start, keys, vals, tmp))
     return rc;
-  nn_gather_kernel<<<nb, 256, 0, st>>>(pts, n, vals[1], g.wx, g.wy, g.wz, out);
-  CK(cudaGetLastError());
-  eng->launches += 3;
+  CK(launch(eng, nn_gather_kernel, nb, 256, 0, st, pts, n, vals[1], g.wx, g.wy, g.wz, out));
   return MCL3DL_OK;
 }
 
@@ -1403,9 +1414,7 @@ int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, DevBuf& d_pts, size_t 
   const float wx = eng->has_lik ? eng->lik.dist_weight[0] : 1.0f;
   const float wy = eng->has_lik ? eng->lik.dist_weight[1] : 1.0f;
   const float wz = eng->has_lik ? eng->lik.dist_weight[2] : 1.0f;
-  bbox_kernel<<<std::min(nb, c.sm_count * 8), tb, 0, st>>>(pts, n, wx, wy, wz, static_cast<uint32_t*>(d_bbox.p));
-  CK(cudaGetLastError());
-  eng->launches++;
+  CK(launch(eng, bbox_kernel, std::min(nb, c.sm_count * 8), tb, 0, st, pts, n, wx, wy, wz, static_cast<uint32_t*>(d_bbox.p)));
   CK(cudaMemcpyAsync(h_bbox, d_bbox.p, sizeof(h_bbox), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   float raw_min[3], raw_max[3], sc_min[3], sc_max[3];
@@ -1486,9 +1495,8 @@ int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, DevBuf& d_pts, size_t 
       if ((rc = reserve(eng, c.nn_row3, (row3_total + 2) * sizeof(uint2))))
         return rc;
       g.row3 = static_cast<const uint2*>(c.nn_row3.p);
-      nn_row3_kernel<<<static_cast<unsigned>((row3_total + 255) / 256), 256, 0, st>>>(g, static_cast<uint2*>(c.nn_row3.p), row3_total);
-      CK(cudaGetLastError());
-      eng->launches++;
+      CK(launch(eng, nn_row3_kernel, static_cast<unsigned>((row3_total + 255) / 256), 256, 0, st, g, static_cast<uint2*>(c.nn_row3.p),
+                row3_total));
     }
     else
     {
@@ -1563,13 +1571,10 @@ int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, DevBuf& d_pts, size_t 
     uint32_t* cell_start = static_cast<uint32_t*>(c.dda_cell_start.p);
     CK(cudaMemsetAsync(cell_start, 0, (cells + 2) * 4, st));
     CK(cudaMemsetAsync(c.dda_occ.p, 0, occ_words * 4, st));
-    dda_key_kernel<<<nb, tb, 0, st>>>(pts, n32, g, keys[0], vals[0], cell_start, static_cast<uint32_t*>(c.dda_occ.p));
-    CK(cudaGetLastError());
+    CK(launch(eng, dda_key_kernel, nb, tb, 0, st, pts, n32, g, keys[0], vals[0], cell_start, static_cast<uint32_t*>(c.dda_occ.p)));
     if ((rc = sort_csr(eng, st, n32, cells, cell_start, keys, vals, d_tmp)))
       return rc;
-    dda_gather_kernel<<<nb, tb, 0, st>>>(pts, n32, vals[1], static_cast<float4*>(c.dda_pts.p));
-    CK(cudaGetLastError());
-    eng->launches += 4;
+    CK(launch(eng, dda_gather_kernel, nb, tb, 0, st, pts, n32, vals[1], static_cast<float4*>(c.dda_pts.p)));
     g.occ = static_cast<const uint32_t*>(c.dda_occ.p);
     g.cell_start = cell_start;
     g.pts = static_cast<const float4*>(c.dda_pts.p);
@@ -1639,9 +1644,7 @@ int voxel_grid(mcl3dl_engine* eng, DeviceCtx& c, cudaStream_t st, const mcl3dl_p
     return rc;
   uint32_t* bb = static_cast<uint32_t*>(b.tmp->p);
   CK(cudaMemcpyAsync(bb, h_bbox, sizeof(h_bbox), cudaMemcpyHostToDevice, st));
-  scan_bbox_kernel<<<std::min(nb, c.sm_count * 8), 256, 0, st>>>(in, n, bb);
-  CK(cudaGetLastError());
-  eng->launches++;
+  CK(launch(eng, scan_bbox_kernel, std::min(nb, c.sm_count * 8), 256, 0, st, in, n, bb));
   CK(cudaMemcpyAsync(h_bbox, bb, sizeof(h_bbox), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   const float mn[3] = {ord2f(h_bbox[0]), ord2f(h_bbox[1]), ord2f(h_bbox[2])};
@@ -1661,23 +1664,18 @@ int voxel_grid(mcl3dl_engine* eng, DeviceCtx& c, cudaStream_t st, const mcl3dl_p
   uint32_t *v0 = static_cast<uint32_t*>(b.vals[0]->p), *v1 = static_cast<uint32_t*>(b.vals[1]->p);
   uint64_t *kl0 = static_cast<uint64_t*>(b.key_label[0]->p), *kl1 = static_cast<uint64_t*>(b.key_label[1]->p);
   uint32_t *fl = static_cast<uint32_t*>(b.flags->p), *ps = static_cast<uint32_t*>(b.pos->p);
-  scan_key_kernel<<<nb, 256, 0, st>>>(in, n, g, k0, v0, kl0);
-  size_t t_sort = 0, t_sort_kl = 0, t_scan = 0;
-  CK(cub::DeviceRadixSort::SortPairs(nullptr, t_sort, k0, k1, v0, v1, n, 0, end_bit, st));
-  CK(cub::DeviceRadixSort::SortKeys(nullptr, t_sort_kl, kl0, kl1, n, 0, 32 + end_bit, st));
-  CK(cub::DeviceScan::ExclusiveSum(nullptr, t_scan, fl, ps, n, st));
-  if ((rc = reserve(eng, *b.tmp, std::max(std::max(t_sort, t_sort_kl), t_scan) + 256)))
-    return rc;
-  size_t tsz = b.tmp->cap;
-  CK(cub::DeviceRadixSort::SortPairs(b.tmp->p, tsz, k0, k1, v0, v1, n, 0, end_bit, st));  // stable: input order inside a voxel
-  tsz = b.tmp->cap;
-  CK(cub::DeviceRadixSort::SortKeys(b.tmp->p, tsz, kl0, kl1, n, 0, 32 + end_bit, st));  // labels ascending inside a voxel
-  scan_heads_kernel<<<nb, 256, 0, st>>>(k1, n, fl);
-  tsz = b.tmp->cap;
-  CK(cub::DeviceScan::ExclusiveSum(b.tmp->p, tsz, fl, ps, n, st));
-  scan_centroid_kernel<<<nb, 256, 0, st>>>(in, k1, v1, kl1, fl, ps, n, g.cells, out, d_count);
-  CK(cudaGetLastError());
-  eng->launches += 6;
+  CK(launch(eng, scan_key_kernel, nb, 256, 0, st, in, n, g, k0, v0, kl0));
+  // stable: input order inside a voxel
+  const auto sort = [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, k0, k1, v0, v1, n, 0, end_bit, st); };
+  // labels ascending inside a voxel
+  const auto sort_kl = [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortKeys(t, b, kl0, kl1, n, 0, 32 + end_bit, st); };
+  const auto scan = [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, fl, ps, n, st); };
+  CK(cub_reserve(*b.tmp, sort, sort_kl, scan));
+  CK(cub_call(eng, *b.tmp, sort));
+  CK(cub_call(eng, *b.tmp, sort_kl));
+  CK(launch(eng, scan_heads_kernel, nb, 256, 0, st, k1, n, fl));
+  CK(cub_call(eng, *b.tmp, scan));
+  CK(launch(eng, scan_centroid_kernel, nb, 256, 0, st, in, k1, v1, kl1, fl, ps, n, g.cells, out, d_count));
   done = true;
   if (runs)
     *runs = VoxelRuns{true, g.cells};
@@ -1716,22 +1714,17 @@ int ns_sample_model(mcl3dl_engine* eng, DeviceCtx& c, int k, uint32_t n, const N
   uint64_t* q = static_cast<uint64_t*>(c.n_q[k].p);
   uint64_t* cum = static_cast<uint64_t*>(c.n_cum.p);
   const int nb = static_cast<int>((n + 255) / 256);
-  ns_key_kernel<<<nb, 256, 0, st>>>(clipped, n, ng.g, k0, v0);
-  size_t t_sort = 0, t_scan = 0;
-  CK(cub::DeviceRadixSort::SortPairs(nullptr, t_sort, k0, k1, v0, v1, n, 0, end_bit, st));
-  CK(cub::DeviceScan::InclusiveSum(nullptr, t_scan, q, cum, static_cast<int>(n), st));
-  if ((rc = reserve(eng, c.n_tmp, std::max(t_sort, t_scan) + 256)))
-    return rc;
-  size_t tsz = c.n_tmp.cap;
-  CK(cub::DeviceRadixSort::SortPairs(c.n_tmp.p, tsz, k0, k1, v0, v1, n, 0, end_bit, st));  // stable: ascending index in a cell
-  ns_gather_kernel<<<nb, 256, 0, st>>>(clipped, v1, n, spts);
-  ns_normal_kernel<<<static_cast<int>((n + 127) / 128), 128, 0, st>>>(clipped, n, ng, k1, spts, fpc[0], fpc[1], fpc[2], max_weight, scale,
-                                                                     static_cast<float*>(c.n_normals[k].p),
-                                                                     static_cast<uint32_t*>(c.n_nb[k].p), q, word + 12 + k);
-  tsz = c.n_tmp.cap;
-  CK(cub::DeviceScan::InclusiveSum(c.n_tmp.p, tsz, q, cum, static_cast<int>(n), st));  // exact: the total stays below 2^62
-  CK(cudaGetLastError());
-  eng->launches += 5;
+  CK(launch(eng, ns_key_kernel, nb, 256, 0, st, clipped, n, ng.g, k0, v0));
+  // stable: ascending index in a cell
+  const auto sort = [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, k0, k1, v0, v1, n, 0, end_bit, st); };
+  // exact: the total stays below 2^62
+  const auto scan = [&](void* t, size_t& b) { return cub::DeviceScan::InclusiveSum(t, b, q, cum, static_cast<int>(n), st); };
+  CK(cub_reserve(c.n_tmp, sort, scan));
+  CK(cub_call(eng, c.n_tmp, sort));
+  CK(launch(eng, ns_gather_kernel, nb, 256, 0, st, clipped, v1, n, spts));
+  CK(launch(eng, ns_normal_kernel, static_cast<int>((n + 127) / 128), 128, 0, st, clipped, n, ng, k1, spts, fpc[0], fpc[1], fpc[2],
+            max_weight, scale, static_cast<float*>(c.n_normals[k].p), static_cast<uint32_t*>(c.n_nb[k].p), q, word + 12 + k));
+  CK(cub_call(eng, c.n_tmp, scan));
   mcl3dl_point* out = static_cast<mcl3dl_point*>(c.n_out[k].p);
   if (num == 0)
     return MCL3DL_OK;
@@ -1756,17 +1749,11 @@ int ns_sample_model(mcl3dl_engine* eng, DeviceCtx& c, int k, uint32_t n, const N
       return rc;
     uint32_t *didx = static_cast<uint32_t*>(c.n_didx.p), *flags = static_cast<uint32_t*>(c.n_dflag.p), *pos = static_cast<uint32_t*>(c.n_dpos.p);
     const int db = static_cast<int>((cnt + 255) / 256);
-    ns_draw_kernel<<<db, 256, 0, st>>>(cum, n, seed, static_cast<uint32_t>(k), d0, cnt, didx, first);
-    ns_first_flag_kernel<<<db, 256, 0, st>>>(didx, first, d0, cnt, flags);
-    size_t t_pos = 0;
-    CK(cub::DeviceScan::ExclusiveSum(nullptr, t_pos, flags, pos, static_cast<int>(cnt), st));
-    if ((rc = reserve(eng, c.n_tmp, t_pos + 256)))
-      return rc;
-    tsz = c.n_tmp.cap;
-    CK(cub::DeviceScan::ExclusiveSum(c.n_tmp.p, tsz, flags, pos, static_cast<int>(cnt), st));
-    ns_take_kernel<<<db, 256, 0, st>>>(clipped, didx, flags, pos, cnt, carry, num, out, word + 14);
-    CK(cudaGetLastError());
-    eng->launches += 4;
+    CK(launch(eng, ns_draw_kernel, db, 256, 0, st, cum, n, seed, static_cast<uint32_t>(k), d0, cnt, didx, first));
+    CK(launch(eng, ns_first_flag_kernel, db, 256, 0, st, didx, first, d0, cnt, flags));
+    CK(cub_call(eng, c.n_tmp,
+                [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, flags, pos, static_cast<int>(cnt), st); }));
+    CK(launch(eng, ns_take_kernel, db, 256, 0, st, clipped, didx, flags, pos, cnt, carry, num, out, word + 14));
     CK(cudaMemcpyAsync(c.h_pinned.p, word + 14, 4, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     std::memcpy(&carry, c.h_pinned.p, 4);
@@ -2123,10 +2110,8 @@ static int map_intake(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_map_cloud* 
   mcl3dl_point* in = static_cast<mcl3dl_point*>(c.i_cloud.p);
   float* in_int = static_cast<float*>(c.i_cloud_int.p);
   const int nb = static_cast<int>((n + 255) / 256);
-  map_read_kernel<<<nb, 256, 0, st>>>(static_cast<const unsigned char*>(c.i_raw.p), v.width, n, v.row_step, v.point_step, v.offset[0],
-                                      v.offset[1], v.offset[2], m->intensity_offset, m->label_offset, in, in_int);
-  CK(cudaGetLastError());
-  eng->launches++;
+  CK(launch(eng, map_read_kernel, nb, 256, 0, st, static_cast<const unsigned char*>(c.i_raw.p), v.width, n, v.row_step, v.point_step,
+            v.offset[0], v.offset[1], v.offset[2], m->intensity_offset, m->label_offset, in, in_int));
   uint32_t* count = static_cast<uint32_t*>(c.i_count.p);
   CK(cudaMemsetAsync(count, 0, 64, st));
   mcl3dl_point* out = static_cast<mcl3dl_point*>(c.i_pts.p);
@@ -2141,11 +2126,9 @@ static int map_intake(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_map_cloud* 
   }
   if (runs.sorted)
   {
-    map_intensity_kernel<<<nb, 256, 0, st>>>(static_cast<const uint32_t*>(c.i_keys[1].p), static_cast<const uint32_t*>(c.i_vals[1].p),
-                                             static_cast<const uint32_t*>(c.i_flags.p), static_cast<const uint32_t*>(c.i_pos.p), n,
-                                             runs.nonfinite_key, in_int, out_int);
-    CK(cudaGetLastError());
-    eng->launches++;
+    CK(launch(eng, map_intensity_kernel, nb, 256, 0, st, static_cast<const uint32_t*>(c.i_keys[1].p),
+              static_cast<const uint32_t*>(c.i_vals[1].p), static_cast<const uint32_t*>(c.i_flags.p),
+              static_cast<const uint32_t*>(c.i_pos.p), n, runs.nonfinite_key, in_int, out_int));
   }
   downsampled = done;
   if (!done)
@@ -2153,17 +2136,9 @@ static int map_intake(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_map_cloud* 
     // unfiltered: the finite points in order (a KdTreeFLANN input drops the others; the grids would index them)
     uint32_t* fl = static_cast<uint32_t*>(c.i_flags.p);
     uint32_t* ps = static_cast<uint32_t*>(c.i_pos.p);
-    map_finite_flags_kernel<<<nb, 256, 0, st>>>(in, n, fl);
-    CK(cudaGetLastError());
-    size_t t_scan = 0;
-    CK(cub::DeviceScan::ExclusiveSum(nullptr, t_scan, fl, ps, n, st));
-    if ((rc = reserve(eng, c.i_tmp, t_scan + 256)))
-      return rc;
-    size_t tsz = c.i_tmp.cap;
-    CK(cub::DeviceScan::ExclusiveSum(c.i_tmp.p, tsz, fl, ps, n, st));
-    map_compact_kernel<<<nb, 256, 0, st>>>(in, in_int, fl, ps, n, out, out_int, count);
-    CK(cudaGetLastError());
-    eng->launches += 3;
+    CK(launch(eng, map_finite_flags_kernel, nb, 256, 0, st, in, n, fl));
+    CK(cub_call(eng, c.i_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, fl, ps, n, st); }));
+    CK(launch(eng, map_compact_kernel, nb, 256, 0, st, in, in_int, fl, ps, n, out, out_int, count));
   }
   CK(cudaMemcpyAsync(c.h_pinned.p, count, 4, cudaMemcpyDeviceToHost, st));
   CK(cudaEventRecord(c.ev[1], st));
@@ -2608,10 +2583,8 @@ static int weight_pass1(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_result* r
   unsigned int* tk;
   if (int rc = weight_scratch(eng, c, n, 0, &nblk, &slots, &tk))
     return rc;
-  weight_kernel<<<nblk, kBlockThreads, 0, c.stream>>>(rec, prior, extra, static_cast<int>(n), static_cast<int>(n_lik),
-                                                      static_cast<float*>(c.d_w.p), slots, tk, h_part);
-  CK(cudaGetLastError());
-  eng->launches++;
+  CK(launch(eng, weight_kernel, nblk, kBlockThreads, 0, c.stream, rec, prior, extra, static_cast<int>(n), static_cast<int>(n_lik),
+            static_cast<float*>(c.d_w.p), slots, tk, h_part));
   *folded = slots + nblk;
   return MCL3DL_OK;
 }
@@ -2625,10 +2598,8 @@ static int weight_pass2(mcl3dl_engine* eng, DeviceCtx& c, const WeightPartial* p
   unsigned int* tk;
   if (int rc = weight_scratch(eng, c, n, 1, &nblk, &slots, &tk))
     return rc;
-  normalize_kernel<<<nblk, kBlockThreads, 0, c.stream>>>(static_cast<const float*>(c.d_w.p), static_cast<int>(n), pass1, total,
-                                                         static_cast<int>(index_offset), post, slots, tk, h_part);
-  CK(cudaGetLastError());
-  eng->launches++;
+  CK(launch(eng, normalize_kernel, nblk, kBlockThreads, 0, c.stream, static_cast<const float*>(c.d_w.p), static_cast<int>(n), pass1,
+            total, static_cast<int>(index_offset), post, slots, tk, h_part));
   *folded = slots + nblk;
   return MCL3DL_OK;
 }
@@ -2759,9 +2730,7 @@ int mcl3dl_particles_predict(mcl3dl_engine* eng, const mcl3dl_pose* a, const mcl
   const float cp[3] = {b->px, b->py, b->pz}, cq[4] = {b->qx, b->qy, b->qz, b->qw};
   const MotionDev m = pf_set_odoms(pp, pq, cp, cq, time_diff, tc_lin, tc_ang);
   const uint32_t n = static_cast<uint32_t>(c.r_n);
-  pf_predict_kernel<<<(n + 255) / 256, 256, 0, c.stream>>>(static_cast<PfState*>(c.r_states[c.r_cur].p), n, m);
-  CK(cudaGetLastError());
-  eng->launches++;
+  CK(launch(eng, pf_predict_kernel, (n + 255) / 256, 256, 0, c.stream, static_cast<PfState*>(c.r_states[c.r_cur].p), n, m));
   return MCL3DL_OK;  // stream-ordered before whatever comes next; get() / measure_update() synchronise
 }
 
@@ -2776,7 +2745,7 @@ int mcl3dl_particles_resample(mcl3dl_engine* eng, const float sigma_pos[3], cons
   CK(cudaSetDevice(c.dev));
   const uint32_t n = static_cast<uint32_t>(c.r_n);
   float* accum = static_cast<float*>(c.r_accum.p);
-  pf_accum_kernel<<<1, 32, 0, c.stream>>>(static_cast<const float*>(c.r_prob.p), n, accum, accum + n);  // one warp, in order
+  CK(launch(eng, pf_accum_kernel, 1, 32, 0, c.stream, static_cast<const float*>(c.r_prob.p), n, accum, accum + n));  // one warp, in order
   Sigma6 sg;
   for (int k = 0; k < 3; ++k)
   {
@@ -2784,12 +2753,9 @@ int mcl3dl_particles_resample(mcl3dl_engine* eng, const float sigma_pos[3], cons
     sg.v[k + 3] = sigma_rpy[k];
   }
   ++c.r_calls;
-  pf_resample_kernel<<<(n + 255) / 256, 256, 0, c.stream>>>(static_cast<const PfState*>(c.r_states[c.r_cur].p), accum, accum + n, n,
-                                                           initial_frac, seed, c.r_calls, sg,
-                                                           static_cast<PfState*>(c.r_states[1 - c.r_cur].p),
-                                                           static_cast<float*>(c.r_prob.p));
-  CK(cudaGetLastError());
-  eng->launches += 2;
+  CK(launch(eng, pf_resample_kernel, (n + 255) / 256, 256, 0, c.stream, static_cast<const PfState*>(c.r_states[c.r_cur].p), accum,
+            accum + n, n, initial_frac, seed, c.r_calls, sg, static_cast<PfState*>(c.r_states[1 - c.r_cur].p),
+            static_cast<float*>(c.r_prob.p)));
   c.r_cur = 1 - c.r_cur;
   return MCL3DL_OK;
 }
@@ -2814,9 +2780,8 @@ int mcl3dl_particles_redraw_odom_noise(mcl3dl_engine* eng, double lin_lin, doubl
   sg.aa = ang_ang;
   sg.al = ang_lin;
   ++c.r_redraw_calls;
-  pf_redraw_kernel<<<(n + 255) / 256, 256, 0, c.stream>>>(static_cast<PfState*>(c.r_states[c.r_cur].p), n, seed, c.r_redraw_calls, sg);
-  CK(cudaGetLastError());
-  eng->launches++;
+  CK(launch(eng, pf_redraw_kernel, (n + 255) / 256, 256, 0, c.stream, static_cast<PfState*>(c.r_states[c.r_cur].p), n, seed,
+            c.r_redraw_calls, sg));
   CK(cudaStreamSynchronize(c.stream));
   return MCL3DL_OK;
 }
@@ -2840,20 +2805,20 @@ int mcl3dl_particles_noise(mcl3dl_engine* eng, const float sigma_pos[3], const f
   CK(cudaSetDevice(c.dev));
   const uint32_t n = static_cast<uint32_t>(c.r_n);
   ++c.r_noise_calls;
-  pf_noise_kernel<<<(n + 255) / 256, 256, 0, c.stream>>>(static_cast<PfState*>(c.r_states[c.r_cur].p), n, seed, c.r_noise_calls, sg);
-  CK(cudaGetLastError());
-  eng->launches++;
+  CK(launch(eng, pf_noise_kernel, (n + 255) / 256, 256, 0, c.stream, static_cast<PfState*>(c.r_states[c.r_cur].p), n, seed,
+            c.r_noise_calls, sg));
   CK(cudaStreamSynchronize(c.stream));
   return MCL3DL_OK;
 }
 
 // An update of the resident set whose likelihood one thread-per-particle kernel computes (pf_imu_kernel,
-// pf_landmark_kernel): launch(d_rec, lik) writes a unit record and the likelihood of every particle, and the weight fold
-// takes the likelihood as the extra factor: w = prior * (((1 * 1) * 1) * lik) = prior * lik; n_lik = 0 makes every
-// particle's match ratio 0.  The posterior replaces the resident probabilities unless the update is discarded.
+// pf_landmark_kernel): kernel(d_rec, lik) launches the kernel that writes a unit record and the likelihood of every
+// particle, and the weight fold takes the likelihood as the extra factor: w = prior * (((1 * 1) * 1) * lik) = prior * lik;
+// n_lik = 0 makes every particle's match ratio 0.  The posterior replaces the resident probabilities unless the update is
+// discarded.
 extern "C++" {
-template <typename Launch>
-static int resident_likelihood_update(mcl3dl_engine* eng, DeviceCtx& c, mcl3dl_update_summary* summary, Launch launch)
+template <typename Kernel>
+static int resident_likelihood_update(mcl3dl_engine* eng, DeviceCtx& c, mcl3dl_update_summary* summary, Kernel kernel)
 {
   const size_t P = c.r_n;
   CK(cudaSetDevice(c.dev));
@@ -2863,9 +2828,7 @@ static int resident_likelihood_update(mcl3dl_engine* eng, DeviceCtx& c, mcl3dl_u
     return rc;
   mcl3dl_result* d_rec = static_cast<mcl3dl_result*>(c.d_out.p);
   float* lik = static_cast<float*>(c.r_extra.p);
-  launch(d_rec, lik);
-  CK(cudaGetLastError());
-  eng->launches++;
+  CK(kernel(d_rec, lik));
   float* prob = static_cast<float*>(c.r_prob.p);
   WeightPartial* h_part = reinterpret_cast<WeightPartial*>(static_cast<char*>(c.h_pinned.p) + s.o_part);
   if ((rc = fold_weights(eng, c, d_rec, prob, lik, prob, P, 0, 0, h_part, nullptr)))
@@ -2889,7 +2852,8 @@ int mcl3dl_particles_imu_update(mcl3dl_engine* eng, const float acc_measure[3], 
   const ImuDev m = pf_imu_setup(acc_measure, sigma);
   const uint32_t n32 = static_cast<uint32_t>(c.r_n);
   return resident_likelihood_update(eng, c, summary, [&](mcl3dl_result* d_rec, float* lik) {
-    pf_imu_kernel<<<(n32 + 255) / 256, 256, 0, c.stream>>>(static_cast<const PfState*>(c.r_states[c.r_cur].p), n32, m, d_rec, lik);
+    return launch(eng, pf_imu_kernel, (n32 + 255) / 256, 256, 0, c.stream, static_cast<const PfState*>(c.r_states[c.r_cur].p), n32, m,
+                  d_rec, lik);
   });
 }
 
@@ -2920,7 +2884,8 @@ int mcl3dl_particles_landmark_update(mcl3dl_engine* eng, const mcl3dl_landmark_p
   std::memcpy(m.sigma_inv, params->sigma_inv, sizeof(m.sigma_inv));
   const uint32_t n32 = static_cast<uint32_t>(c.r_n);
   return resident_likelihood_update(eng, c, summary, [&](mcl3dl_result* d_rec, float* lik) {
-    pf_landmark_kernel<<<(n32 + 255) / 256, 256, 0, c.stream>>>(static_cast<const PfState*>(c.r_states[c.r_cur].p), n32, m, d_rec, lik);
+    return launch(eng, pf_landmark_kernel, (n32 + 255) / 256, 256, 0, c.stream, static_cast<const PfState*>(c.r_states[c.r_cur].p),
+                  n32, m, d_rec, lik);
   });
 }
 
@@ -2933,9 +2898,7 @@ int mcl3dl_particles_reset_odom_err_integ(mcl3dl_engine* eng)
     return MCL3DL_ERR_INVALID_ARG;
   CK(cudaSetDevice(c.dev));
   const uint32_t n = static_cast<uint32_t>(c.r_n);
-  pf_reset_odom_err_kernel<<<(n + 255) / 256, 256, 0, c.stream>>>(static_cast<PfState*>(c.r_states[c.r_cur].p), n);
-  CK(cudaGetLastError());
-  eng->launches++;
+  CK(launch(eng, pf_reset_odom_err_kernel, (n + 255) / 256, 256, 0, c.stream, static_cast<PfState*>(c.r_states[c.r_cur].p), n));
   CK(cudaStreamSynchronize(c.stream));
   return MCL3DL_OK;
 }
@@ -2950,10 +2913,8 @@ int mcl3dl_particles_get_poses(mcl3dl_engine* eng, mcl3dl_pose* out, size_t n)
   CK(cudaSetDevice(c.dev));
   const uint32_t n32 = static_cast<uint32_t>(n);
   // r_poses (room for n poses since the set was sized) is the staging buffer; an update repacks it before it reads it
-  pf_poses_kernel<<<(n32 + 255) / 256, 256, 0, c.stream>>>(static_cast<const PfState*>(c.r_states[c.r_cur].p), n32,
-                                                            static_cast<mcl3dl_pose*>(c.r_poses.p));
-  CK(cudaGetLastError());
-  eng->launches++;
+  CK(launch(eng, pf_poses_kernel, (n32 + 255) / 256, 256, 0, c.stream, static_cast<const PfState*>(c.r_states[c.r_cur].p), n32,
+            static_cast<mcl3dl_pose*>(c.r_poses.p)));
   CK(cudaMemcpyAsync(out, c.r_poses.p, n * sizeof(mcl3dl_pose), cudaMemcpyDeviceToHost, c.stream));
   CK(cudaStreamSynchronize(c.stream));
   return MCL3DL_OK;
@@ -2992,10 +2953,8 @@ int mcl3dl_particles_init(mcl3dl_engine* eng, size_t n, const mcl3dl_init_params
     return rc;
   const uint32_t n32 = static_cast<uint32_t>(n);
   ++c.r_init_calls;
-  pf_init_kernel<<<(n32 + 255) / 256, 256, 0, c.stream>>>(static_cast<PfState*>(c.r_states[0].p), static_cast<float*>(c.r_prob.p),
-                                                         n32, seed, c.r_init_calls, g);
-  CK(cudaGetLastError());
-  eng->launches++;
+  CK(launch(eng, pf_init_kernel, (n32 + 255) / 256, 256, 0, c.stream, static_cast<PfState*>(c.r_states[0].p),
+            static_cast<float*>(c.r_prob.p), n32, seed, c.r_init_calls, g));
   CK(cudaStreamSynchronize(c.stream));
   c.r_n = n;
   c.r_cur = 0;
@@ -3013,19 +2972,15 @@ int mcl3dl_particles_resize(mcl3dl_engine* eng, size_t num)
   CK(cudaSetDevice(c.dev));
   const uint32_t n = static_cast<uint32_t>(c.r_n), num32 = static_cast<uint32_t>(num);
   float* accum = static_cast<float*>(c.r_accum.p);
-  pf_accum_kernel<<<1, 32, 0, c.stream>>>(static_cast<const float*>(c.r_prob.p), n, accum, accum + n);
-  CK(cudaGetLastError());
+  CK(launch(eng, pf_accum_kernel, 1, 32, 0, c.stream, static_cast<const float*>(c.r_prob.p), n, accum, accum + n));
   // the pick reads the current states and accum: they keep their storage until it has run
   int rc = reserve_resident(eng, c, num, {&c.r_states[c.r_cur], &c.r_accum});
   if (rc != MCL3DL_OK)
     return rc;
   float* pscan = static_cast<float*>(c.r_extra.p);
-  gl_pscan_kernel<<<1, 32, 0, c.stream>>>(accum, n, num32, pscan);
-  gl_resize_kernel<<<(num32 + 255) / 256, 256, 0, c.stream>>>(static_cast<const PfState*>(c.r_states[c.r_cur].p), accum, n, pscan, num32,
-                                                            static_cast<PfState*>(c.r_states[1 - c.r_cur].p),
-                                                            static_cast<float*>(c.r_prob.p));
-  CK(cudaGetLastError());
-  eng->launches += 3;
+  CK(launch(eng, gl_pscan_kernel, 1, 32, 0, c.stream, accum, n, num32, pscan));
+  CK(launch(eng, gl_resize_kernel, (num32 + 255) / 256, 256, 0, c.stream, static_cast<const PfState*>(c.r_states[c.r_cur].p), accum, n,
+            pscan, num32, static_cast<PfState*>(c.r_states[1 - c.r_cur].p), static_cast<float*>(c.r_prob.p)));
   c.r_cur = 1 - c.r_cur;
   c.r_n = num;
   if ((rc = reserve_resident(eng, c, num)))  // now the other state buffer and accum as well
@@ -3109,9 +3064,7 @@ int mcl3dl_global_localization(mcl3dl_engine* eng, const mcl3dl_point* pts, size
     h_bbox[9 + k] = 0u;
   }
   CK(cudaMemcpyAsync(d_bbox.p, h_bbox, sizeof(h_bbox), cudaMemcpyHostToDevice, st));
-  bbox_kernel<<<std::min(nb, c.sm_count * 8), 256, 0, st>>>(ds, n_ds, wx, wy, wz, static_cast<uint32_t*>(d_bbox.p));
-  CK(cudaGetLastError());
-  eng->launches++;
+  CK(launch(eng, bbox_kernel, std::min(nb, c.sm_count * 8), 256, 0, st, ds, n_ds, wx, wy, wz, static_cast<uint32_t*>(d_bbox.p)));
   CK(cudaMemcpyAsync(h_bbox, d_bbox.p, sizeof(h_bbox), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   float sc_min[3], sc_max[3];
@@ -3146,17 +3099,9 @@ int mcl3dl_global_localization(mcl3dl_engine* eng, const mcl3dl_point* pts, size
   g.pts = static_cast<const float4*>(d_grid.p);
   uint32_t* flags = static_cast<uint32_t*>(d_flags.p);
   uint32_t* pos = static_cast<uint32_t*>(d_pos.p);
-  gl_flag_kernel<<<nb, 256, 0, st>>>(ds, n_ds, g, m, flags);
-  CK(cudaGetLastError());
-  size_t t_scan = 0;
-  CK(cub::DeviceScan::ExclusiveSum(nullptr, t_scan, flags, pos, n_ds, st));
-  if ((rc = reserve(eng, d_tmp, t_scan + 256)))
-    return rc;
-  size_t tsz = d_tmp.cap;
-  CK(cub::DeviceScan::ExclusiveSum(d_tmp.p, tsz, flags, pos, n_ds, st));
-  scan_compact_kernel<<<nb, 256, 0, st>>>(ds, flags, pos, n_ds, static_cast<mcl3dl_point*>(d_seeds.p), count + 1);
-  CK(cudaGetLastError());
-  eng->launches += 3;
+  CK(launch(eng, gl_flag_kernel, nb, 256, 0, st, ds, n_ds, g, m, flags));
+  CK(cub_call(eng, d_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, flags, pos, n_ds, st); }));
+  CK(launch(eng, scan_compact_kernel, nb, 256, 0, st, ds, flags, pos, n_ds, static_cast<mcl3dl_point*>(d_seeds.p), count + 1));
   uint32_t n_seeds = 0;
   CK(cudaMemcpyAsync(&n_seeds, count + 1, 4, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
@@ -3180,11 +3125,9 @@ int mcl3dl_global_localization(mcl3dl_engine* eng, const mcl3dl_point* pts, size
     return rc;
   const float prob = gl_probability(n_seeds);
   const uint32_t np32 = static_cast<uint32_t>(n_particles);
-  gl_fill_kernel<<<(np32 + 255) / 256, 256, 0, st>>>(static_cast<const mcl3dl_point*>(d_seeds.p), static_cast<const Q4*>(d_yaw.p),
-                                                     static_cast<uint32_t>(gp->div_yaw), np32, prob,
-                                                     static_cast<PfState*>(c.r_states[0].p), static_cast<float*>(c.r_prob.p));
-  CK(cudaGetLastError());
-  eng->launches++;
+  CK(launch(eng, gl_fill_kernel, (np32 + 255) / 256, 256, 0, st, static_cast<const mcl3dl_point*>(d_seeds.p),
+            static_cast<const Q4*>(d_yaw.p), static_cast<uint32_t>(gp->div_yaw), np32, prob, static_cast<PfState*>(c.r_states[0].p),
+            static_cast<float*>(c.r_prob.p)));
   CK(cudaEventRecord(e1, st));
   CK(cudaStreamSynchronize(st));
   c.r_n = n_particles;
@@ -3216,11 +3159,8 @@ static int resident_update(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_point*
   const float nd_a = with_odom ? static_cast<float>(1.0 / std::sqrt(2.0 * M_PI * sg * sg)) : 1.0f;
   const float nd_sq2 = with_odom ? static_cast<float>(sg * sg * 2.0) : 1.0f;
   const uint32_t n32 = static_cast<uint32_t>(P);
-  pf_pack_kernel<<<(n32 + 255) / 256, 256, 0, st>>>(static_cast<const PfState*>(c.r_states[c.r_cur].p), n32, nd_a, nd_sq2,
-                                                  static_cast<mcl3dl_pose*>(c.r_poses.p),
-                                                  with_odom ? static_cast<float*>(c.r_extra.p) : nullptr);
-  CK(cudaGetLastError());
-  eng->launches++;
+  CK(launch(eng, pf_pack_kernel, (n32 + 255) / 256, 256, 0, st, static_cast<const PfState*>(c.r_states[c.r_cur].p), n32, nd_a, nd_sq2,
+            static_cast<mcl3dl_pose*>(c.r_poses.p), with_odom ? static_cast<float*>(c.r_extra.p) : nullptr));
   mcl3dl_result* d_rec = static_cast<mcl3dl_result*>(c.d_out.p);
   rc = launch_models(eng, c, static_cast<const mcl3dl_pose*>(c.r_poses.p), P, d_lik, n_lik, d_beam, n_beam, d_org, n_origins,
                      d_rec, nullptr, st, false);
@@ -3352,24 +3292,16 @@ static int scan_prepare_from(mcl3dl_engine* eng, DeviceCtx& c, size_t n_raw, con
   const ClipDev cb = scan_clip_window(sp->beam_clip_near, sp->beam_clip_far, sp->beam_clip_z_min, sp->beam_clip_z_max);
   uint32_t *fa = static_cast<uint32_t*>(c.s_flags[0].p), *fb = static_cast<uint32_t*>(c.s_flags[1].p);
   uint32_t *pa = static_cast<uint32_t*>(c.s_pos[0].p), *pb = static_cast<uint32_t*>(c.s_pos[1].p);
-  scan_clip_flags_kernel<<<nb, 256, 0, st>>>(d_ds, counts + 0, ca, cb, fa, fb, n);
-  size_t t_scan = 0;
-  CK(cub::DeviceScan::ExclusiveSum(nullptr, t_scan, fa, pa, n, st));
-  if ((rc = reserve(eng, c.s_tmp, t_scan + 256)))
-    return rc;
-  size_t tsz = c.s_tmp.cap;
-  CK(cub::DeviceScan::ExclusiveSum(c.s_tmp.p, tsz, fa, pa, n, st));
-  tsz = c.s_tmp.cap;
-  CK(cub::DeviceScan::ExclusiveSum(c.s_tmp.p, tsz, fb, pb, n, st));
-  scan_compact_kernel<<<nb, 256, 0, st>>>(d_ds, fa, pa, n, static_cast<mcl3dl_point*>(c.s_clip[0].p), counts + 1);
-  scan_compact_kernel<<<nb, 256, 0, st>>>(d_ds, fb, pb, n, static_cast<mcl3dl_point*>(c.s_clip[1].p), counts + 2);
+  CK(launch(eng, scan_clip_flags_kernel, nb, 256, 0, st, d_ds, counts + 0, ca, cb, fa, fb, n));
+  CK(cub_call(eng, c.s_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, fa, pa, n, st); }));
+  CK(cub_call(eng, c.s_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, fb, pb, n, st); }));
+  CK(launch(eng, scan_compact_kernel, nb, 256, 0, st, d_ds, fa, pa, n, static_cast<mcl3dl_point*>(c.s_clip[0].p), counts + 1));
+  CK(launch(eng, scan_compact_kernel, nb, 256, 0, st, d_ds, fb, pb, n, static_cast<mcl3dl_point*>(c.s_clip[1].p), counts + 2));
   for (int k = 0; k < 2; ++k)
     if (num[k])
-      scan_sample_kernel<<<(num[k] + 255) / 256, 256, 0, st>>>(static_cast<const mcl3dl_point*>(c.s_clip[k].p), counts + 1 + k, num[k],
-                                                             sp->seed, static_cast<uint32_t>(k),
-                                                             static_cast<mcl3dl_point*>(c.s_out[k].p), counts + 3 + k);
-  CK(cudaGetLastError());
-  eng->launches += 5;
+      CK(launch(eng, scan_sample_kernel, (num[k] + 255) / 256, 256, 0, st, static_cast<const mcl3dl_point*>(c.s_clip[k].p),
+                counts + 1 + k, num[k], sp->seed, static_cast<uint32_t>(k), static_cast<mcl3dl_point*>(c.s_out[k].p),
+                counts + 3 + k));
   uint32_t h_counts[5];
   CK(cudaMemcpyAsync(c.h_pinned.p, counts, sizeof(h_counts), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
@@ -3433,12 +3365,9 @@ int mcl3dl_scan_accumulate(mcl3dl_engine* eng, const mcl3dl_cloud_view* v, const
   const uint32_t n32 = static_cast<uint32_t>(n);
   const double* t = tf->translation;
   const double* q = tf->rotation;
-  accum_cloud_kernel<<<(n32 + 255) / 256, 256, 0, st>>>(static_cast<const unsigned char*>(c.a_raw.p), v->width, n32, v->row_step,
-                                                        v->point_step, v->offset[0], v->offset[1], v->offset[2], t[0], t[1], t[2],
-                                                        q[0], q[1], q[2], q[3], c.a_clouds,
-                                                        static_cast<mcl3dl_point*>(c.a_pts.p) + c.a_n);
-  CK(cudaGetLastError());
-  eng->launches++;
+  CK(launch(eng, accum_cloud_kernel, (n32 + 255) / 256, 256, 0, st, static_cast<const unsigned char*>(c.a_raw.p), v->width, n32,
+            v->row_step, v->point_step, v->offset[0], v->offset[1], v->offset[2], t[0], t[1], t[2], q[0], q[1], q[2], q[3], c.a_clouds,
+            static_cast<mcl3dl_point*>(c.a_pts.p) + c.a_n));
   CK(cudaStreamSynchronize(st));  // the caller may reuse data as soon as this returns
   c.a_n = total;
   c.a_clouds++;
@@ -3486,10 +3415,8 @@ int mcl3dl_scan_prepare_accumulated(mcl3dl_engine* eng, const mcl3dl_transform* 
   return scan_prepare_from(eng, c, c.a_n, sp, info, [&](cudaStream_t st) -> int {
     const double* t = tf->translation;
     const double* q = tf->rotation;
-    accum_transform_kernel<<<(n + 255) / 256, 256, 0, st>>>(static_cast<const mcl3dl_point*>(c.a_pts.p), n, t[0], t[1], t[2], q[0], q[1],
-                                                           q[2], q[3], c.a_dense ? 1 : 0, static_cast<mcl3dl_point*>(c.s_raw.p));
-    CK(cudaGetLastError());
-    eng->launches++;
+    CK(launch(eng, accum_transform_kernel, (n + 255) / 256, 256, 0, st, static_cast<const mcl3dl_point*>(c.a_pts.p), n, t[0], t[1], t[2],
+              q[0], q[1], q[2], q[3], c.a_dense ? 1 : 0, static_cast<mcl3dl_point*>(c.s_raw.p)));
     return MCL3DL_OK;
   });
 }
@@ -3554,9 +3481,8 @@ int mcl3dl_scan_sample_with_normal(mcl3dl_engine* eng, const mcl3dl_normal_sampl
     if (n[k])
     {
       const int nb = static_cast<int>((n[k] + 255) / 256);
-      scan_bbox_kernel<<<std::min(nb, c.sm_count * 8), 256, 0, st>>>(static_cast<const mcl3dl_point*>(c.s_clip[k].p), n[k], word + 6 * k);
-      CK(cudaGetLastError());
-      eng->launches++;
+      CK(launch(eng, scan_bbox_kernel, std::min(nb, c.sm_count * 8), 256, 0, st, static_cast<const mcl3dl_point*>(c.s_clip[k].p), n[k],
+                word + 6 * k));
     }
   CK(cudaMemcpyAsync(h_bbox, word, sizeof(h_bbox), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
@@ -3676,23 +3602,15 @@ int mcl3dl_match_output(mcl3dl_engine* eng, const mcl3dl_pose* pose, const mcl3d
   uint32_t* ps[2] = {static_cast<uint32_t*>(c.m_pos[0].p), static_cast<uint32_t*>(c.m_pos[1].p)};
   mcl3dl_point* tf = static_cast<mcl3dl_point*>(c.m_tf.p);
   const int nb = static_cast<int>((cnt + 255) / 256);
-  match_classify_kernel<<<nb, 256, 0, st>>>(src, n32, *pose, c.nn, m, tf, f[0], f[1]);
-  CK(cudaGetLastError());
-  size_t t_scan = 0;
-  CK(cub::DeviceScan::ExclusiveSum(nullptr, t_scan, f[0], ps[0], n32, st));
-  if ((rc = reserve(eng, c.m_tmp, t_scan + 256)))
-    return rc;
+  CK(launch(eng, match_classify_kernel, nb, 256, 0, st, src, n32, *pose, c.nn, m, tf, f[0], f[1]));
   char* hp = static_cast<char*>(c.m_host.p);
   uint32_t* h_counts = reinterpret_cast<uint32_t*>(hp);
   mcl3dl_point* h_out[2] = {reinterpret_cast<mcl3dl_point*>(hp + 64), reinterpret_cast<mcl3dl_point*>(hp + 64 + cnt * 16)};
   for (int k = 0; k < 2; ++k)
   {
-    size_t tsz = c.m_tmp.cap;
-    CK(cub::DeviceScan::ExclusiveSum(c.m_tmp.p, tsz, f[k], ps[k], n32, st));
-    scan_compact_kernel<<<nb, 256, 0, st>>>(tf, f[k], ps[k], n32, h_out[k], h_counts + k);
+    CK(cub_call(eng, c.m_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, f[k], ps[k], n32, st); }));
+    CK(launch(eng, scan_compact_kernel, nb, 256, 0, st, tf, f[k], ps[k], n32, h_out[k], h_counts + k));
   }
-  CK(cudaGetLastError());
-  eng->launches += 5;
   CK(cudaStreamSynchronize(st));
   *n_matched = h_counts[0];
   *n_unmatched = h_counts[1];
@@ -3742,12 +3660,10 @@ int mcl3dl_particles_estimate(mcl3dl_engine* eng, const mcl3dl_pose* prev, float
   double* parts = reinterpret_cast<double*>(static_cast<char*>(c.r_est.p) + hdr);
   const PfState* states = static_cast<const PfState*>(c.r_states[c.r_cur].p);
   const float* probs = static_cast<const float*>(c.r_prob.p);
-  pf_est_pass1_kernel<<<grid, 256, 0, st>>>(states, probs, n, b, parts);
-  pf_est_finish1_kernel<<<1, 32, 0, st>>>(parts, grid, h);
-  pf_est_pass2_kernel<<<grid, 256, 0, st>>>(states, probs, n, h, parts);
-  pf_est_finish2_kernel<<<1, 32, 0, st>>>(parts, grid, h);
-  CK(cudaGetLastError());
-  eng->launches += 4;
+  CK(launch(eng, pf_est_pass1_kernel, grid, 256, 0, st, states, probs, n, b, parts));
+  CK(launch(eng, pf_est_finish1_kernel, 1, 32, 0, st, parts, grid, h));
+  CK(launch(eng, pf_est_pass2_kernel, grid, 256, 0, st, states, probs, n, h, parts));
+  CK(launch(eng, pf_est_finish2_kernel, 1, 32, 0, st, parts, grid, h));
   char* hp = static_cast<char*>(c.h_pinned.p);
   CK(cudaMemcpyAsync(hp, h, sizeof(EstHeader), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
@@ -3866,9 +3782,7 @@ int mcl3dl_measure_exchange_device(mcl3dl_engine* eng, const mcl3dl_pose* d_pose
   if (rc != MCL3DL_OK)
     return rc;
   unsigned int* tk = static_cast<unsigned int*>(c.x_ticket.p);
-  exchange_signal_kernel<<<1, 32, 0, st>>>(c.xt, tk, tk + 1);
-  CK(cudaGetLastError());
-  eng->launches++;
+  CK(launch(eng, exchange_signal_kernel, 1, 32, 0, st, c.xt, tk, tk + 1));
   ++c.x_step;  // host mirror of the device counter; exact for eager calls, resynchronised by mcl3dl_exchange_current
   if (d_all_out)
     *d_all_out = static_cast<const mcl3dl_result*>(c.xchg.p) + static_cast<size_t>(c.x_step & 1u) * c.xt.world * c.x_local;
@@ -4171,11 +4085,9 @@ int mcl3dl_beam_cast(mcl3dl_engine* eng, const mcl3dl_pose* pose, const mcl3dl_p
   CK(cudaMemcpyAsync(dp, hp + 64, in_end - 64, cudaMemcpyHostToDevice, st));
   mcl3dl_beam_ray* h_rec = reinterpret_cast<mcl3dl_beam_ray*>(hp + o_rec);
   const auto kernel = kd ? beam_cast_kernel<true> : beam_cast_kernel<false>;
-  kernel<<<static_cast<unsigned>((n + kBlockThreads - 1) / kBlockThreads), kBlockThreads, 0, st>>>(
-      reinterpret_cast<const mcl3dl_pose*>(dp), reinterpret_cast<const float4*>(d_scan), static_cast<int>(n),
-      reinterpret_cast<const float*>(dp + o_org - 64), static_cast<uint32_t>(n_origins), c.dda, c.kd, c.nn, h_rec, bad);
-  CK(cudaGetLastError());
-  eng->launches++;
+  CK(launch(eng, kernel, static_cast<unsigned>((n + kBlockThreads - 1) / kBlockThreads), kBlockThreads, 0, st,
+            reinterpret_cast<const mcl3dl_pose*>(dp), reinterpret_cast<const float4*>(d_scan), static_cast<int>(n),
+            reinterpret_cast<const float*>(dp + o_org - 64), static_cast<uint32_t>(n_origins), c.dda, c.kd, c.nn, h_rec, bad));
   CK(cudaStreamSynchronize(st));
   if (*bad)
     return MCL3DL_ERR_INVALID_ARG;
