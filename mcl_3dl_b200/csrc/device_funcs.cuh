@@ -605,6 +605,29 @@ __device__ __forceinline__ int nnf_lookup(const NnFieldDev& f, float qx, float q
   return nnf_slot(f, d, (vx & 1) | ((vy & 1) << 1) | ((vz & 1) << 2), start);
 }
 
+// nnf_lookup in three steps, for callers that look up several queries at once (kernels.cuh: nf_phase_a): the address
+// of every query, then every directory load, then every decode.  Address: the directory index of q's coarse cell in
+// `cell` and the voxel's sub-index in `sub`; false when q lies outside the lattice (then `cell` is 0).  The bounds
+// test is a select, not a branch, so that nothing separates the loads that follow.  (nnf_lookup keeps its own branch: its callers, the KD
+// caster's searches, are compiled as they were.)
+__device__ __forceinline__ bool nnf_address(const NnFieldDev& f, float qx, float qy, float qz, size_t& cell, int& sub)
+{
+  const int vx = near_cell(qx, f.ox, f.inv_e), vy = near_cell(qy, f.oy, f.inv_e), vz = near_cell(qz, f.oz, f.inv_e);
+  const bool in = (static_cast<unsigned>(vx) < static_cast<unsigned>(f.nx)) &
+                  (static_cast<unsigned>(vy) < static_cast<unsigned>(f.ny)) &
+                  (static_cast<unsigned>(vz) < static_cast<unsigned>(f.nz));
+  cell = in ? (static_cast<size_t>(vz >> 1) * f.cny + (vy >> 1)) * f.cnx + (vx >> 1) : 0;
+  sub = (vx & 1) | ((vy & 1) << 1) | ((vz & 1) << 2);
+  return in;
+}
+
+// The directory entry at an address, loaded only when it is inside the lattice (`in`); otherwise an empty entry,
+// which nnf_slot decodes as no candidates at index 0.  nnf_slot then decodes the entry as nnf_lookup does.
+__device__ __forceinline__ uint2 nnf_entry(const NnFieldDev& f, bool in, size_t cell)
+{
+  return in ? __ldg(f.dir + cell) : make_uint2(0u, 0u);
+}
+
 // Warp-cooperative candidate scan (kernels.cuh: nf_warp_scan, phase B).  The candidate lists of a warp's evals are laid
 // end to end in one list of (eval, candidate) slots, lane after lane and within a lane u = 0 .. U - 1, so the list of
 // eval e = u * 32 + lane occupies slots [base, base + count) and is the o-th list in slot order, o = lane * U + u (its

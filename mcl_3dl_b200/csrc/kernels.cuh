@@ -631,6 +631,52 @@ __device__ __forceinline__ void nf_warp_scan(NfWarpSmem& ws, const NnGridDev& g,
   }
 }
 
+// Phase A of one warp trip of the NN-field kernels, for this lane's evals u = 0 .. kNfU - 1 (eval e = u * 32 + lane).
+// Eval u has a query when bit u of `has` is set: scan point sp[u] moved by the pose and rescaled.  Its query goes to
+// ws.q[e] (what an eval without one stores there is never read: it has no candidates), its candidate count to c[u] and
+// its first candidate to s[u] (0 and 0 without a query or outside the lattice, -1 in an overflow cell); returns the
+// lane's candidates in all.  Three passes: every transform and address, then every directory load, then every decode.
+// The loads depend only on their own transforms, and no branch separates them (nnf_address and nnf_entry select), so
+// they are in flight together: one round trip for the trip's directory entries.  A decode between them would cost one
+// each: the compiler does not move a load across nnf_slot's wide-cell branch.
+__device__ __forceinline__ int nf_phase_a(NfWarpSmem& ws, const NnGridDev& g, const Q4& rn, const F3& pos,
+                                          const float4 (&sp)[kNfU], uint32_t has, int (&c)[kNfU], uint32_t (&s)[kNfU])
+{
+  const int lane = threadIdx.x & 31;
+  const NnFieldDev& f = g.field;
+  uint32_t cell[kNfU];  // 32 bits: a staged field has fewer than 2^31 cells (engine.cu: build_nn_field)
+  int sub[kNfU];
+  bool in[kNfU];
+#pragma unroll
+  for (int u = 0; u < kNfU; ++u)
+  {
+    const bool h = (has >> u) & 1u;
+    F3 v;
+    v.x = sp[u].x;
+    v.y = sp[u].y;
+    v.z = sp[u].z;
+    const F3 t = transform_point(rn, pos, v);
+    // PointRepresentation::vectorize with rescale values (mcl_3dl.cpp:1270)
+    const float4 q = make_float4(fmul(t.x, g.wx), fmul(t.y, g.wy), fmul(t.z, g.wz), 0.0f);
+    ws.q[u * 32 + lane] = q;  // .w: nf_warp_scan's, once the eval's first slot is known
+    size_t a;
+    in[u] = nnf_address(f, q.x, q.y, q.z, a, sub[u]) & h;
+    cell[u] = static_cast<uint32_t>(a);
+  }
+  uint2 d[kNfU];
+#pragma unroll
+  for (int u = 0; u < kNfU; ++u) d[u] = nnf_entry(f, in[u], cell[u]);
+  int tot = 0;
+#pragma unroll
+  for (int u = 0; u < kNfU; ++u)
+  {
+    s[u] = 0;
+    c[u] = nnf_slot(f, d[u], sub[u], s[u]);
+    tot += max(c[u], 0);
+  }
+  return tot;
+}
+
 template <int TPP, bool STAGED, bool OVF>
 __global__ void __launch_bounds__(kBlockThreads, MCL3DL_NF_MINB)
     lik_kernel_nf(const mcl3dl_pose* __restrict__ poses, int P, const float4* __restrict__ scan, int N, NnGridDev g,
@@ -648,10 +694,8 @@ __global__ void __launch_bounds__(kBlockThreads, MCL3DL_NF_MINB)
   constexpr int PPB = kBlockThreads / TPP;
   const int sub = threadIdx.x / TPP;
   const int l = threadIdx.x % TPP;
-  const int lane = threadIdx.x & 31;
   NfWarpSmem& ws = nfw[threadIdx.x >> 5];
   const int n_groups = (P + PPB - 1) / PPB;
-  const NnFieldDev& f = g.field;
   uint32_t st_rows = 0, st_pts = 0;
   bool staged_ready = !(STAGED && N > 0);
   for (int grp = blockIdx.x; grp < n_groups; grp += gridDim.x)
@@ -682,33 +726,19 @@ __global__ void __launch_bounds__(kBlockThreads, MCL3DL_NF_MINB)
     for (int j0 = 0; j0 < N; j0 += kNfU * TPP)
     {
       const int j = j0 + l;
-      // ---- phase A: the queries and directory entries of up to kNfU evals (independent loads in flight)
-      int c[kNfU];
-      uint32_t s[kNfU];
-      int tot = 0;
+      // ---- phase A: this lane's points j, j + TPP, ... (clamped to the scan: the evals past it have no query)
+      float4 sp[kNfU];
+      uint32_t has = 0;
 #pragma unroll
       for (int u = 0; u < kNfU; ++u)
       {
-        c[u] = 0;
-        s[u] = 0;
-        float4 q = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-        if (live && j + u * TPP < N)
-        {
-          const float4 sp = STAGED ? pts[j + u * TPP] : __ldg(pts + j + u * TPP);
-          F3 v;
-          v.x = sp.x;
-          v.y = sp.y;
-          v.z = sp.z;
-          const F3 t = transform_point(rn, pos, v);
-          // PointRepresentation::vectorize with rescale values (mcl_3dl.cpp:1270)
-          q.x = fmul(t.x, g.wx);
-          q.y = fmul(t.y, g.wy);
-          q.z = fmul(t.z, g.wz);
-          c[u] = nnf_lookup(f, q.x, q.y, q.z, s[u]);
-          tot += max(c[u], 0);
-        }
-        ws.q[u * 32 + lane] = q;  // .w: nf_warp_scan's, once the eval's first slot is known
+        const int k = min(j + u * TPP, N - 1);
+        sp[u] = STAGED ? pts[k] : __ldg(pts + k);
+        has |= static_cast<uint32_t>(live && j + u * TPP < N) << u;
       }
+      int c[kNfU];
+      uint32_t s[kNfU];
+      const int tot = nf_phase_a(ws, g, rn, pos, sp, has, c, s);
       float d2[kNfU];
       nf_warp_scan<OVF>(ws, g, lp, c, s, tot, d2, st_rows, st_pts);
       // ---- the owners score their evals in scan order
@@ -775,10 +805,17 @@ __global__ void __launch_bounds__(kBlockThreads, MCL3DL_NF_MINB)
   const int s0 = (blockIdx.x % sh.n_slices) * sh.slice, s1 = min(N, s0 + sh.slice);
   const int p = group * 32 + lane;
   const bool live = p < P;
-  const NnFieldDev& f = g.field;
   uint32_t st_rows = 0, st_pts = 0;
   long long sum = 0;
   uint32_t cnt = 0;
+  // A trip's points j0 .. j0 + kNfU - 1 are the same for every lane: lane l loads point j0 + l % kNfU (clamped to the
+  // slice: the evals past it have no query), and phase A takes them from lanes 0 .. kNfU - 1 by shuffles.  One point
+  // per lane, not kNfU, stays in registers while the pose is normalised.
+  float4 pt;
+  auto load_points = [&](int j0) { pt = __ldg(scan + min(j0 + (lane & (kNfU - 1)), s1 - 1)); };
+  // the first trip's points do not depend on the pose: in flight with it
+  if (s0 < s1)
+    load_points(s0);
   F3 pos;
   Q4 rn;
   pos.x = pos.y = pos.z = 0.0f;
@@ -795,43 +832,29 @@ __global__ void __launch_bounds__(kBlockThreads, MCL3DL_NF_MINB)
   {
     keep = __float_as_uint(rn.x) ^ __float_as_uint(rn.y) ^ __float_as_uint(rn.z) ^ __float_as_uint(rn.w) ^
            __float_as_uint(pos.x) ^ __float_as_uint(pos.y) ^ __float_as_uint(pos.z);
+    if (s0 < s1)
+      keep ^= __float_as_uint(pt.x) ^ __float_as_uint(pt.y) ^ __float_as_uint(pt.z);
     pm_cut_sink(acc, p, live, keep);
     return;
   }
-  // every lane of the warp runs every trip (dead particles: no candidates), as in lik_kernel_nf
-  for (int j0 = s0; j0 < s1; j0 += kNfU)
+  // every lane of the warp runs every trip (dead particles: no candidates), as in lik_kernel_nf.  A later trip's points
+  // are loaded as the trip before it ends, so none stays live through a trip's candidate scan.
+  for (int j0 = s0; j0 < s1; j0 += kNfU, j0 < s1 ? load_points(j0) : void())
   {
-    // ---- phase A: one scan point per u, the same for every lane (one broadcast load)
-    int c[kNfU];
-    uint32_t s[kNfU];
-    int tot = 0;
+    // ---- phase A
+    float4 sp[kNfU];
+    uint32_t has = 0;
 #pragma unroll
     for (int u = 0; u < kNfU; ++u)
     {
-      c[u] = 0;
-      s[u] = 0;
-      float4 q = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-      if (j0 + u < s1)
-      {
-        const float4 sp = __ldg(scan + j0 + u);
-        if (live)
-        {
-          F3 v;
-          v.x = sp.x;
-          v.y = sp.y;
-          v.z = sp.z;
-          const F3 t = transform_point(rn, pos, v);
-          // PointRepresentation::vectorize with rescale values (mcl_3dl.cpp:1270)
-          q.x = fmul(t.x, g.wx);
-          q.y = fmul(t.y, g.wy);
-          q.z = fmul(t.z, g.wz);
-          c[u] = nnf_lookup(f, q.x, q.y, q.z, s[u]);
-          tot += max(c[u], 0);
-          st_rows++;
-        }
-      }
-      ws.q[u * 32 + lane] = q;
+      sp[u] = make_float4(__shfl_sync(0xffffffffu, pt.x, u), __shfl_sync(0xffffffffu, pt.y, u),
+                          __shfl_sync(0xffffffffu, pt.z, u), 0.0f);
+      has |= static_cast<uint32_t>(live && j0 + u < s1) << u;
     }
+    int c[kNfU];
+    uint32_t s[kNfU];
+    const int tot = nf_phase_a(ws, g, rn, pos, sp, has, c, s);
+    st_rows += __popc(has);  // one directory entry per eval with a query
     if (MCL3DL_PM_CUT == 3)
     {
 #pragma unroll
