@@ -276,6 +276,49 @@ void mcl3dl_beam_params_from_reference(mcl3dl_beam_params* out,
 
 int mcl3dl_get_map_info(const mcl3dl_engine*, mcl3dl_map_info* out);
 
+/* ---- Map window: large maps.
+ * mcl3dl_set_map, mcl3dl_map_load and mcl3dl_map_append / mcl3dl_map_update_commit lay the likelihood search grid over
+ * the whole map when its lattice fits: fewer than 2^31 cells, and no more than MCL3DL_MAP_MAX_CELLS (environment, read at
+ * mcl3dl_create; default 2^31 - 1, a smaller value forces windows on small maps).  Otherwise the map is staged WINDOWED
+ * instead of refused: its points and bounding boxes stay on every device and the search structures (CSR grid, near
+ * fields, NN field, KD caster's near field) are built over the points inside a window, a box of raw map space around the
+ * particles.  The DDA caster's grid stays whole-map as before (and is refused beyond its own int point_total limit).
+ *   Rule: every call that reads the map (mcl3dl_measure, mcl3dl_measure_update, mcl3dl_beam_status, mcl3dl_beam_cast,
+ *   mcl3dl_match_output, mcl3dl_particles_measure_update / _prepared) first reduces its inputs on the device to the box
+ *   its searches need: the finite particle positions grown by the largest norm of a finite scan point or origin (times
+ *   the particles' largest |q|^2), the searches' radii per axis in raw coordinates (likelihood rpad, the KD caster's
+ *   second radius and its march, the match output's radius) and a relative pad for the float transform.  When that box
+ *   is not inside the window, the window is rebuilt as the box grown by the scan reach on each side (less when that
+ *   exceeds the cap).  One 32-byte copy back and one synchronise per device and call, on a windowed map only (a
+ *   multi-device call enqueues every device's check with its inputs, then reads them; MCL3DL_TIMING's h2d_ms leaves
+ *   them out); a whole-staged map
+ *   runs exactly as before.  Each search returns the exact nearest neighbour within its radius, so the records are
+ *   those of a whole staging.  Non-finite particles and points are left out of the box (they find nothing either way).
+ *   Appends add to the device point list and rebuild the window (at the next call) only when an appended point lies
+ *   inside it; an append that takes a whole-staged map over the lattice makes it windowed.  mcl3dl_map_get returns the
+ *   whole map; mcl3dl_get_map_info reports the staged window's lattice (zero dimensions before the first window).
+ *   Refused with MCL3DL_ERR_TOO_LARGE on a windowed map, as the whole map was before:
+ *     - a call whose required box alone exceeds the cap (e.g. particles spread over the map): the window and the
+ *       resident particle set stay as they were;
+ *     - mcl3dl_measure_device and mcl3dl_measure_exchange_device (they run on the caller's stream or in a captured
+ *       graph, where no synchronise may happen);
+ *     - field mode (mcl3dl_field_mode, _field_nodes, _field_upload, and set_map in field mode): the volume is whole-map;
+ *     - mcl3dl_global_localization: its seeds cover the whole map. */
+typedef struct
+{
+  int32_t windowed;   /* 1: the staged map is windowed */
+  int32_t staged;     /* 1: a window's structures are built */
+  float box_min[3];   /* the window, raw map space */
+  float box_max[3];
+  int32_t dims[3];    /* its likelihood lattice, cells per axis */
+  int32_t _pad;
+  uint64_t rebuilds;  /* windows built since the map was staged (device 0) */
+  double rebuild_ms;  /* stream time of the last one: the point selection plus the build, event to event; like
+                         mcl3dl_map_info.build_ms it includes the build's own count readbacks, not the allocations
+                         between the two */
+} mcl3dl_window_info;
+int mcl3dl_map_window_info(const mcl3dl_engine*, mcl3dl_window_info* out);
+
 /* ---- Resident particle set (SURVEY.md §8 row f3; the per-particle arithmetic is verified on the host bit for bit
  * against the oracle, the kernels by tests/test_gpu_resident.py on an H100).
  * The particles of pf::ParticleFilter<State6DOF> stay in device memory between updates, so an update moves only the

@@ -15,7 +15,7 @@ SOURCES = [os.path.join(CSRC, "engine.cu")]
 DEPS = SOURCES + [os.path.join(CSRC, "kernels.cuh"), os.path.join(CSRC, "device_funcs.cuh"),
                   os.path.join(CSRC, "device_math.cuh"), os.path.join(CSRC, "pf_kernels.cuh"), os.path.join(CSRC, "pf_funcs.cuh"),
                   os.path.join(CSRC, "scan_kernels.cuh"), os.path.join(CSRC, "scan_funcs.cuh"), os.path.join(CSRC, "match_funcs.cuh"),
-                  os.path.join(CSRC, "accum_funcs.cuh"),
+                  os.path.join(CSRC, "accum_funcs.cuh"), os.path.join(CSRC, "window_funcs.cuh"),
                   os.path.join(os.path.dirname(HERE), "include", "mcl3dl_b200.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-fmad=false", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]

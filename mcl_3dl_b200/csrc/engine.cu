@@ -25,6 +25,7 @@
 #include "match_funcs.cuh"
 #include "pf_kernels.cuh"
 #include "scan_kernels.cuh"
+#include "window_funcs.cuh"
 
 using namespace mcl3dl;
 
@@ -117,6 +118,119 @@ __global__ void nn_gather_kernel(const mcl3dl_point* __restrict__ pts, uint32_t 
   const uint32_t i = order[k];
   const float4 p = __ldg(reinterpret_cast<const float4*>(pts) + i);
   out[k] = make_float4(fmul(p.x, wx), fmul(p.y, wy), fmul(p.z, wz), __uint_as_float(i));
+}
+
+// ---- map window (window_funcs.cuh)
+// What one call's queries need, folded into a zeroed WinNeed: the box of the finite particle positions, max(1, |q|^2) of
+// their quaternions, the largest norm of a finite point of the two scans and of an origin.  Non-finite particles, points
+// and origins are left out: their searches find nothing in any staging.
+__global__ void window_need_kernel(const mcl3dl_pose* __restrict__ poses, uint32_t P, const mcl3dl_point* __restrict__ a,
+                                   uint32_t na, const mcl3dl_point* __restrict__ b, uint32_t nb, const float* __restrict__ org,
+                                   uint32_t norg, uint32_t* __restrict__ need)
+{
+  uint32_t w[8] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
+  const size_t total = static_cast<size_t>(P) + na + nb + norg;
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total; i += static_cast<size_t>(gridDim.x) * blockDim.x)
+  {
+    if (i < P)
+    {
+      const mcl3dl_pose p = poses[i];
+      if (isfinite(p.px) && isfinite(p.py) && isfinite(p.pz) && isfinite(p.qx) && isfinite(p.qy) && isfinite(p.qz) && isfinite(p.qw))
+      {
+        const float v[3] = {p.px, p.py, p.pz};
+#pragma unroll
+        for (int k = 0; k < 3; ++k)
+        {
+          w[k] = max(w[k], ~f2ord(v[k]));
+          w[3 + k] = max(w[3 + k], f2ord(v[k]));
+        }
+        const double q2 = static_cast<double>(p.qx) * p.qx + static_cast<double>(p.qy) * p.qy + static_cast<double>(p.qz) * p.qz +
+                          static_cast<double>(p.qw) * p.qw;
+        w[7] = max(w[7], __float_as_uint(__double2float_ru(fmax(q2, 1.0))));
+      }
+      continue;
+    }
+    size_t j = i - P;
+    float x, y, z;
+    if (j < na)
+    {
+      x = a[j].x;
+      y = a[j].y;
+      z = a[j].z;
+    }
+    else if ((j -= na) < nb)
+    {
+      x = b[j].x;
+      y = b[j].y;
+      z = b[j].z;
+    }
+    else
+    {
+      j -= nb;
+      x = org[3 * j];
+      y = org[3 * j + 1];
+      z = org[3 * j + 2];
+    }
+    if (isfinite(x) && isfinite(y) && isfinite(z))
+    {
+      const double n2 = static_cast<double>(x) * x + static_cast<double>(y) * y + static_cast<double>(z) * z;
+      w[6] = max(w[6], __float_as_uint(__double2float_ru(__dsqrt_ru(n2) * (1.0 + 0x1p-40))));
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < 8; ++k)
+  {
+    const uint32_t m = __reduce_max_sync(0xffffffffu, w[k]);
+    if ((threadIdx.x & 31) == 0 && m)
+      atomicMax(need + k, m);
+  }
+}
+
+// 1 for the map points inside the window box (the scan position of each comes from an exclusive sum)
+__global__ void window_flag_kernel(const mcl3dl_point* __restrict__ pts, uint32_t n, WinBox box, uint32_t* __restrict__ flags)
+{
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n)
+    return;
+  const mcl3dl_point p = pts[i];
+  flags[i] = win_point_inside(box, p.x, p.y, p.z) ? 1u : 0u;
+}
+
+// Appended points inside the window box (an append to a windowed map rebuilds the window only then)
+__global__ void window_count_kernel(const mcl3dl_point* __restrict__ pts, uint32_t n, WinBox box, uint32_t* __restrict__ count)
+{
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n)
+    return;
+  const mcl3dl_point p = pts[i];
+  if (win_point_inside(box, p.x, p.y, p.z))
+    atomicAdd(count, 1u);
+}
+
+// The flagged points in map order and their original indices; n_out = their count
+__global__ void window_compact_kernel(const mcl3dl_point* __restrict__ pts, const uint32_t* __restrict__ flags,
+                                      const uint32_t* __restrict__ pos, uint32_t n, mcl3dl_point* __restrict__ out,
+                                      uint32_t* __restrict__ idx, uint32_t* __restrict__ n_out)
+{
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n)
+    return;
+  if (i == n - 1)
+    *n_out = pos[i] + flags[i];
+  if (flags[i])
+  {
+    out[pos[i]] = pts[i];
+    idx[pos[i]] = i;
+  }
+}
+
+// The window's CSR points carry their index into the window's point list: make it the map index (raw_pts)
+__global__ void window_reindex_kernel(float4* __restrict__ pts, uint32_t n, const uint32_t* __restrict__ idx)
+{
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n)
+    return;
+  pts[k].w = __uint_as_float(__ldg(idx + __float_as_uint(pts[k].w)));
 }
 
 // Window table of the likelihood grid (NnGridDev::row3), from the finished CSR.
@@ -440,7 +554,7 @@ struct DeviceCtx
     for (cudaEvent_t e : ev)
       if (e)
         cudaEventDestroy(e);
-    for (cudaEvent_t e : {ev_fork, ev_join, ev_b0, ev_b1})
+    for (cudaEvent_t e : {ev_fork, ev_join, ev_b0, ev_b1, ev_w0, ev_w1})
       if (e)
         cudaEventDestroy(e);
     for (cudaStream_t s : {side, stream})
@@ -479,6 +593,23 @@ struct DeviceCtx
   bool fld_nodes_valid = false;
   float near_kd_r = 0.0f;            // radius the KD field was built for
   size_t map_bytes = 0;
+  size_t map_base = 0;  // the part of map_bytes a window rebuild keeps (raw points, DDA grid)
+  // map window (window_funcs.cuh), when the whole map's likelihood lattice is refused: w_on = the map is staged windowed;
+  // w_valid = the search structures hold the points inside w_box; w_stale = an append put points inside it since.  The
+  // window's points in map order and their map indices, the reduction's block and its page-locked copy, the lattice,
+  // the bytes of the window's structures, the rebuild count and the last rebuild's stream time (ev_w0 / ev_w1 around
+  // the selection, then around the compaction and build).
+  bool w_on = false, w_valid = false, w_stale = false;
+  bool w_pending = false;  // window_need enqueued a reduction that window_settle has not read yet
+  WinBox w_box{};
+  int32_t w_dims[3] = {0, 0, 0};
+  float w_org[3] = {0.0f, 0.0f, 0.0f};
+  DevBuf w_pts, w_idx, w_need;
+  PinnedBuf w_host;
+  size_t w_bytes = 0;
+  uint64_t w_rebuilds = 0;
+  double w_ms = 0.0;
+  cudaEvent_t ev_w0 = nullptr, ev_w1 = nullptr;
   // per-update I/O
   DevBuf d_poses /* whole input block of the host path */, d_out, d_status;
   PinnedBuf h_pinned;
@@ -584,6 +715,8 @@ struct mcl3dl_engine
   int nnf_kd_r2 = 1;  // MCL3DL_NNF_KD_R2=0: the NN field also covers the KD-tree raycaster's second search radius
   int nnf = 1;  // stage the NN field (exact per-voxel candidate lists) and use lik_kernel_nf*; MCL3DL_NNF=0: lik_kernel_wi
   size_t nnf_max_bytes = size_t(32) << 30;  // MCL3DL_NNF_MAX_MB: directory + candidates above this -> no field
+  // MCL3DL_MAP_MAX_CELLS: a map whose likelihood lattice has more cells is staged windowed, and no window may exceed it
+  size_t map_max_cells = (size_t(1) << 31) - 1;
   uint64_t nnf_bytes = 0, nnf_cands = 0, nnf_overflow_cells = 0, nnf_wide_cells = 0;
   // page-locked blocks handed to the caller by mcl3dl_host_alloc: pose / record arrays that live in one of them are
   // DMA-ed (or, small updates, written by the kernels) in place instead of going through the engine's staging block
@@ -1382,6 +1515,113 @@ int build_nn_csr(mcl3dl_engine* eng, cudaStream_t st, const mcl3dl_point* pts, u
   return MCL3DL_OK;
 }
 
+// Cell edge of the likelihood search grid.  The window (q -/+ rpad) must span at most 3 cells per axis: cell edge
+// strictly above rpad (1 % margin: the float cell function can be off by ~1e-7 x cells-per-axis, and the kernels rely on
+// <= 3).
+float lik_cell(const mcl3dl_engine* eng)
+{
+  return std::max(eng->lik.match_dist_min * eng->nn_cell_factor, eng->likdev.rpad * 1.01f);
+}
+
+// The likelihood search grid over pts[0..n) in lattice g (weights, dimensions and origin set; `cells` cells of edge
+// `cell`) over the rescaled box [sc_min, sc_max]: its CSR, near field, NN field or window table, and the KD-tree
+// raycaster's near field.  pts is the whole map, or the points of a map window: then idx gives each one's map index,
+// which the gathered float4.w must carry (the KD caster's colliding point and the match output read raw_pts by it), and
+// n may be 0.  keys / vals: two arrays of n each; tmp: cub scratch; n_before, first, reselected and incremental are
+// build_map_on_device's.  The bytes staged are added to c.map_bytes.
+int build_search(mcl3dl_engine* eng, DeviceCtx& c, cudaStream_t st, const mcl3dl_point* pts, uint32_t n32, size_t n_before,
+                 uint32_t first, const float sc_min[3], const float sc_max[3], NnGridDev g, size_t cells, float cell,
+                 uint32_t* const keys[2], uint32_t* const vals[2], DevBuf& d_tmp, const uint32_t* idx, uint64_t& reselected,
+                 bool& incremental)
+{
+  int rc = MCL3DL_OK;
+  const size_t n = n32;
+  const float wx = g.wx, wy = g.wy, wz = g.wz;
+  if ((rc = reserve(eng, c.nn_cell_start, (cells + 1) * 4)) || (rc = reserve(eng, c.nn_pts, std::max<size_t>(n, 1) * 16)))
+    return rc;
+  uint32_t* cell_start = static_cast<uint32_t*>(c.nn_cell_start.p);
+  if (n32 == 0)
+    CK(cudaMemsetAsync(cell_start, 0, (cells + 1) * 4, st));
+  else if ((rc = build_nn_csr(eng, st, pts, n32, g, cells, keys, vals, d_tmp, cell_start, static_cast<float4*>(c.nn_pts.p))))
+    return rc;
+  if (idx && n32)
+    CK(launch(eng, window_reindex_kernel, (n32 + 255) / 256, 256, 0, st, static_cast<float4*>(c.nn_pts.p), n32, idx));
+  g.cell_start = cell_start;
+  g.pts = static_cast<const float4*>(c.nn_pts.p);
+#if MCL3DL_NEAR_BITS
+  if (n32 && (rc = build_near_field(eng, c, st, pts, n32, first, wx, wy, wz, eng->likdev.rpad, eng->near_k, sc_min, sc_max, c.near_lik,
+                                    g.near, 0)))
+    return rc;
+#endif
+  // NN field: exact for the likelihood radius and, with the KD-tree raycaster, for its marching radius as well
+  {
+    float radius = eng->likdev.rpad;
+    if (eng->has_beam && !eng->beam.use_raycast_using_dda)
+    {
+      KdRayDev tmp{};
+      fill_kd_scalars(eng->beam, tmp);
+      // the marching search always; the second (sin_angle_) search as well when asked for — it runs once per colliding
+      // ray, through the CSR window search otherwise (a wider field means longer candidate lists for every query)
+      radius = std::max(radius, eng->nnf_kd_r2 ? tmp.r2_pad : tmp.r1_pad);
+    }
+    g.field = NnFieldDev{};
+    bool done = false;
+    // (the field's radius follows the beam params, which set_params may have changed since the field was built)
+    if (incremental && eng->nnf && radius == c.nn.field.radius &&
+        (rc = update_nn_field(eng, c, st, pts, static_cast<uint32_t>(n_before), n32, g, sc_min, sc_max, done, reselected)))
+      return rc;
+    if (!done)
+    {
+      incremental = false;
+      if (n_before > 0 || idx)
+        c.nnf_cand = DevBuf();  // the rebuild compacts: no dead lists, no room kept from earlier appends
+      if (n32 && eng->nnf && (rc = build_nn_field(eng, c, st, pts, n32, g, radius, sc_min, sc_max)))
+        return rc;
+      if (g.field.dir)
+        reselected = static_cast<uint64_t>(g.field.cnx) * g.field.cny * g.field.cnz;
+    }
+  }
+  // window table of the CSR-window kernel (lik_kernel_wi): only when the field is not staged
+  size_t row3_total = 0;
+  g.nyp = (g.ny + 4) & ~1;  // even pitch with room for the 4-entry fetch starting at (ly & ~1)
+  if (!g.field.dir)
+  {
+    row3_total = static_cast<size_t>(g.nz) * g.nx * g.nyp;
+    if ((rc = reserve(eng, c.nn_row3, (row3_total + 2) * sizeof(uint2))))
+      return rc;
+    g.row3 = static_cast<const uint2*>(c.nn_row3.p);
+    CK(launch(eng, nn_row3_kernel, static_cast<unsigned>((row3_total + 255) / 256), 256, 0, st, g, static_cast<uint2*>(c.nn_row3.p),
+              row3_total));
+  }
+  else
+  {
+    c.nn_row3 = DevBuf();
+    g.row3 = nullptr;
+  }
+  c.nn = g;
+  c.map_bytes += (cells + 1) * 4 + n * 16 + row3_total * sizeof(uint2);
+  eng->info.nn_dims[0] = g.nx;
+  eng->info.nn_dims[1] = g.ny;
+  eng->info.nn_dims[2] = g.nz;
+  eng->info.nn_cell = cell;
+  eng->info.nn_origin[0] = g.ox;
+  eng->info.nn_origin[1] = g.oy;
+  eng->info.nn_origin[2] = g.oz;
+  // the KD-tree raycaster's near field (its scalars are set)
+  if (eng->has_beam && !eng->beam.use_raycast_using_dda)
+  {
+#if MCL3DL_NEAR_BITS
+    // (set_params may have widened the marching radius since the field was built: then it is built anew)
+    c.kd.near = NearBitsDev{};
+    if (n32 && (rc = build_near_field(eng, c, st, pts, n32, c.near_kd_r == c.kd.r1_pad ? first : 0u, wx, wy, wz, c.kd.r1_pad,
+                                      eng->near_kd_k, sc_min, sc_max, c.near_kd, c.kd.near, 1)))
+      return rc;
+    c.near_kd_r = c.kd.r1_pad;
+#endif
+  }
+  return MCL3DL_OK;
+}
+
 int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, DevBuf& d_pts, size_t n, size_t n_before, uint64_t& reselected,
                         bool& incremental)
 {
@@ -1430,92 +1670,90 @@ int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, DevBuf& d_pts, size_t 
   const uint32_t first = incremental ? static_cast<uint32_t>(n_before) : 0u;  // near fields: bits of points [first, n)
   reselected = 0;
   c.map_bytes = 0;
+  if (eng->has_beam && !eng->beam.use_raycast_using_dda)
+    fill_kd_scalars(eng->beam, c.kd);
 
-  // ---- likelihood search grid
+  // ---- likelihood search grid over the whole map, or, when its lattice is refused or exceeds MCL3DL_MAP_MAX_CELLS, a
+  // windowed staging: the points and boxes are kept and the search structures wait for the first call's window
+  const bool was_windowed = c.w_on;
+  c.w_on = false;
+  size_t search_bytes = 0;
   if (eng->has_lik)
   {
     NnGridDev g{};
-    // the window (q -/+ rpad) must span at most 3 cells per axis: cell edge strictly above rpad
-    // (1 % margin: the float cell function can be off by ~1e-7 x cells-per-axis, and the kernels rely on <= 3)
-    const float cell = std::max(eng->lik.match_dist_min * eng->nn_cell_factor, eng->likdev.rpad * 1.01f);
+    const float cell = lik_cell(eng);
     if (!(cell > 0.0f))
       return MCL3DL_ERR_INVALID_ARG;
     g.wx = wx;
     g.wy = wy;
     g.wz = wz;
     size_t cells = 0;
-    if (!nn_lattice(cell, sc_min, sc_max, g, cells))
-      return MCL3DL_ERR_TOO_LARGE;
-    if ((rc = reserve(eng, c.nn_cell_start, (cells + 1) * 4)) || (rc = reserve(eng, c.nn_pts, n * 16)))
+    if (!nn_lattice(cell, sc_min, sc_max, g, cells) || cells > eng->map_max_cells)
+      c.w_on = true;
+    else if ((rc = build_search(eng, c, st, pts, n32, n_before, first, sc_min, sc_max, g, cells, cell, keys, vals, d_tmp, nullptr,
+                                reselected, incremental)))
       return rc;
-    uint32_t* cell_start = static_cast<uint32_t*>(c.nn_cell_start.p);
-    if ((rc = build_nn_csr(eng, st, pts, n32, g, cells, keys, vals, d_tmp, cell_start, static_cast<float4*>(c.nn_pts.p))))
-      return rc;
-    g.cell_start = cell_start;
-    g.pts = static_cast<const float4*>(c.nn_pts.p);
-#if MCL3DL_NEAR_BITS
-    if ((rc = build_near_field(eng, c, st, pts, n32, first, wx, wy, wz, eng->likdev.rpad, eng->near_k, sc_min, sc_max, c.near_lik,
-                               g.near, 0)))
-      return rc;
-#endif
-    // NN field: exact for the likelihood radius and, with the KD-tree raycaster, for its marching radius as well
+    search_bytes = c.map_bytes;
+  }
+  if (c.w_on)
+  {
+    incremental = false;
+    if (!was_windowed || !c.w_valid || n_before == 0)
     {
-      float radius = eng->likdev.rpad;
-      if (eng->has_beam && !eng->beam.use_raycast_using_dda)
+      // a new map, or nothing staged yet: the first call that reads the map builds its window (a window of an earlier
+      // map indexes that map's points and was laid out for its parameters)
+      c.w_valid = false;
+      c.w_stale = false;
+      c.w_box = WinBox{};
+      if (n_before == 0)
       {
-        KdRayDev tmp{};
-        fill_kd_scalars(eng->beam, tmp);
-        // the marching search always; the second (sin_angle_) search as well when asked for — it runs once per colliding
-        // ray, through the CSR window search otherwise (a wider field means longer candidate lists for every query)
-        radius = std::max(radius, eng->nnf_kd_r2 ? tmp.r2_pad : tmp.r1_pad);
+        c.w_rebuilds = 0;
+        c.w_ms = 0.0;
       }
-      g.field = NnFieldDev{};
-      bool done = false;
-      // (the field's radius follows the beam params, which set_params may have changed since the field was built)
-      if (incremental && eng->nnf && radius == c.nn.field.radius &&
-          (rc = update_nn_field(eng, c, st, pts, static_cast<uint32_t>(n_before), n32, g, sc_min, sc_max, done, reselected)))
-        return rc;
-      if (!done)
+      c.nn = NnGridDev{};
+      c.nn_cell_start = DevBuf();
+      c.nn_pts = DevBuf();
+      c.nn_row3 = DevBuf();
+      c.nnf_dir = DevBuf();
+      c.nnf_cand = DevBuf();
+      c.nnf_wide = DevBuf();
+      c.near_lik = DevBuf();
+      c.near_kd = DevBuf();
+      c.kd.near = NearBitsDev{};
+      eng->nnf_bytes = eng->nnf_cands = eng->nnf_overflow_cells = eng->nnf_wide_cells = 0;
+      for (int k = 0; k < 3; ++k)
       {
-        incremental = false;
-        if (n_before > 0)
-          c.nnf_cand = DevBuf();  // the rebuild compacts: no dead lists, no room kept from earlier appends
-        if (eng->nnf && (rc = build_nn_field(eng, c, st, pts, n32, g, radius, sc_min, sc_max)))
-          return rc;
-        if (g.field.dir)
-          reselected = static_cast<uint64_t>(g.field.cnx) * g.field.cny * g.field.cnz;
+        eng->info.nn_dims[k] = 0;
+        eng->info.nn_origin[k] = 0.0f;
       }
-    }
-    // window table of the CSR-window kernel (lik_kernel_wi): only when the field is not staged
-    size_t row3_total = 0;
-    g.nyp = (g.ny + 4) & ~1;  // even pitch with room for the 4-entry fetch starting at (ly & ~1)
-    if (!g.field.dir)
-    {
-      row3_total = static_cast<size_t>(g.nz) * g.nx * g.nyp;
-      if ((rc = reserve(eng, c.nn_row3, (row3_total + 2) * sizeof(uint2))))
-        return rc;
-      g.row3 = static_cast<const uint2*>(c.nn_row3.p);
-      CK(launch(eng, nn_row3_kernel, static_cast<unsigned>((row3_total + 255) / 256), 256, 0, st, g, static_cast<uint2*>(c.nn_row3.p),
-                row3_total));
+      eng->info.nn_cell = lik_cell(eng);
     }
     else
     {
-      c.nn_row3 = DevBuf();
-      g.row3 = nullptr;
+      // an append to a windowed map: the window is rebuilt when an appended point lies inside it
+      DevBuf d_cnt;
+      if ((rc = reserve(eng, d_cnt, 4)) || (rc = reserve(eng, c.w_host, 64)))
+        return rc;
+      uint32_t* cnt = static_cast<uint32_t*>(d_cnt.p);
+      CK(cudaMemsetAsync(cnt, 0, 4, st));
+      const uint32_t n_new = static_cast<uint32_t>(n - n_before);
+      if (n_new)
+        CK(launch(eng, window_count_kernel, (n_new + 255) / 256, 256, 0, st, pts + n_before, n_new, c.w_box, cnt));
+      CK(cudaMemcpyAsync(c.w_host.p, cnt, 4, cudaMemcpyDeviceToHost, st));
+      CK(cudaStreamSynchronize(st));
+      // (stays stale when an earlier append, not yet followed by a call that reads the map, put points inside)
+      c.w_stale = c.w_stale || *static_cast<const uint32_t*>(c.w_host.p) != 0;
+      for (int k = 0; k < 3; ++k)
+      {
+        eng->info.nn_dims[k] = c.w_dims[k];
+        eng->info.nn_origin[k] = c.w_org[k];
+      }
+      eng->info.nn_cell = lik_cell(eng);
     }
-    c.nn = g;
-    c.map_bytes += (cells + 1) * 4 + n * 16 + row3_total * sizeof(uint2);
-    eng->info.nn_dims[0] = g.nx;
-    eng->info.nn_dims[1] = g.ny;
-    eng->info.nn_dims[2] = g.nz;
-    eng->info.nn_cell = cell;
-    eng->info.nn_origin[0] = g.ox;
-    eng->info.nn_origin[1] = g.oy;
-    eng->info.nn_origin[2] = g.oz;
   }
   // ---- the raw points by original index (the KD-tree raycaster's colliding point; the chunk rule of
-  // mcl3dl_match_output; the base of mcl3dl_map_append).  device_bytes counts them where the models read them: with a
-  // likelihood grid.
+  // mcl3dl_match_output; the base of mcl3dl_map_append; a window's point list).  device_bytes counts them where the
+  // models read them: with a likelihood grid.
   c.raw_pts = std::move(d_pts);
   if (eng->has_lik)
     c.map_bytes += n * 16;
@@ -1526,14 +1764,6 @@ int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, DevBuf& d_pts, size_t 
     if (!eng->has_lik)
       return MCL3DL_ERR_INVALID_ARG;
     fill_dda_scalars(eng->beam, c.dda);
-    fill_kd_scalars(eng->beam, c.kd);
-#if MCL3DL_NEAR_BITS
-    // (set_params may have widened the marching radius since the field was built: then it is built anew)
-    if ((rc = build_near_field(eng, c, st, pts, n32, c.near_kd_r == c.kd.r1_pad ? first : 0u, wx, wy, wz, c.kd.r1_pad,
-                               eng->near_kd_k, sc_min, sc_max, c.near_kd, c.kd.near, 1)))
-      return rc;
-    c.near_kd_r = c.kd.r1_pad;
-#endif
     c.kd.raw_pts = static_cast<const float4*>(c.raw_pts.p);
   }
   // ---- DDA grid: updatePointCloud, raycast_using_dda.h:162-190
@@ -1592,8 +1822,206 @@ int build_map_on_device(mcl3dl_engine* eng, DeviceCtx& c, DevBuf& d_pts, size_t 
   float ms = 0;
   CK(cudaEventElapsedTime(&ms, e0, e1));
   eng->info.build_ms = std::max(eng->info.build_ms, static_cast<double>(ms));
+  c.map_base = c.map_bytes - search_bytes;  // what a window rebuild keeps: the raw points and the DDA grid
+  if (c.w_on && c.w_valid)
+    c.map_bytes += c.w_bytes;
   eng->info.device_bytes = c.map_bytes;
   return MCL3DL_OK;
+}
+
+// ---- map window (window_funcs.cuh)
+// Stage the search structures over the map points inside box `b` (raw space): the points are selected in map order, the
+// grids are built over them exactly as over a whole map, with the lattice laid over the box, and each gathered point
+// keeps its map index.  Points outside the box never enter a cell.
+int build_window(mcl3dl_engine* eng, DeviceCtx& c, const WinBox& b)
+{
+  cudaStream_t st = c.stream;
+  const size_t n = eng->n_points;
+  const uint32_t n32 = static_cast<uint32_t>(n);
+  const float w[3] = {eng->lik.dist_weight[0], eng->lik.dist_weight[1], eng->lik.dist_weight[2]};
+  const float cell = lik_cell(eng);
+  NnGridDev g{};
+  float org[3];
+  int dims[3];
+  size_t cells = 0;
+  if (!win_box_lattice(b, w, cell, dims, org, cells) || cells > eng->map_max_cells)
+    return MCL3DL_ERR_TOO_LARGE;
+  g.wx = w[0];
+  g.wy = w[1];
+  g.wz = w[2];
+  g.inv_cell = 1.0f / cell;
+  g.nx = dims[0];
+  g.ny = dims[1];
+  g.nz = dims[2];
+  g.ox = org[0];
+  g.oy = org[1];
+  g.oz = org[2];
+  DevBuf d_flags, d_pos, d_cnt, d_keys[2], d_vals[2], d_tmp;
+  int rc;
+  if ((rc = reserve(eng, d_flags, n * 4)) || (rc = reserve(eng, d_pos, n * 4)) || (rc = reserve(eng, d_cnt, 4)) ||
+      (rc = reserve(eng, c.w_host, 64)))
+    return rc;
+  // the selection's flags and scan positions first: the window's point list is sized by their count
+  CK(cudaEventRecord(c.ev_w0, st));
+  const mcl3dl_point* raw = static_cast<const mcl3dl_point*>(c.raw_pts.p);
+  uint32_t* flags = static_cast<uint32_t*>(d_flags.p);
+  uint32_t* pos = static_cast<uint32_t*>(d_pos.p);
+  uint32_t* cnt = static_cast<uint32_t*>(d_cnt.p);
+  const int nb = static_cast<int>((n + 255) / 256);
+  CK(launch(eng, window_flag_kernel, nb, 256, 0, st, raw, n32, b, flags));
+  CK(cub_call(eng, d_tmp, [&](void* t, size_t& bytes) { return cub::DeviceScan::ExclusiveSum(t, bytes, flags, pos, n32, st); }));
+  CK(cudaEventRecord(c.ev_w1, st));
+  uint32_t* h = static_cast<uint32_t*>(c.w_host.p);
+  CK(cudaMemcpyAsync(h, pos + (n32 - 1), 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(h + 1, flags + (n32 - 1), 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  float ms_select = 0;
+  CK(cudaEventElapsedTime(&ms_select, c.ev_w0, c.ev_w1));
+  const uint32_t m = h[0] + h[1];
+  const size_t mk = std::max<uint32_t>(m, 1u);
+  // the point list and map indices at the window's size (a much smaller window gives the larger buffers back)
+  if (c.w_pts.cap > 2 * mk * 16)
+    c.w_pts = DevBuf();
+  if (c.w_idx.cap > 2 * mk * 4)
+    c.w_idx = DevBuf();
+  if ((rc = reserve(eng, c.w_pts, mk * 16)) || (rc = reserve(eng, c.w_idx, mk * 4)) || (rc = reserve(eng, d_keys[0], mk * 4)) ||
+      (rc = reserve(eng, d_keys[1], mk * 4)) || (rc = reserve(eng, d_vals[0], mk * 4)) || (rc = reserve(eng, d_vals[1], mk * 4)))
+    return rc;
+  CK(cudaEventRecord(c.ev_w0, st));
+  CK(launch(eng, window_compact_kernel, nb, 256, 0, st, raw, flags, pos, n32, static_cast<mcl3dl_point*>(c.w_pts.p),
+            static_cast<uint32_t*>(c.w_idx.p), cnt));
+  uint32_t* const keys[2] = {static_cast<uint32_t*>(d_keys[0].p), static_cast<uint32_t*>(d_keys[1].p)};
+  uint32_t* const vals[2] = {static_cast<uint32_t*>(d_vals[0].p), static_cast<uint32_t*>(d_vals[1].p)};
+  float sc_min[3], sc_max[3];
+  for (int k = 0; k < 3; ++k)
+  {
+    sc_min[k] = b.lo[k] * w[k];
+    sc_max[k] = b.hi[k] * w[k];
+  }
+  c.w_valid = false;
+  c.map_bytes = 0;
+  uint64_t reselected = 0;
+  bool incremental = false;
+  if ((rc = build_search(eng, c, st, static_cast<const mcl3dl_point*>(c.w_pts.p), m, 0, 0u, sc_min, sc_max, g, cells, cell, keys, vals,
+                         d_tmp, static_cast<const uint32_t*>(c.w_idx.p), reselected, incremental)))
+    return rc;
+  CK(cudaEventRecord(c.ev_w1, st));
+  CK(cudaStreamSynchronize(st));
+  float ms = 0;
+  CK(cudaEventElapsedTime(&ms, c.ev_w0, c.ev_w1));
+  c.w_bytes = c.map_bytes + mk * 20;  // + the window's point list and map indices
+  c.map_bytes = c.map_base + c.w_bytes;
+  eng->info.device_bytes = c.map_bytes;
+  c.w_box = b;
+  for (int k = 0; k < 3; ++k)
+  {
+    c.w_dims[k] = dims[k];
+    c.w_org[k] = org[k];
+  }
+  c.w_valid = true;
+  c.w_stale = false;
+  c.w_rebuilds++;
+  c.w_ms = static_cast<double>(ms_select) + ms;
+  return MCL3DL_OK;
+}
+
+// The window check of one call that reads the map, on a windowed map, in two steps so that a multi-device call enqueues
+// every device's reduction before it waits for any.  window_need enqueues on c.stream the reduction of the particles
+// [poses, +P) with the scans and origins given (device pointers) and its 32-byte copy back; window_settle synchronises,
+// forms the required box for the search `s` and rebuilds the window when the box is not inside it.  TOO_LARGE: the
+// required box alone exceeds the cap (or is not finite); the staged window is left as it was.  A whole-staged map
+// returns at once from both.
+int window_need(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_pose* poses, size_t P, const mcl3dl_point* a, size_t na,
+                const mcl3dl_point* b, size_t nb, const float* org, size_t norg, const WinSearch& s,
+                const mcl3dl_pose* host_pose = nullptr)
+{
+  c.w_pending = false;
+  if (!c.w_on || (c.w_valid && !c.w_stale && !(s.r_scaled > 0.0f)))
+    return MCL3DL_OK;  // (no search of this call reads the window: DDA beam only)
+  cudaStream_t st = c.stream;
+  int rc;
+  if ((rc = reserve(eng, c.w_need, 64)) || (rc = reserve(eng, c.w_host, 64)))
+    return rc;
+  CK(cudaMemsetAsync(c.w_need.p, 0, sizeof(WinNeed), st));
+  if (host_pose)  // one pose from the host: behind the reduction's block
+  {
+    static_assert(sizeof(WinNeed) + sizeof(mcl3dl_pose) <= 64, "pose slot");
+    std::memcpy(static_cast<char*>(c.w_host.p) + sizeof(WinNeed), host_pose, sizeof(mcl3dl_pose));
+    CK(cudaMemcpyAsync(static_cast<char*>(c.w_need.p) + sizeof(WinNeed), static_cast<char*>(c.w_host.p) + sizeof(WinNeed),
+                       sizeof(mcl3dl_pose), cudaMemcpyHostToDevice, st));
+    poses = reinterpret_cast<const mcl3dl_pose*>(static_cast<char*>(c.w_need.p) + sizeof(WinNeed));
+    P = 1;
+  }
+  const size_t total = P + na + nb + norg;
+  const int grid = static_cast<int>(std::max<size_t>(1, std::min<size_t>((total + 255) / 256, static_cast<size_t>(c.sm_count) * 8)));
+  CK(launch(eng, window_need_kernel, grid, 256, 0, st, poses, static_cast<uint32_t>(P), a, static_cast<uint32_t>(na), b,
+            static_cast<uint32_t>(nb), org, static_cast<uint32_t>(norg), static_cast<uint32_t*>(c.w_need.p)));
+  CK(cudaMemcpyAsync(c.w_host.p, c.w_need.p, sizeof(WinNeed), cudaMemcpyDeviceToHost, st));
+  c.w_pending = true;
+  return MCL3DL_OK;
+}
+
+int window_settle(mcl3dl_engine* eng, DeviceCtx& c, const WinSearch& s)
+{
+  if (!c.w_pending)
+    return MCL3DL_OK;
+  c.w_pending = false;
+  CK(cudaSetDevice(c.dev));
+  CK(cudaStreamSynchronize(c.stream));
+  WinNeed need;
+  std::memcpy(&need, c.w_host.p, sizeof(need));
+  if (!win_has_particles(need))
+  {
+    // no finite particle: no search can find a point, so any staged window serves; the first one sits at the map's corner
+    if (c.w_valid)
+      return MCL3DL_OK;
+    for (int k = 0; k < 3; ++k)
+    {
+      need.pmax[k] = c.map_box[k];
+      need.pmin_c[k] = ~c.map_box[k];
+    }
+  }
+  const float w[3] = {eng->lik.dist_weight[0], eng->lik.dist_weight[1], eng->lik.dist_weight[2]};
+  WinBox req;
+  if (!win_required(need, s, w, req))
+  {
+    eng->err = "map window: the required box is not finite";
+    return MCL3DL_ERR_TOO_LARGE;
+  }
+  if (c.w_valid && !c.w_stale && win_contains(c.w_box, req))
+    return MCL3DL_OK;
+  WinBox win;
+  if (!win_choose(req, win_reach(need), w, lik_cell(eng), eng->map_max_cells, win))
+  {
+    eng->err = "map window: the particles' required box exceeds the lattice cap";
+    return MCL3DL_ERR_TOO_LARGE;
+  }
+  return build_window(eng, c, win);
+}
+
+// Both steps, for a call on one device
+int ensure_window(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_pose* poses, size_t P, const mcl3dl_point* a, size_t na,
+                  const mcl3dl_point* b, size_t nb, const float* org, size_t norg, const WinSearch& s,
+                  const mcl3dl_pose* host_pose = nullptr)
+{
+  if (int rc = window_need(eng, c, poses, P, a, na, b, nb, org, norg, s, host_pose))
+    return rc;
+  return window_settle(eng, c, s);
+}
+
+// The searches of a measure call: the likelihood radius, and with a beam scan and the KD caster its second radius and march
+WinSearch measure_search(const mcl3dl_engine* eng, const DeviceCtx& c, size_t n_lik, size_t n_beam)
+{
+  WinSearch s{0.0f, 0.0f, 0.0f};
+  if (n_lik)
+    s.r_scaled = eng->likdev.rpad;
+  if (n_beam && !eng->beam.use_raycast_using_dda)
+  {
+    s.r_scaled = std::max(s.r_scaled, std::max(c.kd.r1_pad, c.kd.r2_pad));
+    s.grid_min = c.kd.grid_min;
+    s.hit_tolerance = c.kd.hit_tolerance;
+  }
+  return s;
 }
 
 // After a build: a field-mode volume of the previous map is stale; in field mode the new one is staged.
@@ -1602,6 +2030,8 @@ int restage_field(mcl3dl_engine* eng, DeviceCtx& c)
   c.fld_nodes_valid = false;
   c.fld_mem = DevBuf();
   c.fld_nodes = cudaPitchedPtr{};
+  if (eng->field_mode && eng->has_lik && c.w_on)
+    return MCL3DL_ERR_TOO_LARGE;  // the volume covers the whole map
   return eng->field_mode && eng->has_lik ? stage_field(eng, c, nullptr) : MCL3DL_OK;
 }
 
@@ -1841,6 +2271,8 @@ int mcl3dl_create(mcl3dl_engine** out, const int* device_ids, int n_devices)
     eng->field_max_bytes = static_cast<size_t>(std::max(std::atol(v), 1L)) << 20;
   if (const char* v = std::getenv("MCL3DL_NNF_MAX_MB"))
     eng->nnf_max_bytes = static_cast<size_t>(std::max(std::atol(v), 1L)) << 20;
+  if (const char* v = std::getenv("MCL3DL_MAP_MAX_CELLS"))
+    eng->map_max_cells = std::min(std::max<size_t>(std::strtoull(v, nullptr, 10), 8), (size_t(1) << 31) - 1);
   if (const char* o = std::getenv("MCL3DL_OVERLAP"))
     eng->overlap = std::atoi(o) != 0;
   eng->devs = std::vector<DeviceCtx>(n_devices);  // at its final size: a context never moves
@@ -1875,7 +2307,8 @@ int mcl3dl_create(mcl3dl_engine** out, const int* device_ids, int n_devices)
     if (cudaStreamCreateWithFlags(&c.side, cudaStreamNonBlocking) != cudaSuccess ||
         cudaEventCreateWithFlags(&c.ev_fork, cudaEventDisableTiming) != cudaSuccess ||
         cudaEventCreateWithFlags(&c.ev_join, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreate(&c.ev_b0) != cudaSuccess || cudaEventCreate(&c.ev_b1) != cudaSuccess)
+        cudaEventCreate(&c.ev_b0) != cudaSuccess || cudaEventCreate(&c.ev_b1) != cudaSuccess ||
+        cudaEventCreate(&c.ev_w0) != cudaSuccess || cudaEventCreate(&c.ev_w1) != cudaSuccess)
     {
       mcl3dl_destroy(eng);
       return MCL3DL_ERR_CUDA;
@@ -2354,6 +2787,8 @@ int mcl3dl_field_mode(mcl3dl_engine* eng, int enable)
   {
     if (!eng->has_lik)
       return MCL3DL_ERR_INVALID_ARG;
+    if (eng->devs[0].w_on)
+      return MCL3DL_ERR_TOO_LARGE;
     for (DeviceCtx& c : eng->devs)
       if (!c.fld_nodes_valid)
       {
@@ -2371,6 +2806,8 @@ int mcl3dl_field_nodes(mcl3dl_engine* eng, float* nodes_out, int32_t dims_out[3]
   if (!eng || !eng->has_map || eng->devs.empty())
     return MCL3DL_ERR_NO_MAP;
   DeviceCtx& c = eng->devs[0];
+  if (c.w_on)
+    return MCL3DL_ERR_TOO_LARGE;
   const NnFieldDev& f = c.nn.field;
   if (!f.dir)
     return MCL3DL_ERR_INVALID_ARG;
@@ -2410,6 +2847,8 @@ int mcl3dl_field_upload(mcl3dl_engine* eng, const float* nodes, const int32_t di
     return MCL3DL_ERR_INVALID_ARG;
   if (!eng->has_map || !eng->has_lik)
     return MCL3DL_ERR_NO_MAP;
+  if (eng->devs[0].w_on)
+    return MCL3DL_ERR_TOO_LARGE;
   for (DeviceCtx& c : eng->devs)
   {
     const NnFieldDev& f = c.nn.field;
@@ -2442,6 +2881,27 @@ int mcl3dl_get_map_info(const mcl3dl_engine* eng, mcl3dl_map_info* out)
   if (!eng->has_map)
     return MCL3DL_ERR_NO_MAP;
   *out = eng->info;
+  return MCL3DL_OK;
+}
+
+int mcl3dl_map_window_info(const mcl3dl_engine* eng, mcl3dl_window_info* out)
+{
+  if (!eng || !out)
+    return MCL3DL_ERR_INVALID_ARG;
+  if (!eng->has_map)
+    return MCL3DL_ERR_NO_MAP;
+  const DeviceCtx& c = eng->devs[0];
+  *out = mcl3dl_window_info{};
+  out->windowed = c.w_on ? 1 : 0;
+  out->staged = c.w_on && c.w_valid ? 1 : 0;
+  for (int k = 0; k < 3; ++k)
+  {
+    out->box_min[k] = c.w_box.lo[k];
+    out->box_max[k] = c.w_box.hi[k];
+    out->dims[k] = out->staged ? c.w_dims[k] : 0;
+  }
+  out->rebuilds = c.w_rebuilds;
+  out->rebuild_ms = c.w_ms;
   return MCL3DL_OK;
 }
 
@@ -2651,6 +3111,8 @@ int mcl3dl_measure_device(mcl3dl_engine* eng, const mcl3dl_pose* d_poses, size_t
   if (P == 0)
     return MCL3DL_OK;
   DeviceCtx& c = eng->devs[0];
+  if (c.w_on)
+    return MCL3DL_ERR_TOO_LARGE;  // a window check synchronises: not on the caller's stream
   CK(cudaSetDevice(c.dev));
   cudaStream_t st = static_cast<cudaStream_t>(cuda_stream);
   return launch_models(eng, c, d_poses, P, d_lik, n_lik, d_beam, n_beam, d_origins_xyz, n_origins, d_out, nullptr, st, false);
@@ -3001,6 +3463,8 @@ int mcl3dl_global_localization(mcl3dl_engine* eng, const mcl3dl_point* pts, size
   if (!pts && !eng->has_map)
     return MCL3DL_ERR_NO_MAP;
   DeviceCtx& c = eng->devs[0];
+  if (eng->has_map && c.w_on)
+    return MCL3DL_ERR_TOO_LARGE;  // the seeds cover the whole map: no window holds them
   const size_t cnt = pts ? n : eng->n_points;
   mcl3dl_global_localization_info out{};
   out.n_input = cnt;
@@ -3161,6 +3625,10 @@ static int resident_update(mcl3dl_engine* eng, DeviceCtx& c, const mcl3dl_point*
   const uint32_t n32 = static_cast<uint32_t>(P);
   CK(launch(eng, pf_pack_kernel, (n32 + 255) / 256, 256, 0, st, static_cast<const PfState*>(c.r_states[c.r_cur].p), n32, nd_a, nd_sq2,
             static_cast<mcl3dl_pose*>(c.r_poses.p), with_odom ? static_cast<float*>(c.r_extra.p) : nullptr));
+  // (the pack writes only the packed poses and factors: a refused window leaves the resident set as it was)
+  if ((rc = ensure_window(eng, c, static_cast<const mcl3dl_pose*>(c.r_poses.p), P, d_lik, n_lik, d_beam, n_beam, d_org, n_origins,
+                          measure_search(eng, c, n_lik, n_beam))))
+    return rc;
   mcl3dl_result* d_rec = static_cast<mcl3dl_result*>(c.d_out.p);
   rc = launch_models(eng, c, static_cast<const mcl3dl_pose*>(c.r_poses.p), P, d_lik, n_lik, d_beam, n_beam, d_org, n_origins,
                      d_rec, nullptr, st, false);
@@ -3598,6 +4066,9 @@ int mcl3dl_match_output(mcl3dl_engine* eng, const mcl3dl_pose* pose, const mcl3d
   m.chunk_length = mp->chunk_length;
   m.pos_to_chunk = static_cast<float>(1.0 / static_cast<double>(mp->chunk_length));
   m.max_search_radius = mp->max_search_radius;
+  const WinSearch ms{m.rpad, 0.0f, 0.0f};
+  if ((rc = ensure_window(eng, c, nullptr, 0, src, cnt, nullptr, 0, nullptr, 0, ms, pose)))
+    return rc;
   uint32_t* f[2] = {static_cast<uint32_t*>(c.m_flags[0].p), static_cast<uint32_t*>(c.m_flags[1].p)};
   uint32_t* ps[2] = {static_cast<uint32_t*>(c.m_pos[0].p), static_cast<uint32_t*>(c.m_pos[1].p)};
   mcl3dl_point* tf = static_cast<mcl3dl_point*>(c.m_tf.p);
@@ -3773,6 +4244,8 @@ int mcl3dl_measure_exchange_device(mcl3dl_engine* eng, const mcl3dl_pose* d_pose
   if (eng->devs.size() != 1 || !d_poses)
     return MCL3DL_ERR_INVALID_ARG;
   DeviceCtx& c = eng->devs[0];
+  if (c.w_on)
+    return MCL3DL_ERR_TOO_LARGE;
   if (!c.x_ready || P != c.x_local)
     return MCL3DL_ERR_INVALID_ARG;
   CK(cudaSetDevice(c.dev));
@@ -3846,6 +4319,24 @@ static int measure_host(mcl3dl_engine* eng, const mcl3dl_pose* poses, size_t P, 
     if (poses_direct)
       CK(cudaMemcpyAsync(c.d_poses.p, poses + s.p0, s.o_lik, cudaMemcpyHostToDevice, st));
     if (timed) CK(cudaEventRecord(c.ev[1], st));
+    const char* d_in = static_cast<const char*>(c.d_poses.p);
+    if ((rc = window_need(eng, c, reinterpret_cast<const mcl3dl_pose*>(d_in), s.n, reinterpret_cast<const mcl3dl_point*>(d_in + s.o_lik),
+                          n_lik, reinterpret_cast<const mcl3dl_point*>(d_in + s.o_beam), n_beam,
+                          reinterpret_cast<const float*>(d_in + s.o_org), n_origins, measure_search(eng, c, n_lik, n_beam))))
+      return rc;
+  }
+  // (a windowed map: every device's window check was enqueued above; each is read before that device's models launch)
+  for (size_t d = 0; d < G; ++d)
+  {
+    DeviceCtx& c = eng->devs[d];
+    const Share& s = sh[d];
+    if (s.n == 0)
+      continue;
+    if ((rc = window_settle(eng, c, measure_search(eng, c, n_lik, n_beam))))
+      return rc;
+    CK(cudaSetDevice(c.dev));
+    cudaStream_t st = c.stream;
+    const size_t b_rec = s.n * sizeof(mcl3dl_result), b_status = status ? s.n * n_beam : 0;
     // small updates: the kernels store their records straight into the pinned block (cudaMallocHost memory is mapped
     // into the unified address space), which saves the D2H copy launch; large ones keep the bulk copy
     const bool zc = !status && s.n <= eng->zero_copy_max;  // (per-ray status bytes would be scattered 1-byte PCIe writes)
@@ -3923,6 +4414,23 @@ int mcl3dl_measure_update(mcl3dl_engine* eng, const mcl3dl_pose* poses, size_t P
         (rc = reserve(eng, c.d_out, s.n * sizeof(mcl3dl_result))) || (rc = reserve(eng, c.d_post, s.n * 4)) ||
         (rc = stage_inputs(eng, c, s, poses, lik_pts, beam_pts, origins_xyz, n_origins, prior, extra, false)))
       return rc;
+    const char* d_in = static_cast<const char*>(c.d_poses.p);
+    if ((rc = window_need(eng, c, reinterpret_cast<const mcl3dl_pose*>(d_in), s.n, reinterpret_cast<const mcl3dl_point*>(d_in + s.o_lik),
+                          n_lik, reinterpret_cast<const mcl3dl_point*>(d_in + s.o_beam), n_beam,
+                          reinterpret_cast<const float*>(d_in + s.o_org), n_origins, measure_search(eng, c, n_lik, n_beam))))
+      return rc;
+  }
+  // (a windowed map: every device's window check was enqueued above; each is read before that device's models launch)
+  for (size_t d = 0; d < G; ++d)
+  {
+    DeviceCtx& c = eng->devs[d];
+    const Share& s = sh[d];
+    if (s.n == 0)
+      continue;
+    if ((rc = window_settle(eng, c, measure_search(eng, c, n_lik, n_beam))))
+      return rc;
+    CK(cudaSetDevice(c.dev));
+    cudaStream_t st = c.stream;
     const char* d_in = static_cast<const char*>(c.d_poses.p);
     const float* d_prior = reinterpret_cast<const float*>(d_in + s.o_prior);
     const float* d_extra = extra ? reinterpret_cast<const float*>(d_in + s.o_extra) : nullptr;
@@ -4083,6 +4591,9 @@ int mcl3dl_beam_cast(mcl3dl_engine* eng, const mcl3dl_pose* pose, const mcl3dl_p
     d_scan = reinterpret_cast<const mcl3dl_point*>(dp + o_scan - 64);
   }
   CK(cudaMemcpyAsync(dp, hp + 64, in_end - 64, cudaMemcpyHostToDevice, st));
+  if (kd && (rc = ensure_window(eng, c, reinterpret_cast<const mcl3dl_pose*>(dp), 1, nullptr, 0, d_scan, n,
+                                reinterpret_cast<const float*>(dp + o_org - 64), n_origins, measure_search(eng, c, 0, n))))
+    return rc;
   mcl3dl_beam_ray* h_rec = reinterpret_cast<mcl3dl_beam_ray*>(hp + o_rec);
   const auto kernel = kd ? beam_cast_kernel<true> : beam_cast_kernel<false>;
   CK(launch(eng, kernel, static_cast<unsigned>((n + kBlockThreads - 1) / kBlockThreads), kBlockThreads, 0, st,

@@ -58,6 +58,18 @@ class MapInfo(C.Structure):
                 ("dda_max", C.c_float * 3), ("device_bytes", C.c_uint64), ("build_ms", C.c_double)]
 
 
+class MapWindowInfo(C.Structure):
+    """mcl3dl_window_info (mcl3dl_map_window_info): whether the staged map is windowed, the staged window (raw box, lattice dimensions), the
+    windows built since the map was staged and the stream time of the last one (header: rebuild_ms)."""
+    _fields_ = [("windowed", C.c_int32), ("staged", C.c_int32), ("box_min", C.c_float * 3), ("box_max", C.c_float * 3),
+                ("dims", C.c_int32 * 3), ("_pad", C.c_int32), ("rebuilds", C.c_uint64), ("rebuild_ms", C.c_double)]
+
+    def as_dict(self):
+        return {"windowed": bool(self.windowed), "staged": bool(self.staged), "box_min": tuple(self.box_min),
+                "box_max": tuple(self.box_max), "dims": tuple(self.dims), "rebuilds": int(self.rebuilds),
+                "rebuild_ms": float(self.rebuild_ms)}
+
+
 class MapAppendInfo(C.Structure):
     _fields_ = [("n_before", C.c_uint64), ("n_appended", C.c_uint64), ("n_after", C.c_uint64), ("incremental", C.c_int32),
                 ("cells_reselected", C.c_uint64), ("build_ms", C.c_double)]
@@ -246,7 +258,8 @@ EXPORTED_SYMBOLS = ["mcl3dl_measure_update", "mcl3dl_collect_stats", "mcl3dl_rea
                     "mcl3dl_particles_init", "mcl3dl_scan_sample_with_normal", "mcl3dl_scan_normals", "mcl3dl_beam_cast",
                     "mcl3dl_scan_accumulate", "mcl3dl_scan_accumulate_clear", "mcl3dl_scan_accumulated_get",
                     "mcl3dl_scan_prepare_accumulated", "mcl3dl_map_load", "mcl3dl_map_update_set",
-                    "mcl3dl_map_update_commit", "mcl3dl_map_update_clear", "mcl3dl_map_get"]
+                    "mcl3dl_map_update_commit", "mcl3dl_map_update_clear", "mcl3dl_map_get",
+                    "mcl3dl_map_window_info"]
 
 _LIBS = {}
 
@@ -280,6 +293,7 @@ def load_library(path=None):
                                                     C.c_uint32, C.c_float, C.c_int, C.c_int, C.c_float, C.c_float]
     L.mcl3dl_beam_params_from_reference.restype = None
     L.mcl3dl_get_map_info.argtypes = [vp, vp]
+    L.mcl3dl_map_window_info.argtypes = [vp, vp]
     L.mcl3dl_collect_stats.argtypes = [vp, C.c_int]
     L.mcl3dl_read_stats.argtypes = [vp, vp]
     L.mcl3dl_last_timing.argtypes = [vp] + [C.POINTER(C.c_double)] * 4
@@ -414,6 +428,13 @@ class Engine:
         mi = MapInfo()
         self._check(self.L.mcl3dl_get_map_info(self.h, C.byref(mi)))
         return mi
+
+    def map_window_info(self):
+        """The map window (include/mcl3dl_b200.h, "Map window"): {"windowed", "staged", "box_min", "box_max", "dims",
+        "rebuilds", "rebuild_ms"}."""
+        wi = MapWindowInfo()
+        self._check(self.L.mcl3dl_map_window_info(self.h, C.byref(wi)))
+        return wi.as_dict()
 
     def near_field_info(self):
         """[(k, bytes)] of the near-field screens of the staged map: [0] likelihood search, [1] KD-tree raycaster."""
